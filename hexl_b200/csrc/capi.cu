@@ -728,6 +728,17 @@ int ntt_multi_on_device(bool forward, int dev, hexl_b200_ntt* const* handles, ui
                         const std::vector<uint64_t*>* mirrors = nullptr, bool gather = false,
                         const uint64_t* mul = nullptr);
 
+// Digits one ks_mac_kernel launch may add up for the `count` moduli of `mods`.  Each product is a lazy forward-transform
+// output (< 4q) times a key word (< q) and the kernel sums them unreduced in 128 bits, so at most
+// (2^128 - 1) / ((4q - 1)(q - 1)) of them fit for the largest q: the whole 64-entry key block below 2^60, down to 16
+// just below 2^61.  Launches beyond the first add their reduced sums into prod (the `accumulate` flag).
+static uint64_t ks_mac_digits_per_launch(const KsModuli& mods, uint64_t count) {
+  uint64_t q = 0;
+  for (uint64_t e = 0; e < count; ++e) q = std::max(q, mods.m[e].q);
+  const unsigned __int128 largest_product = (unsigned __int128)(4 * q - 1) * (q - 1);
+  return (uint64_t)std::min<unsigned __int128>(kParamBlock, ~(unsigned __int128)0 / largest_product);
+}
+
 // key-switch-internal.cpp:25-201 as a short chain of launches on the caller's stream, every
 // step batched over the RNS moduli (multi-modulus NTTs + the glue kernels of seal.cu): about a
 // dozen launches whatever the number of moduli, instead of ~10 per modulus.  Every pointer is
@@ -785,8 +796,9 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
     // every digit into every modulus of the round (:77-85) happens inside the transform: it reads the digits from
     // t_coef (L2-resident) and reduces on load, instead of a reduce kernel writing decomp x cnt x n words for it
     if (int rc = ntt_multi_on_device(true, dev, hs.data(), cnt, ops, t_coef, 4, decomp, s, nullptr, true)) return rc;
-    for (uint64_t j0 = 0; j0 < decomp; j0 += kParamBlock) {  // key pointers ride in the kernel parameters
-      const uint64_t jc = std::min<uint64_t>(kParamBlock, decomp - j0);
+    const uint64_t jmax = ks_mac_digits_per_launch(mods, cnt);
+    for (uint64_t j0 = 0; j0 < decomp; j0 += jmax) {  // key pointers ride in the kernel parameters
+      const uint64_t jc = std::min<uint64_t>(jmax, decomp - j0);
       KeyPointers kp;
       for (uint64_t j = 0; j < jc; ++j) kp.p[j] = d_key_ptrs_host[j0 + j];
       LAUNCH(launch_ks_mac(prod + i0 * kcc * n, ops + j0 * n, per_mod, kp, n, jc, kcc, key_modulus_size, cnt, mods,
@@ -1730,8 +1742,9 @@ static int key_switch_sharded(uint64_t* result, const uint64_t* t_target, uint64
         mods.m[e] = KsModulus{q, mu, R.w, R.wp, e0 + e};        // key slot = index inside the shard
       }
       if (bad(ntt_multi_on_device(true, z.device, h.data() + z.lo + e0, c, z.ops + e0 * per_mod, z.t_coef, 4, decomp, z.stream, nullptr, true))) break;
-      for (uint64_t j0 = 0; j0 < decomp && !rc; j0 += kParamBlock) {
-        const uint64_t jc = std::min<uint64_t>(kParamBlock, decomp - j0);
+      const uint64_t jmax = ks_mac_digits_per_launch(mods, c);
+      for (uint64_t j0 = 0; j0 < decomp && !rc; j0 += jmax) {
+        const uint64_t jc = std::min<uint64_t>(jmax, decomp - j0);
         KeyPointers kp;
         for (uint64_t j = 0; j < jc; ++j) kp.p[j] = z.keys[j0 + j];
         cu(launch_ks_mac(z.prod + e0 * kcc * n, z.ops + e0 * per_mod + j0 * n, per_mod, kp, n, jc, kcc, cnt, c, mods, j0 != 0, z.stream), "ks_mac");

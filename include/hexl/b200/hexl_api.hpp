@@ -563,6 +563,10 @@ inline void DyadicMultiply(uint64_t* result, const uint64_t* operand1, const uin
 }
 
 // hexl/include/hexl/experimental/seal/key-switch.hpp:34
+// Every modulus the switch uses must be below 2^61.  The result is exact for every accepted input; it differs from the
+// reference only where the reference's unreduced 128-bit sum of digit x key products wraps (moduli above 2^60 with
+// more than floor((2^128 - 1) / ((4q - 1)(q - 1))) digits, 16 just below 2^61).  The same holds for the resident-key
+// overload below.
 inline void KeySwitch(uint64_t* result, const uint64_t* t_target_iter_ptr, uint64_t n, uint64_t decomp_modulus_size,
                       uint64_t key_modulus_size, uint64_t rns_modulus_size, uint64_t key_component_count,
                       const uint64_t* moduli, const uint64_t** k_switch_keys, const uint64_t* modswitch_factors,

@@ -234,7 +234,11 @@ int hexl_b200_dyadic_multiply(uint64_t* result, const uint64_t* operand1, const 
                               uint64_t n, const uint64_t* moduli, uint64_t num_moduli, void* stream);
 /* KeySwitch, key-switch.hpp:34 (CKKS): result (key_component_count x decomp x n) is
  * updated in place; t_target_iter_ptr holds decomp x n digits in NTT form;
- * k_switch_keys[j] holds key_component_count x key_modulus_size x n. */
+ * k_switch_keys[j] holds key_component_count x key_modulus_size x n.
+ * Every modulus the switch uses must be below 2^61 (HEXL_B200_ERR_INVALID_ARG otherwise).  The result is exact for
+ * every accepted input.  It differs from the reference only where the reference's unreduced 128-bit sum of digit x
+ * key products wraps: moduli above 2^60 with more than J(q) = floor((2^128 - 1) / ((4q - 1)(q - 1))) digits (16 just
+ * below 2^61), where this library adds the digits up in chunks of at most J(q) instead. */
 int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, uint64_t n,
                          uint64_t decomp_modulus_size, uint64_t key_modulus_size, uint64_t rns_modulus_size,
                          uint64_t key_component_count, const uint64_t* moduli,
@@ -248,7 +252,8 @@ int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, ui
  * hexl_b200_set_host_devices when that was called -- and hexl_b200_key_switch_resident runs `batch` key switches
  * against them: ciphertext c uses result + c * key_component_count * decomp * n and t_target + c * decomp * n.
  * Host buffers are pipelined (copies of one ciphertext under the kernels of its neighbours) and split across the
- * devices holding the keys; device buffers run on `stream` on their own device. */
+ * devices holding the keys; device buffers run on `stream` on their own device.  Moduli, exactness and the difference
+ * from the reference are as for hexl_b200_key_switch, sharded handles included. */
 typedef struct hexl_b200_keys hexl_b200_keys;
 int hexl_b200_keys_upload(hexl_b200_keys** out, const uint64_t* const* k_switch_keys, uint64_t n,
                           uint64_t decomp_modulus_size, uint64_t key_modulus_size, uint64_t key_component_count);

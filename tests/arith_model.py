@@ -181,6 +181,12 @@ def shoup_lazy(x, w, q):
     return (x * w - mulhi(x, shoup(w, q)) * q) & M64
 
 
+def ks_mac_digits_per_launch(q):
+    """capi.cu:ks_mac_digits_per_launch -- digits one ks_mac_kernel launch adds up for moduli up to q: each product is
+    a lazy transform output (< 4q) times a key word (< q), and their sum must stay below 2^128"""
+    return min(64, ((1 << 128) - 1) // ((4 * q - 1) * (q - 1)))
+
+
 def ks_mac_finish(acc, q):
     """ks_mac_kernel's tail: a 128-bit accumulator hi:lo -> [0, q):  hi * (2^64 mod q) + lo, both lazily"""
     hi, lo = acc >> 64, acc & M64
