@@ -177,11 +177,12 @@ cudaError_t launch_pipe_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* 
 }
 
 // log2(N / 4096) for which the pipelined kernel is used; 0 = none.  HEXL_B200_PIPE: 1 = always (N = 2^14..2^17),
-// 0 = never, unset = the 64-bit modes' forward at N = 2^17.  One H100 SXM at 400 W, 2^28 coefficients, 55-bit q
-// (tools/tune_split.py, ms, vs the two-kernel split): forward 14.9 vs 17.2, inverse 15.5 vs 15.4; at N = 2^16 the
-// forward's 14.0 vs 15.3 did not carry over to the benchmark's whole step, so the split stays there.  32-bit words
-// use the distributed-shared-memory kernel instead (dsmem_log_r).  A batch of fewer polynomials than the pipeline
-// is deep gains nothing from it.
+// 0 = never, unset = the 64-bit modes' forward at N = 2^17.  One H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit q
+// (tools/tune_split.py, ms, pipelined vs the two-kernel split), with the coefficient arrays in registers: N = 2^17
+// forward 3.10 vs 3.67, inverse 3.58 vs 3.71; N = 2^16 forward 2.86 vs 3.47, inverse 3.51 vs 3.71.  (Before, with
+// the arrays in local memory: 2^17 forward 14.9 vs 17.2, inverse 15.5 vs 15.4.)  The N = 2^16 defaults stay the
+// split until the gain is confirmed on the benchmark's whole step.  32-bit words use the distributed-shared-memory
+// kernel instead (dsmem_log_r).  A batch of fewer polynomials than the pipeline is deep gains nothing from it.
 template <int MODE>
 inline int pipe_log_r(int log_n, u64 batch, bool forward) {
   static const int mode = env_int("HEXL_B200_PIPE", -1);
@@ -238,14 +239,19 @@ cudaError_t launch_dsmem_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64*
 // One H100 SXM at 400 W, 2^28 coefficients, 29-bit q, forward / inverse ms vs the cluster kernel that keeps the
 // intermediate in L2: N = 2^14 6.41 / 6.69 vs 6.90 / 7.26, 2^15 6.42 / 6.77 vs 6.83 / 7.29, 2^16 7.54 / 7.84 vs
 // 7.99 / 8.15, 2^17 7.81 / 8.10 vs 8.25 / 8.42 (and vs 7.79 / 8.23, 8.10 / 8.30 for the pipelined kernel at 2^16 /
-// 2^17), so it is the default at every size (HEXL_B200_DSMEM=0 disables it).
+// 2^17), so it is the default at every size (HEXL_B200_DSMEM=0 disables it).  Re-timed on an H100 80GB HBM3 (power
+// limit not recorded) with the coefficient arrays
+// in registers: N = 2^16 1.76 / 1.79 vs 1.97 / 1.94, 2^17 1.94 / 2.08 vs 2.22 / 2.13 (pipelined 2.05 / 2.15).
 int dsmem_log_r(int log_n) {
   static const int mode = env_int("HEXL_B200_DSMEM", 1);
   const int lr = log_n - DsmemCfg<2>::LOGC;
   return (mode != 0 && lr >= 2 && lr <= 5) ? lr : 0;
 }
 
-// log2(N / 4096) for which the single fused kernel is used; 0 = none
+// log2(N / 4096) for which the single fused kernel is used; 0 = none.  Off by default for the 64-bit modes
+// (HEXL_B200_FUSED=1 enables it).  One H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit q, coefficient arrays in
+// registers, ms vs the default path: N = 2^16 forward 3.04 vs 3.47, inverse 3.10 vs 3.71; N = 2^17 inverse 3.91 vs
+// 3.71.  Like the pipelined N = 2^16 forward, the 2^16 gain is not yet confirmed on the benchmark's whole step.
 template <int MODE>
 int fused_log_r(int log_n) {
   static const bool enabled = MODE == kSmall ? env_int("HEXL_B200_FUSED_SMALL", 1) != 0 : env_int("HEXL_B200_FUSED", 0) != 0;

@@ -44,6 +44,23 @@
 namespace hexl_b200 {
 namespace {
 
+// f(Idx<I>{}) for I = BEGIN, ..., END - 1.  Every loop over a register array below is written this way, so each
+// index is a compile-time constant by construction: a `#pragma unroll` loop is only unrolled when the compiler
+// decides so, and a register array indexed at run time is placed in local memory (the sm_90a front end unrolled
+// the stage loops, whose inner trip counts depend on the outer index, only partially).  The body reads the index
+// as `constexpr int i = I;`.
+template <int I>
+struct Idx {
+  __host__ __device__ constexpr operator int() const { return I; }
+};
+template <int BEGIN, int END, typename F>
+__device__ __forceinline__ void static_for(F&& f) {
+  if constexpr (BEGIN < END) {
+    f(Idx<BEGIN>{});
+    static_for<BEGIN + 1, END>(f);
+  }
+}
+
 // ----------------------------------------------------------------- arithmetic
 // H100 has no 64-bit integer multiplier; a 64x64 product is built from 32-bit
 // IMADs (FMA pipe, full rate) while 64-bit adds/compares/selects cost two
@@ -544,46 +561,58 @@ __device__ __forceinline__ void reg_stages(typename Ar<MODE>::E (&v)[16], unsign
   using PT = PassTw<LOGC, LB, HB, LOB>;
   using Tw = typename Ar<MODE>::Tw;
   const Tw* sroot = stab + PT::kOffset + ((u >> LB) << 4);  // this thread's sub-tree table
-  Tw wc[8];
-  auto stage_node0 = [&](int step) {
-    const int beta = FWD ? HB - step : LOB + step;
-    return (base << (LOGC - 1 - beta)) + ((u64)(u >> LB) << (LB + 3 - beta));
-  };
-#pragma unroll
-  for (int step = 0; step <= HB - LOB; ++step) {
-    const int beta = FWD ? HB - step : LOB + step;  // index bit of this stage
-    const int eb = beta - LB;                       // register bit
-    const int sp = LOGC - 1 - beta;                 // stage number inside the row
+  static_for<0, HB - LOB + 1>([&](auto STEP) {
+    constexpr int step = STEP;
+    constexpr int beta = FWD ? HB - step : LOB + step;  // index bit of this stage
+    constexpr int eb = beta - LB;                       // register bit
+    constexpr int sp = LOGC - 1 - beta;                 // stage number inside the row
     // FAST inverse: multiple of q covering every Y of this stage (GENERIC: 2q)
     const typename Ar<MODE>::E cq = stage_cq<MODE>(step, m);
-    if (!FWD && sp == 0 && fold) {
-      // root stage of the whole transform: one group, N^-1 folded in
-#pragma unroll
-      for (int l = 0; l < (1 << eb); ++l) inv_bfly_last(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
-    } else {
-#pragma unroll
-      for (int g = 0; g < (8 >> eb); ++g) {
-        if (PT::kShared)
-          wc[g] = sroot[(8 >> eb) + g];             // local node 2^s' + g, s' = 3 - eb
-        else if (HEXL_B200_ABLATE & 4)
-          wc[g] = stab[((8 >> eb) + g + (u & 15) * 16) & 255];
+    auto fetch = [&](int g) {
+      if constexpr (PT::kShared)
+        return sroot[(8 >> eb) + g];                // local node 2^s' + g, s' = 3 - eb
+      else if constexpr ((HEXL_B200_ABLATE & 4) != 0)
+        return stab[((8 >> eb) + g + (u & 15) * 16) & 255];
+      else
+        return ld_tw(tw + (base << (LOGC - 1 - beta)) + ((u64)(u >> LB) << (LB + 3 - beta)) + g);
+    };
+    auto groups = [&] {
+      // Forward stages fetch all their twiddles first.  The inverse fetches each group's twiddle just before its
+      // butterflies: its first stage per pass has 8 groups, and 8 twiddles held next to the 16 coefficients push
+      // the 64-bit row kernels past their register bound.
+      Tw wc[8 >> eb];
+      if constexpr (FWD) static_for<0, (8 >> eb)>([&](auto G) { constexpr int g = G; wc[g] = fetch(g); });
+      static_for<0, (8 >> eb)>([&](auto G) {
+        constexpr int g = G;
+        Tw wt;
+        if constexpr (FWD)
+          wt = wc[g];
         else
-          wc[g] = ld_tw(tw + stage_node0(step) + g);
-      }
-#pragma unroll
-      for (int g = 0; g < (8 >> eb); ++g) {
-        const typename TwUse<MODE>::T wg = TwUse<MODE>::prep(wc[g]);
-#pragma unroll
-        for (int l = 0; l < (1 << eb); ++l) {
-          const int e = (g << (eb + 1)) | l;
-          if (FWD)
+          wt = fetch(g);
+        const typename TwUse<MODE>::T wg = TwUse<MODE>::prep(wt);
+        static_for<0, (1 << eb)>([&](auto L) {
+          constexpr int e = (g << (eb + 1)) | L;
+          if constexpr (FWD)
             fwd_bfly<MODE>(v[e], v[e | (1 << eb)], wg, m);
           else
             inv_bfly<MODE>(v[e], v[e | (1 << eb)], wg, m, cq);
-        }
+        });
+      });
+    };
+    if constexpr (!FWD && sp == 0) {
+      if (fold) {
+        // root stage of the whole transform: one group, N^-1 folded in
+        static_for<0, (1 << eb)>([&](auto L) {
+          constexpr int l = L;
+          inv_bfly_last(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
+        });
+      } else {
+        groups();
       }
+    } else {
+      groups();
     }
-  }
+  });
   if constexpr (!FWD && MODE == kFast) {
     if (!(fold && LOGC - 1 - HB == 0)) inv_pass_fixup<HB - LOB + 1, 16>(v, m);
   }
@@ -602,23 +631,19 @@ __device__ __forceinline__ void smem_exchange(E (&v)[16], E* srow, unsigned u) {
     const unsigned uf = reg_index<LB_FROM>(u, 0), ut = reg_index<LB_TO>(u, 0);
     E* wr = srow + (uf + (uf >> 4));
     const E* rd = srow + (ut + (ut >> 4));
-#pragma unroll
-    for (int e = 0; e < 16; ++e) wr[pad_slot(e, LB_FROM)] = v[e];
+    static_for<0, 16>([&](auto I) { constexpr int e = I; wr[pad_slot(e, LB_FROM)] = v[e]; });
     if (kWarpLocal)
       __syncwarp();
     else
       __syncthreads();
-#pragma unroll
-    for (int e = 0; e < 16; ++e) v[e] = rd[pad_slot(e, LB_TO)];
+    static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = rd[pad_slot(e, LB_TO)]; });
   } else {
-#pragma unroll
-    for (int e = 0; e < 16; ++e) srow[swz<E>(reg_index<LB_FROM>(u, e))] = v[e];
+    static_for<0, 16>([&](auto I) { constexpr int e = I; srow[swz<E>(reg_index<LB_FROM>(u, e))] = v[e]; });
     if (kWarpLocal)
       __syncwarp();
     else
       __syncthreads();
-#pragma unroll
-    for (int e = 0; e < 16; ++e) v[e] = srow[swz<E>(reg_index<LB_TO>(u, e))];
+    static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = srow[swz<E>(reg_index<LB_TO>(u, e))]; });
   }
 }
 
@@ -656,6 +681,8 @@ __device__ __forceinline__ void inv_passes(typename Ar<MODE>::E (&v)[16], typena
   }
 }
 
+// 64-bit row kernels of 256 threads: 3 CTAs per SM (80 registers).  One H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit
+// q, N = 2^16 (tools/tune_split.py): forward / inverse 3.47 / 3.71 ms, against 3.58 / 3.94 ms with 2 CTAs per SM.
 #ifndef HEXL_B200_ROW_MIN_BLOCKS
 #define HEXL_B200_ROW_MIN_BLOCKS 3
 #endif
@@ -735,17 +762,16 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
   // cta_stab: every row of this CTA has the same root (whole polynomials, N == C): one table
   // filled by all threads of the CTA instead of one per row
   Tw* stab = cta_stab ? cta_stab : reinterpret_cast<Tw*>(srow + row_elems<E>(LOGC));
-#pragma unroll
-  for (int e = 0; e < 16; ++e) {
-    if (HEXL_B200_ABLATE & 1)
+  static_for<0, 16>([&](auto I) {
+    constexpr int e = I;
+    if constexpr ((HEXL_B200_ABLATE & 1) != 0)
       v[e] = (E)((u * 16 + e) * 0x9E3779B97F4A7C15ull + base) & (E)(m.q - 1);
     else
       v[e] = ld_row<LD, E>(in, reg_index<LB0>(u, e));
-  }
+  });
   if constexpr (LD != kSmemRow && sizeof(E) == 8) {
     if (reduce_in) {  // NttMulti::gather: the input is a value of ANOTHER modulus
-#pragma unroll
-      for (int e = 0; e < 16; ++e) v[e] = reduce_any(v[e], m);
+      static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = reduce_any(v[e], m); });
     }
   }
   if constexpr (RowCfg<LOGC>::TW_TABLES) {
@@ -760,16 +786,16 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
   reg_stages<MODE, LOGC, LB0, LOGC - 1, LB0, true>(v, u, base, tw, stab, m, false, Tw{}, Tw{});
   fwd_passes<MODE, LOGC, 1>(v, srow, u, base, tw, stab, m);
   // registers now hold 16 consecutive coefficients per thread (LB = 0)
-#pragma unroll
-  for (int e = 0; e < 16; ++e) v[e] = fwd_out<MODE>(v[e], m, out_mf);
+  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = fwd_out<MODE>(v[e], m, out_mf); });
   // store layout: 16 lanes write one 128-byte line per instruction; reaching it
   // from LB = 0 is a warp-local exchange
   constexpr int LB_OUT = LB0 < 4 ? LB0 : 4;
   if constexpr (LOGC > 4) smem_exchange<0, LB_OUT>(v, srow, u);
   if (active) {
-#pragma unroll
-    for (int e = 0; e < 16; ++e)
+    static_for<0, 16>([&](auto I) {
+      constexpr int e = I;
       if (!(HEXL_B200_ABLATE & 2) || v[e] == (E)0x123456789abcdefull) st_row<ST, E>(out, reg_index<LB_OUT>(u, e), v[e]);
+    });
   }
 }
 
@@ -788,13 +814,13 @@ __device__ __forceinline__ void row_inv_body(void* out, const void* in, typename
   constexpr int LB0 = LOGC - 4;
   constexpr int LB_IN = LB0 < 4 ? LB0 : 4;  // 16 lanes read one 128-byte line per instruction
   Tw* stab = cta_stab ? cta_stab : reinterpret_cast<Tw*>(srow + row_elems<E>(LOGC));
-#pragma unroll
-  for (int e = 0; e < 16; ++e) v[e] = ld_row<LD, E>(in, reg_index<LB_IN>(u, e));
+  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, reg_index<LB_IN>(u, e)); });
   if constexpr (LD != kSmemRow && sizeof(E) == 8) {
     if (prod) {  // NttMulti::mul: the transform of a point-wise product, multiplied on load
-#pragma unroll
-      for (int e = 0; e < 16; ++e)
+      static_for<0, 16>([&](auto I) {
+        constexpr int e = I;
         v[e] = prod_lazy<MODE>(v[e], ld_coef<LD>(prod->b + reg_index<LB_IN>(u, e)), m, prod->mu, prod->shift);
+      });
     }
   }
   if constexpr (Cfg::TW_TABLES) {
@@ -810,12 +836,16 @@ __device__ __forceinline__ void row_inv_body(void* out, const void* in, typename
   // last pass left the registers in the coalesced layout (LB = LOGC-4);
   // only the kernel holding the root stage applies the output range
   if (active) {
-#pragma unroll
-    for (int e = 0; e < 16; ++e) st_row<ST, E>(out, reg_index<LB0>(u, e), fold ? inv_out(v[e], m, out_mf) : v[e]);
+    static_for<0, 16>([&](auto I) {
+      constexpr int e = I;
+      st_row<ST, E>(out, reg_index<LB0>(u, e), fold ? inv_out(v[e], m, out_mf) : v[e]);
+    });
     if (mir && fold) {
       for (unsigned p = 0; p < mir->count; ++p) {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) mir->p[p][mir->off + reg_index<LB0>(u, e)] = (u64)inv_out(v[e], m, out_mf);
+        static_for<0, 16>([&](auto I) {
+          constexpr int e = I;
+          mir->p[p][mir->off + reg_index<LB0>(u, e)] = (u64)inv_out(v[e], m, out_mf);
+        });
       }
     }
   }
@@ -877,29 +907,37 @@ __device__ __forceinline__ void col_stages(typename Ar<MODE>::E (&v)[1 << LOGR],
   using E = typename Ar<MODE>::E;
   using Tw = typename Ar<MODE>::Tw;
   constexpr int R = 1 << LOGR;
-#pragma unroll
-  for (int step = 0; step < LOGR; ++step) {
-    const int s = FWD ? step : LOGR - 1 - step;      // stage inside the sub-block
-    const int eb = LOGR - 1 - s;                     // register bit
+  static_for<0, LOGR>([&](auto STEP) {
+    constexpr int step = STEP;
+    constexpr int s = FWD ? step : LOGR - 1 - step;  // stage inside the sub-block
+    constexpr int eb = LOGR - 1 - s;                 // register bit
     const E cq = stage_cq<MODE>(step, m);
-    if (!FWD && root_fold && s == 0) {
-#pragma unroll
-      for (int l = 0; l < (1 << eb); ++l) inv_bfly_last(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
-    } else {
-#pragma unroll
-      for (int gi = 0; gi < (1 << s); ++gi) {
+    auto groups = [&] {
+      static_for<0, (1 << s)>([&](auto GI) {
+        constexpr int gi = GI;
         const typename TwUse<MODE>::T w = TwUse<MODE>::prep(stw[(1 << s) + gi]);
-#pragma unroll
-        for (int l = 0; l < (1 << eb); ++l) {
-          const int e = (gi << (eb + 1)) | l;
-          if (FWD)
+        static_for<0, (1 << eb)>([&](auto L) {
+          constexpr int e = (gi << (eb + 1)) | L;
+          if constexpr (FWD)
             fwd_bfly<MODE>(v[e], v[e | (1 << eb)], w, m);
           else
             inv_bfly<MODE>(v[e], v[e | (1 << eb)], w, m, cq);
-        }
+        });
+      });
+    };
+    if constexpr (!FWD && s == 0) {
+      if (root_fold) {
+        static_for<0, (1 << eb)>([&](auto L) {
+          constexpr int l = L;
+          inv_bfly_last(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
+        });
+      } else {
+        groups();
       }
+    } else {
+      groups();
     }
-  }
+  });
   if constexpr (!FWD && MODE == kFast) {
     if (!root_fold) inv_pass_fixup<LOGR, R>(v, m);
   }
@@ -913,23 +951,27 @@ __device__ __forceinline__ void col_body(u64* result, const u64* operand, u64 of
   using E = typename Ar<MODE>::E;
   constexpr int R = 1 << LOGR;
   E v[R];
-#pragma unroll
-  for (int e = 0; e < R; ++e) v[e] = (E)ld_coef<LD>(operand + off + ((u64)e << log_stride));
+  static_for<0, R>([&](auto I) {
+    constexpr int e = I;
+    v[e] = (E)ld_coef<LD>(operand + off + ((u64)e << log_stride));
+  });
   if constexpr (FWD && sizeof(E) == 8) {
     if (reduce_in) {
-#pragma unroll
-      for (int e = 0; e < R; ++e) v[e] = reduce_any(v[e], m);
+      static_for<0, R>([&](auto I) { constexpr int e = I; v[e] = reduce_any(v[e], m); });
     }
   }
   col_stages<MODE, LOGR, FWD>(v, stw, m, root_fold, inv_n, inv_n_w);
   const bool final_out = !FWD && root_fold;
-#pragma unroll
-  for (int e = 0; e < R; ++e)
+  static_for<0, R>([&](auto I) {
+    constexpr int e = I;
     st_coef<ST>(result + off + ((u64)e << log_stride), final_out ? inv_out(v[e], m, out_mf) : v[e]);
+  });
   if (mir && final_out) {
     for (unsigned p = 0; p < mir->count; ++p) {
-#pragma unroll
-      for (int e = 0; e < R; ++e) mir->p[p][mir->off + off + ((u64)e << log_stride)] = (u64)inv_out(v[e], m, out_mf);
+      static_for<0, R>([&](auto I) {
+        constexpr int e = I;
+        mir->p[p][mir->off + off + ((u64)e << log_stride)] = (u64)inv_out(v[e], m, out_mf);
+      });
     }
   }
 }
@@ -1220,18 +1262,20 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_B
   asm volatile("barrier.cluster.wait.aligned;" ::: "memory");
   // phase 1: my columns of every row -> the row owners' shared memory
   unsigned owner_base[Cfg::K];
-#pragma unroll
-  for (int o = 0; o < Cfg::K; ++o) owner_base[o] = dsmem_address(rows, o);
+  static_for<0, Cfg::K>([&](auto I) { constexpr int o = I; owner_base[o] = dsmem_address(rows, o); });
 #pragma unroll 1
   for (int c = threadIdx.x; c < Cfg::COLS; c += Cfg::THREADS) {
     const unsigned col = rank * Cfg::COLS + c;
     unsigned v[Cfg::R];
-#pragma unroll
-    for (int e = 0; e < Cfg::R; ++e) v[e] = (unsigned)ld_coef<kStream>(operand + poly_off + ((u64)e << Cfg::LOGC) + col);
+    static_for<0, Cfg::R>([&](auto I) {
+      constexpr int e = I;
+      v[e] = (unsigned)ld_coef<kStream>(operand + poly_off + ((u64)e << Cfg::LOGC) + col);
+    });
     col_stages<kSmall, LOGR, true>(v, stw, m, false, Twiddle32{}, Twiddle32{});
-#pragma unroll
-    for (int e = 0; e < Cfg::R; ++e)  // row e lives in CTA e % K, slot e / K
+    static_for<0, Cfg::R>([&](auto I) {  // row e lives in CTA e % K, slot e / K
+      constexpr int e = I;
       dsmem_store(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::C + col) * 4u, v[e]);
+    });
   }
   cluster_barrier();
   // phase 2: my rows, shared memory -> HBM
@@ -1269,18 +1313,20 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_B
   cluster_barrier();
   // phase 2: my columns gathered from the row owners, root stage folded with N^-1, -> HBM
   unsigned owner_base[Cfg::K];
-#pragma unroll
-  for (int o = 0; o < Cfg::K; ++o) owner_base[o] = dsmem_address(rows, o);
+  static_for<0, Cfg::K>([&](auto I) { constexpr int o = I; owner_base[o] = dsmem_address(rows, o); });
 #pragma unroll 1
   for (int c = threadIdx.x; c < Cfg::COLS; c += Cfg::THREADS) {
     const unsigned col = rank * Cfg::COLS + c;
     unsigned v[Cfg::R];
-#pragma unroll
-    for (int e = 0; e < Cfg::R; ++e) v[e] = dsmem_load(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::C + col) * 4u);
+    static_for<0, Cfg::R>([&](auto I) {
+      constexpr int e = I;
+      v[e] = dsmem_load(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::C + col) * 4u);
+    });
     col_stages<kSmall, LOGR, false>(v, stw, m, true, inv_n, inv_n_w);
-#pragma unroll
-    for (int e = 0; e < Cfg::R; ++e)
+    static_for<0, Cfg::R>([&](auto I) {
+      constexpr int e = I;
       st_coef<kStream>(result + poly_off + ((u64)e << Cfg::LOGC) + col, inv_out(v[e], m, out_mf));
+    });
   }
   cluster_barrier();  // nobody leaves while a peer may still read its rows
 }

@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(RowCfg<LOGC, MODE>::THREADS, RowCfg<LOGC, MODE
     const ProdIn prod{MUL ? multi.mul + row * Cfg::C : nullptr, P.prod_mu, P.prod_shift};
     row_inv_body<MODE, LOGC, kStream, kStream>(result + row * Cfg::C, operand + row * Cfg::C, srow, u, base, P.inv, m,
                                                out_mf, fold != 0, P.inv_n, P.inv_n_w, active, nullptr,
-                                               multi.mirrors ? &mir : nullptr, MUL ? &prod : nullptr);
+                                               &mir, MUL ? &prod : nullptr);
   }
 }
 
@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(256)
   const u64* src = (FWD && gather) ? operand + (((poly % gather) - poly) << log_n) : operand;
   col_body<MODE, LOGR, FWD, kStream, kStream>(result, src, (blk << log_s) + c, log_cols, stw, m, out_mf,
                                               !FWD && fold && log_s == log_n, P.inv_n, P.inv_n_w,
-                                              (!FWD && multi.mirrors) ? &mir : nullptr, FWD && gather != 0);
+                                              FWD ? nullptr : &mir, FWD && gather != 0);
 }
 
 // The persistent pipelined single kernel of ntt_kernels.cuh (ntt_pipe_fwd / _inv) for RNS batches: the same work
@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MO
         const MirrorList mir{multi.mirror, multi.mirrors, 0};
         col_body<MODE, LOGR, false, kViaL2, kStream>(result, result, poly_off + (j - Cfg::R) * Cfg::THREADS + threadIdx.x,
                                                      Cfg::LOGC, stw, m, out_mf, true, P.inv_n, P.inv_n_w,
-                                                     multi.mirrors ? &mir : nullptr);
+                                                     &mir);
       }
     }
     if (producer) {
@@ -192,41 +192,52 @@ inline int pipe_multi_log_r(int log_n, u64 units, bool forward) {
   return (forward && log_n == 17) ? lr : 0;
 }
 
-// N < 16: one thread per polynomial, everything in registers (launch-bound shapes only)
-template <bool FWD>
-__global__ void ntt_tiny_multi(u64* result, const u64* operand, const __grid_constant__ NttMulti multi, int log_n,
-                               u64 units, int out_mf) {
+// N = 2^LOGN < 16: one thread per polynomial, everything in registers (launch-bound shapes only)
+template <bool FWD, int LOGN>
+__global__ void ntt_tiny_multi(u64* result, const u64* operand, const __grid_constant__ NttMulti multi, u64 units,
+                               int out_mf) {
   const u64 unit = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (unit >= units) return;
   const NttDeviceParams P = *multi.p[unit / multi.group];
   const Mod m = make_mod(P.q, P.mu);
-  const int n = 1 << log_n;
-  u64 v[8];
+  constexpr int n = 1 << LOGN;
+  u64 v[n];
   const u64 src_unit = (FWD && multi.gather) ? unit % multi.gather : unit;
-  for (int e = 0; e < n; ++e) {
+  static_for<0, n>([&](auto I) {
+    constexpr int e = I;
     v[e] = operand[src_unit * n + e];
     if (FWD && multi.gather) v[e] %= P.q;
     if (!FWD && multi.mul) v[e] = prod_lazy<kGeneric>(v[e], multi.mul[unit * n + e], m, P.prod_mu, P.prod_shift);
-  }
-  for (int k = 0; k < log_n; ++k) {
-    const int s = FWD ? k : log_n - 1 - k;  // stage: 2^s groups, span t
-    const int t = n >> (s + 1);
-    for (int i = 0; i < (1 << s); ++i)
-      for (int j = 0; j < t; ++j) {
+  });
+  static_for<0, LOGN>([&](auto K) {
+    constexpr int k = K;
+    constexpr int s = FWD ? k : LOGN - 1 - k;  // stage: 2^s groups, span t
+    constexpr int t = n >> (s + 1);
+    static_for<0, (1 << s)>([&](auto I) {
+      constexpr int i = I;
+      static_for<0, t>([&](auto J) {
+        constexpr int j = J;
         u64& X = v[2 * i * t + j];
         u64& Y = v[2 * i * t + j + t];
-        if (FWD)
+        if constexpr (FWD)
           fwd_bfly<kGeneric>(X, Y, P.fwd[(1 << s) + i], m);
-        else if (s == 0)
+        else if constexpr (s == 0)
           inv_bfly_last(X, Y, P.inv_n, P.inv_n_w, m, m.two_q);
         else
           inv_bfly<kGeneric>(X, Y, P.inv[(1 << s) + i], m, m.two_q);
-      }
-  }
-  for (int e = 0; e < n; ++e) result[unit * n + e] = FWD ? fwd_out<kGeneric>(v[e], m, out_mf) : inv_out(v[e], m, out_mf);
+      });
+    });
+  });
+  static_for<0, n>([&](auto I) {
+    constexpr int e = I;
+    result[unit * n + e] = FWD ? fwd_out<kGeneric>(v[e], m, out_mf) : inv_out(v[e], m, out_mf);
+  });
   if (!FWD)
     for (unsigned p = 0; p < multi.mirrors; ++p)
-      for (int e = 0; e < n; ++e) multi.mirror[p][unit * n + e] = inv_out(v[e], m, out_mf);
+      static_for<0, n>([&](auto I) {
+        constexpr int e = I;
+        multi.mirror[p][unit * n + e] = inv_out(v[e], m, out_mf);
+      });
 }
 
 template <int MODE, int LOGC>
@@ -342,10 +353,18 @@ cudaError_t launch_ntt_multi(bool forward, const NttMulti& multi, int log_n, u64
   if (units == 0) return cudaSuccess;
   if (log_n < 4) {
     const unsigned threads = 128, grid = (unsigned)((units + threads - 1) / threads);
-    if (forward)
-      ntt_tiny_multi<true><<<grid, threads, 0, stream>>>(result, operand, multi, log_n, units, out_mf);
-    else
-      ntt_tiny_multi<false><<<grid, threads, 0, stream>>>(result, operand, multi, log_n, units, out_mf);
+    switch (log_n) {
+#define TINY_CASE(L)                                                                                 \
+  case L:                                                                                            \
+    if (forward)                                                                                     \
+      ntt_tiny_multi<true, L><<<grid, threads, 0, stream>>>(result, operand, multi, units, out_mf);  \
+    else                                                                                             \
+      ntt_tiny_multi<false, L><<<grid, threads, 0, stream>>>(result, operand, multi, units, out_mf); \
+    break;
+      TINY_CASE(0) TINY_CASE(1) TINY_CASE(2) TINY_CASE(3)
+#undef TINY_CASE
+      default: return cudaErrorInvalidValue;
+    }
     count_launch();
     return cudaGetLastError();
   }
