@@ -1281,6 +1281,9 @@ int hexl_b200_eltwise_reduce_mod(uint64_t* result, const uint64_t* operand, uint
   REQUIRE(out_mf == 1 || out_mf == 2, "output_mod_factor must be 1 or 2; got %llu", (unsigned long long)out_mf);
   EltParams p{};
   p.result = result; p.a = operand; p.n = n; p.q = q; p.out_mf = (int)out_mf;
+  // From q >= 2^63 on, every 64-bit word is below 2q, so input_mod_factor 4 is the 2 case; reducing from [0, 4q) would
+  // subtract 2q, which wraps (as it does in every tier of the reference).
+  if (in_mf == 4 && q >= (1ull << 63)) in_mf = 2;
   if (in_mf == out_mf) {  // eltwise-reduce-mod.cpp:94-99: plain copy (no-op in place)
     if (result == operand) return 0;
     return eltwise_dispatch(EltOp::Copy, p, stream);

@@ -59,8 +59,10 @@ struct FSubVS {
     return a >= s ? a - s : a + q - s;
   }
 };
-// generalised Barrett, alpha = 62, beta = -2 (eltwise-mult-mod-internal.hpp:52-99)
-template <int IN_MF>
+// generalised Barrett, alpha = 62, beta = -2 (eltwise-mult-mod-internal.hpp:52-99).  The quotient estimate is low by at
+// most one while bits(q) <= 61, so z < 2q.  At 62 bits (shift == 60) alpha - bits(q) = 0 and it can be low by two:
+// WIDE reduces z from [0, 3q) with a second conditional subtraction (the reference's scalar tier makes one only).
+template <int IN_MF, bool WIDE>
 struct FMult {
   u64 q, mu;
   int shift;
@@ -69,8 +71,8 @@ struct FMult {
     u64 lo = x * y, hi = mulhi(x, y);
     // c1 = floor(U / 2^shift); shift in [0, 60]
     u64 c1 = shift ? ((lo >> shift) | (hi << (64 - shift))) : lo;
-    u64 z = lo - mulhi(c1, mu) * q;
-    return csub(z, q);
+    u64 z = csub(lo - mulhi(c1, mu) * q, q);
+    return WIDE ? csub(z, q) : z;
   }
 };
 template <int IN_MF, bool ADD>
@@ -223,6 +225,15 @@ cudaError_t run(const EltParams& p, F f, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+template <bool WIDE>
+cudaError_t run_mult(const EltParams& p, cudaStream_t s) {
+  switch (p.in_mf) {
+    case 1: return run<FMult<1, WIDE>, 2>(p, FMult<1, WIDE>{p.q, p.mu, p.shift}, s);
+    case 2: return run<FMult<2, WIDE>, 2>(p, FMult<2, WIDE>{p.q, p.mu, p.shift}, s);
+    default: return run<FMult<4, WIDE>, 2>(p, FMult<4, WIDE>{p.q, p.mu, p.shift}, s);
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_eltwise(EltOp op, const EltParams& p, cudaStream_t s) {
@@ -231,12 +242,8 @@ cudaError_t launch_eltwise(EltOp op, const EltParams& p, cudaStream_t s) {
     case EltOp::AddVS: return run<FAddVS, 1>(p, FAddVS{p.q, p.scalar}, s);
     case EltOp::SubVV: return run<FSubVV, 2>(p, FSubVV{p.q}, s);
     case EltOp::SubVS: return run<FSubVS, 1>(p, FSubVS{p.q, p.scalar}, s);
-    case EltOp::MultVV:
-      switch (p.in_mf) {
-        case 1: return run<FMult<1>, 2>(p, FMult<1>{p.q, p.mu, p.shift}, s);
-        case 2: return run<FMult<2>, 2>(p, FMult<2>{p.q, p.mu, p.shift}, s);
-        default: return run<FMult<4>, 2>(p, FMult<4>{p.q, p.mu, p.shift}, s);
-      }
+    case EltOp::MultVV:  // shift = bits(q) - 2: 60 for the 62-bit moduli
+      return p.shift == 60 ? run_mult<true>(p, s) : run_mult<false>(p, s);
     case EltOp::Fma:
       switch (p.in_mf) {
         case 1: return run<FFma<1, true>, 2>(p, FFma<1, true>{p.q, p.scalar, p.scalar_p}, s);

@@ -12,15 +12,18 @@ namespace {
 constexpr int kThreads = 256;
 
 // generalised Barrett x*y mod q for x, y < q (same arithmetic as EltwiseMultMod,
-// eltwise-mult-mod-internal.hpp:71-99)
+// eltwise-mult-mod-internal.hpp:71-99).  WIDE: the launch has a 62-bit modulus, whose quotient estimate can be low by
+// two, so the product is reduced from [0, 3q) with a second conditional subtraction (eltwise.cu:FMult).
 struct MulCtx {
   u64 q, mu;
   int shift;
 };
+template <bool WIDE>
 __device__ __forceinline__ u64 mulmod(u64 x, u64 y, const MulCtx& c) {
   const u64 lo = x * y, hi = mulhi(x, y);
   const u64 c1 = c.shift ? ((lo >> c.shift) | (hi << (64 - c.shift))) : lo;
-  return csub(lo - mulhi(c1, c.mu) * c.q, c.q);
+  const u64 z = csub(lo - mulhi(c1, c.mu) * c.q, c.q);
+  return WIDE ? csub(z, c.q) : z;
 }
 
 // ---- DyadicMultiply: (x0*y0, x0*y1 + x1*y0, x1*y1) for every RNS modulus.
@@ -54,7 +57,7 @@ __device__ __forceinline__ void st_slots(u64* p, const Slots<VEC>& r) {
   }
 }
 
-template <int VEC>
+template <int VEC, bool WIDE>
 __global__ void __launch_bounds__(kThreads)
     dyadic_kernel(u64* result, const u64* op1, const u64* op2, u64 n, u64 num_moduli, u64 first, u64 count,
                   const __grid_constant__ DyadicModuli mods) {
@@ -69,9 +72,9 @@ __global__ void __launch_bounds__(kThreads)
     Slots<VEC> r0, r1, r2;
 #pragma unroll
     for (int k = 0; k < VEC; ++k) {
-      r0.v[k] = mulmod(x0.v[k], y0.v[k], c);
-      r1.v[k] = csub(mulmod(x0.v[k], y1.v[k], c) + mulmod(x1.v[k], y0.v[k], c), c.q);
-      r2.v[k] = mulmod(x1.v[k], y1.v[k], c);
+      r0.v[k] = mulmod<WIDE>(x0.v[k], y0.v[k], c);
+      r1.v[k] = csub(mulmod<WIDE>(x0.v[k], y1.v[k], c) + mulmod<WIDE>(x1.v[k], y0.v[k], c), c.q);
+      r2.v[k] = mulmod<WIDE>(x1.v[k], y1.v[k], c);
     }
     st_slots<VEC>(result + o, r0);
     st_slots<VEC>(result + o + poly, r1);
@@ -82,7 +85,7 @@ __global__ void __launch_bounds__(kThreads)
 // ---- EltwiseMultMod / AddMod / SubMod over an RNS batch: block e of per_mod elements under
 // modulus e (eltwise-mult-mod-internal.hpp:33-101, eltwise-add-mod.cpp:16-40, eltwise-sub-mod.cpp:16-40
 // per element; MultMod inputs < in_mf * q_e with in_mf in {1,2,4}, Add/Sub inputs < q_e).
-template <int VEC>
+template <int VEC, bool WIDE>
 __global__ void __launch_bounds__(kThreads)
     rns_eltwise_kernel(u64* result, const u64* a, const u64* b, u64 per_mod, u64 count, int op, int in_mf,
                        const __grid_constant__ DyadicModuli mods) {
@@ -112,7 +115,7 @@ __global__ void __launch_bounds__(kThreads)
         xv = csub(xv, c.q);
         yv = csub(yv, c.q);
       }
-      r.v[k] = mulmod(xv, yv, c);
+      r.v[k] = mulmod<WIDE>(xv, yv, c);
     }
     st_slots<VEC>(result + i * VEC, r);
   }
@@ -185,6 +188,13 @@ __global__ void __launch_bounds__(kThreads)
 
 unsigned blocks_for(u64 items) { return (unsigned)((items + kThreads - 1) / kThreads); }
 
+// the block needs mulmod<true>: one of its moduli has 62 bits (shift = bits(q) - 2 = 60)
+bool has_62_bit_modulus(const DyadicModuli& mods, u64 count) {
+  for (u64 e = 0; e < count; ++e)
+    if (mods.m[e].shift == 60) return true;
+  return false;
+}
+
 }  // namespace
 
 cudaError_t launch_dyadic_multiply(u64* result, const u64* op1, const u64* op2, u64 n, u64 num_moduli, u64 first,
@@ -199,10 +209,9 @@ cudaError_t launch_dyadic_multiply(u64* result, const u64* op1, const u64* op2, 
                      reinterpret_cast<uintptr_t>(op2)) & 15) == 0;
   u64 blocks = blocks_for(vec ? total / 2 : total);
   if (blocks > (u64)sms * 16) blocks = (u64)sms * 16;
-  if (vec)
-    dyadic_kernel<2><<<(unsigned)blocks, kThreads, 0, stream>>>(result, op1, op2, n, num_moduli, first, count, mods);
-  else
-    dyadic_kernel<1><<<(unsigned)blocks, kThreads, 0, stream>>>(result, op1, op2, n, num_moduli, first, count, mods);
+  auto kernel = vec ? dyadic_kernel<2, false> : dyadic_kernel<1, false>;
+  if (has_62_bit_modulus(mods, count)) kernel = vec ? dyadic_kernel<2, true> : dyadic_kernel<1, true>;
+  kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(result, op1, op2, n, num_moduli, first, count, mods);
   count_launch();
   return cudaGetLastError();
 }
@@ -218,10 +227,10 @@ cudaError_t launch_rns_eltwise(int op, u64* result, const u64* a, const u64* b, 
                    ((reinterpret_cast<uintptr_t>(result) | reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0;
   u64 blocks = blocks_for(vec ? total / 2 : total);
   if (blocks > (u64)sms * 16) blocks = (u64)sms * 16;
-  if (vec)
-    rns_eltwise_kernel<2><<<(unsigned)blocks, kThreads, 0, stream>>>(result, a, b, per_mod, count, op, in_mf, mods);
-  else
-    rns_eltwise_kernel<1><<<(unsigned)blocks, kThreads, 0, stream>>>(result, a, b, per_mod, count, op, in_mf, mods);
+  auto kernel = vec ? rns_eltwise_kernel<2, false> : rns_eltwise_kernel<1, false>;
+  if (op == kRnsMult && has_62_bit_modulus(mods, count))
+    kernel = vec ? rns_eltwise_kernel<2, true> : rns_eltwise_kernel<1, true>;
+  kernel<<<(unsigned)blocks, kThreads, 0, stream>>>(result, a, b, per_mod, count, op, in_mf, mods);
   count_launch();
   return cudaGetLastError();
 }

@@ -501,6 +501,9 @@ inline void EltwiseSubMod(uint64_t* result, const uint64_t* operand1, uint64_t o
   b200_detail::Throw(hexl_b200_eltwise_sub_mod_scalar(result, operand1, operand2, n, modulus, stream));
 }
 // hexl/include/hexl/eltwise/eltwise-mult-mod.hpp:23
+// Exact for every accepted input (q < 2^62, input_mod_factor * q < 2^63).  For 62-bit moduli the generalised Barrett
+// quotient estimate can be low by two and the product takes a second conditional subtraction; the reference's scalar
+// tier takes one and returns words in [q, 2q) for some operands near q at some moduli above about 2^61.7.
 inline void EltwiseMultMod(uint64_t* result, const uint64_t* operand1, const uint64_t* operand2, uint64_t n,
                            uint64_t modulus, uint64_t input_mod_factor, void* stream = nullptr) {
   b200_detail::Throw(hexl_b200_eltwise_mult_mod(result, operand1, operand2, n, modulus, input_mod_factor, stream));
@@ -511,6 +514,8 @@ inline void EltwiseFMAMod(uint64_t* result, const uint64_t* arg1, uint64_t arg2,
   b200_detail::Throw(hexl_b200_eltwise_fma_mod(result, arg1, arg2, arg3, n, modulus, input_mod_factor, stream));
 }
 // hexl/include/hexl/eltwise/eltwise-reduce-mod.hpp:24
+// Exact for every modulus above 1.  For q >= 2^63 every 64-bit word is below 2q, so input_mod_factor 4 is treated as
+// 2; every tier of the reference subtracts 2q there, which wraps.
 inline void EltwiseReduceMod(uint64_t* result, const uint64_t* operand, uint64_t n, uint64_t modulus,
                              uint64_t input_mod_factor, uint64_t output_mod_factor, void* stream = nullptr) {
   b200_detail::Throw(
@@ -557,6 +562,8 @@ inline void EltwiseMontgomeryFormOut(uint64_t* result, const uint64_t* a, uint64
 inline NTT GetNTT(size_t N, uint64_t modulus) { return NTT::FromCache(N, modulus); }
 
 // hexl/include/hexl/experimental/seal/dyadic-multiply.hpp:26
+// Exact for every modulus below 2^62, like EltwiseMultMod: for 62-bit moduli the products take the second conditional
+// subtraction the reference's scalar tier lacks.
 inline void DyadicMultiply(uint64_t* result, const uint64_t* operand1, const uint64_t* operand2, uint64_t n,
                            const uint64_t* moduli, uint64_t num_moduli, void* stream = nullptr) {
   b200_detail::Throw(hexl_b200_dyadic_multiply(result, operand1, operand2, n, moduli, num_moduli, stream));

@@ -186,7 +186,11 @@ int hexl_b200_eltwise_sub_mod(uint64_t* result, const uint64_t* operand1,
 int hexl_b200_eltwise_sub_mod_scalar(uint64_t* result, const uint64_t* operand1,
                                      uint64_t operand2, uint64_t n, uint64_t modulus,
                                      void* stream);
-/* EltwiseMultMod, eltwise-mult-mod.hpp:23; in_mf in {1,2,4} */
+/* EltwiseMultMod, eltwise-mult-mod.hpp:23; in_mf in {1,2,4}, q < 2^62, in_mf * q < 2^63.
+ * Exact for every accepted input; the same holds for hexl_b200_eltwise_mult_mod_multi and
+ * hexl_b200_dyadic_multiply.  For 62-bit moduli the generalised Barrett quotient estimate can be low
+ * by two and the product takes a second conditional subtraction; the reference's scalar tier takes one
+ * and returns words in [q, 2q) for some operands near q at some moduli above about 2^61.7. */
 int hexl_b200_eltwise_mult_mod(uint64_t* result, const uint64_t* operand1,
                                const uint64_t* operand2, uint64_t n, uint64_t modulus,
                                uint64_t input_mod_factor, void* stream);
@@ -194,7 +198,9 @@ int hexl_b200_eltwise_mult_mod(uint64_t* result, const uint64_t* operand1,
 int hexl_b200_eltwise_fma_mod(uint64_t* result, const uint64_t* arg1, uint64_t arg2,
                               const uint64_t* arg3, uint64_t n, uint64_t modulus,
                               uint64_t input_mod_factor, void* stream);
-/* EltwiseReduceMod, eltwise-reduce-mod.hpp:24; in_mf in {modulus,2,4}, out_mf in {1,2} */
+/* EltwiseReduceMod, eltwise-reduce-mod.hpp:24; in_mf in {modulus,2,4}, out_mf in {1,2}.
+ * Exact for every q > 1.  For q >= 2^63 every 64-bit word is below 2q and in_mf 4 is treated as 2;
+ * every tier of the reference subtracts 2q there, which wraps. */
 int hexl_b200_eltwise_reduce_mod(uint64_t* result, const uint64_t* operand, uint64_t n,
                                  uint64_t modulus, uint64_t input_mod_factor,
                                  uint64_t output_mod_factor, void* stream);

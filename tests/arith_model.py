@@ -167,13 +167,14 @@ def reduce_from(x, q, k):
 
 
 def eltwise_mult(a, b, q, in_mf):
+    """z < 2q while bits(q) <= 61; at 62 bits (shift = 60) z < 3q and a second conditional subtraction follows"""
     x, y = reduce_from(a, q, in_mf), reduce_from(b, q, in_mf)
     pmu, shift = prod_constants(q)
     u = x * y
     lo, hi = u & M64, u >> 64
     c1 = ((lo >> shift) | (hi << (64 - shift))) & M64 if shift else lo
-    z = (lo - mulhi(c1, pmu) * q) & M64
-    return csub(z, q)
+    z = csub((lo - mulhi(c1, pmu) * q) & M64, q)
+    return csub(z, q) if shift == 60 else z
 
 
 # ---- key-switch glue (seal.cu)

@@ -6,6 +6,7 @@ import random
 import pytest
 
 import arith_model as am
+from eltwise_exact import BARRETT_62_BIT_WITNESSES
 
 M64 = am.M64
 
@@ -79,12 +80,16 @@ def test_sign_bit_conditional_subtraction():
             assert am.csub_s(x, b) == am.csub(x, b)
 
 
-@pytest.mark.parametrize("lo_bits,hi_bits,approx,out_bound_q", [(32, 56, True, 4), (56, 61, True, 4), (3, 62, False, 2)])
+@pytest.mark.parametrize("lo_bits,hi_bits,approx,out_bound_q",
+                         [(32, 56, True, 4), (56, 61, True, 4), (3, 61, False, 2), (61, 62, False, 3)])
 def test_product_multiplied_on_load_ranges(lo_bits, hi_bits, approx, out_bound_q):
-    """prod_lazy: canonical operands -> [0,2q) with the exact quotient, [0,4q) with the three-product estimate;
-    the 128-bit product and the shifted word c1 are formed without losing bits for every q < 2^62."""
+    """prod_lazy: canonical operands -> [0,2q) with the exact quotient for every q < 2^61 (all PolyMultiplyMulti
+    accepts), [0,4q) with the three-product estimate; at 62 bits the exact quotient's estimate can be low by two, so
+    only [0,3q) holds.  The 128-bit product and the shifted word c1 are formed without losing
+    bits for every q < 2^62."""
     rng = random.Random(5)
-    for q in _moduli(lo_bits, hi_bits, rng, 8):
+    witnesses = [q for q in BARRETT_62_BIT_WITNESSES if (1 << lo_bits) <= q < (1 << hi_bits)]
+    for q in _moduli(lo_bits, hi_bits, rng, 8) + witnesses:
         for x in _operands(q, rng, 40):
             for y in _operands(q, rng, 40):
                 r = am.prod_lazy(x, y, q, approx)
@@ -145,15 +150,18 @@ def test_montgomery_reduction(r):
 
 @pytest.mark.parametrize("in_mf", [1, 2, 4])
 def test_eltwise_generalised_barrett(in_mf):
+    """exact for every q < 2^62 with in_mf * q < 2^63, the 62-bit witnesses included, where operands within 2^20 of q
+    need the second conditional subtraction"""
     rng = random.Random(8)
-    qs = [3, 5, 65537, (1 << 40) + 15, (1 << 50) - 27, (1 << 60) - 93, (1 << 61) - 1]
-    if in_mf == 1:
-        qs.append((1 << 62) - 57)
+    qs = [3, 5, 65537, (1 << 40) + 15, (1 << 50) - 27, (1 << 60) - 93, (1 << 61) - 1, (1 << 62) - 57]
+    qs += list(BARRETT_62_BIT_WITNESSES)
     for q in qs:
-        assert in_mf * q < (1 << 63)
-        for a in _operands(in_mf * q, rng, 40):
-            for b in _operands(in_mf * q, rng, 40):
-                assert am.eltwise_mult(a, b, q, in_mf) == (a * b) % q
+        if in_mf * q >= (1 << 63):
+            continue
+        band = [q - 1 - rng.randrange(min(q, 1 << 20)) for _ in range(40)]
+        for a in _operands(in_mf * q, rng, 40) + band:
+            for b in _operands(in_mf * q, rng, 40) + band:
+                assert am.eltwise_mult(a, b, q, in_mf) == (a * b) % q, (a, b, q)
 
 
 def test_key_switch_mac_chunk_never_wraps():
