@@ -177,12 +177,12 @@ cudaError_t launch_pipe_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* 
 }
 
 // log2(N / 4096) for which the pipelined kernel is used; 0 = none.  HEXL_B200_PIPE: 1 = always (N = 2^14..2^17),
-// 0 = never, unset = the 64-bit modes' forward at N = 2^17.  One H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit q
-// (tools/tune_split.py, ms, pipelined vs the two-kernel split), with the coefficient arrays in registers: N = 2^17
-// forward 3.10 vs 3.67, inverse 3.58 vs 3.71; N = 2^16 forward 2.86 vs 3.47, inverse 3.51 vs 3.71.  (Before, with
-// the arrays in local memory: 2^17 forward 14.9 vs 17.2, inverse 15.5 vs 15.4.)  The N = 2^16 defaults stay the
-// split until the gain is confirmed on the benchmark's whole step.  32-bit words use the distributed-shared-memory
-// kernel instead (dsmem_log_r).  A batch of fewer polynomials than the pipeline is deep gains nothing from it.
+// 0 = never, unset = the 64-bit modes' forward at N = 2^15..2^17.  One H100 80GB HBM3 (power limit not recorded), 2^28
+// coefficients, 55-bit q (tools/tune_split.py, ms, pipelined vs the two-kernel split), with the coefficient arrays in
+// registers: N = 2^17 forward 3.10 vs 3.67, inverse 3.58 vs 3.71.  (Before, with the arrays in local memory: 2^17
+// forward 14.9 vs 17.2, inverse 15.5 vs 15.4.)  At N = 2^14..2^16 see dsmem_log_r for every candidate: the pipelined
+// forward is the fastest at 2^15 and 2^16, its inverse never is.  32-bit words use the distributed-shared-memory
+// kernel instead.  A batch of fewer polynomials than the pipeline is deep gains nothing from it.
 template <int MODE>
 inline int pipe_log_r(int log_n, u64 batch, bool forward) {
   static const int mode = env_int("HEXL_B200_PIPE", -1);
@@ -190,15 +190,15 @@ inline int pipe_log_r(int log_n, u64 batch, bool forward) {
   const int lr = log_n - 12;
   if (mode == 0 || lr < 2 || lr > 5 || batch < (u64)min_batch || batch >= (1ull << 31)) return 0;
   if (mode > 0) return lr;
-  const bool wins = MODE != kSmall && forward && log_n == 17;
+  const bool wins = MODE != kSmall && forward && log_n >= 15;
   return wins ? lr : 0;
 }
 
-// SMALL mode: the single kernel that keeps the intermediate in the cluster's shared memory
-template <int LOGR>
+// The single kernel that keeps the intermediate in the cluster's shared memory
+template <int MODE, int LOGR>
 cudaError_t launch_dsmem(bool fwd, const NttDeviceTables& t, u64* result, const u64* operand, u64 batch, int out_mf,
                          cudaStream_t stream) {
-  using Cfg = DsmemCfg<LOGR>;
+  using Cfg = DsmemCfg<LOGR, MODE>;
   const Mod m = make_mod(t);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(batch * Cfg::K));
@@ -214,49 +214,72 @@ cudaError_t launch_dsmem(bool fwd, const NttDeviceTables& t, u64* result, const 
   cfg.numAttrs = 1;
   cudaError_t e;
   if (fwd) {
-    if ((e = ensure_dynamic_smem<ntt_dsmem_fwd<LOGR>>(Cfg::SMEM)) != cudaSuccess) return e;
-    e = cudaLaunchKernelEx(&cfg, ntt_dsmem_fwd<LOGR>, result, operand, t.fwd32, m, out_mf);
+    if ((e = ensure_dynamic_smem<ntt_dsmem_fwd<MODE, LOGR>>(Cfg::SMEM)) != cudaSuccess) return e;
+    e = cudaLaunchKernelEx(&cfg, ntt_dsmem_fwd<MODE, LOGR>, result, operand, Tab<MODE>::fwd(t), m, out_mf);
   } else {
-    if ((e = ensure_dynamic_smem<ntt_dsmem_inv<LOGR>>(Cfg::SMEM)) != cudaSuccess) return e;
-    e = cudaLaunchKernelEx(&cfg, ntt_dsmem_inv<LOGR>, result, operand, t.inv32, m, out_mf, t.inv_n32, t.inv_n_w32);
+    if ((e = ensure_dynamic_smem<ntt_dsmem_inv<MODE, LOGR>>(Cfg::SMEM)) != cudaSuccess) return e;
+    e = cudaLaunchKernelEx(&cfg, ntt_dsmem_inv<MODE, LOGR>, result, operand, Tab<MODE>::inv(t), m, out_mf,
+                           Tab<MODE>::inv_n(t), Tab<MODE>::inv_n_w(t));
   }
   count_launch();
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 
+template <int MODE>
 cudaError_t launch_dsmem_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* result, const u64* operand,
                              u64 batch, int out_mf, cudaStream_t stream) {
   switch (log_r) {
-    case 2: return launch_dsmem<2>(fwd, t, result, operand, batch, out_mf, stream);
-    case 3: return launch_dsmem<3>(fwd, t, result, operand, batch, out_mf, stream);
-    case 4: return launch_dsmem<4>(fwd, t, result, operand, batch, out_mf, stream);
-    case 5: return launch_dsmem<5>(fwd, t, result, operand, batch, out_mf, stream);
+    case 2: return launch_dsmem<MODE, 2>(fwd, t, result, operand, batch, out_mf, stream);
+    case 3: return launch_dsmem<MODE, 3>(fwd, t, result, operand, batch, out_mf, stream);
+  }
+  if constexpr (MODE == kSmall) {
+    if (log_r == 4) return launch_dsmem<MODE, 4>(fwd, t, result, operand, batch, out_mf, stream);
+    if (log_r == 5) return launch_dsmem<MODE, 5>(fwd, t, result, operand, batch, out_mf, stream);
   }
   return cudaErrorInvalidValue;
 }
 
-// log2(N / 4096) for which the distributed-shared-memory kernel is used (SMALL mode); 0 = none.
+// log2(N / 4096) for which the distributed-shared-memory kernel is used; 0 = none.  HEXL_B200_DSMEM=0 disables it.
+// SMALL mode (32-bit words):
 // One H100 SXM at 400 W, 2^28 coefficients, 29-bit q, forward / inverse ms vs the cluster kernel that keeps the
 // intermediate in L2: N = 2^14 6.41 / 6.69 vs 6.90 / 7.26, 2^15 6.42 / 6.77 vs 6.83 / 7.29, 2^16 7.54 / 7.84 vs
 // 7.99 / 8.15, 2^17 7.81 / 8.10 vs 8.25 / 8.42 (and vs 7.79 / 8.23, 8.10 / 8.30 for the pipelined kernel at 2^16 /
-// 2^17), so it is the default at every size (HEXL_B200_DSMEM=0 disables it).  Re-timed on an H100 80GB HBM3 (power
-// limit not recorded) with the coefficient arrays
-// in registers: N = 2^16 1.76 / 1.79 vs 1.97 / 1.94, 2^17 1.94 / 2.08 vs 2.22 / 2.13 (pipelined 2.05 / 2.15).
+// 2^17), so it is the default at every size.  Re-timed on an H100 80GB HBM3 (power limit not recorded) with the
+// coefficient arrays in registers: N = 2^16 1.76 / 1.79 vs 1.97 / 1.94, 2^17 1.94 / 2.08 vs 2.22 / 2.13 (pipelined
+// 2.05 / 2.15).
+// 64-bit words, one H100 80GB HBM3 at 700 W (1980 MHz maximum SM clock), 2^28 coefficients, q of 55 (FAST) / 60 (WIDE)
+// / 61 (GENERIC) bits, forward / inverse ms, this kernel | the fused kernel through L2 | pipelined | two-kernel split:
+//   N = 2^14  FAST 2.96 / 2.75 | 3.01 / 2.90 | 3.20 / 5.92 | 3.49 / 3.71   WIDE 3.45 / 3.24 | 3.28 / 3.32 | 3.43 / 6.26
+//             GENERIC 3.35 / 3.37 | 3.41 / 3.57 | 3.48 / 6.54
+//   N = 2^15  FAST 3.02 / 2.93 | 3.04 / 2.93 | 2.95 / 4.38 | 3.49 / 3.73   WIDE 3.51 / 3.43 | 3.35 / 3.47 | 3.24 / 4.70
+//             GENERIC 3.46 / 3.60 | 3.46 / 3.67 | 3.28 / 4.98
+//   N = 2^16  FAST 3.23 / 3.43 | 3.07 / 3.13 | 2.88 / 3.54 | 3.49 / 3.73   WIDE 3.57 / 4.01 | 3.41 / 3.56 | 3.26 / 3.87
+//             GENERIC 3.71 / 4.20 | 3.54 / 3.82 | 3.27 / 4.07
+// So the 64-bit modes use it at N = 2^14 (except where the WIDE forward is 5 % behind the fused kernel, kept for one
+// rule per size) and for the 2^15 inverse (the 2^15 forward takes the pipelined kernel when the batch is deep enough
+// for it, this one otherwise).  At 2^16 it loses both ways -- its column phase stores to the peers' shared memory in
+// 8-byte words, and each CTA's phases are serialised at the cluster barrier -- to the pipelined forward and the fused
+// inverse.  On the benchmark's step (8192 polynomials at 2^16, 55-bit) this kernel in both directions took 13.2 ms
+// against 14.4 ms for the split.
+template <int MODE>
 int dsmem_log_r(int log_n) {
   static const int mode = env_int("HEXL_B200_DSMEM", 1);
   const int lr = log_n - DsmemCfg<2>::LOGC;
-  return (mode != 0 && lr >= 2 && lr <= 5) ? lr : 0;
+  if (mode == 0 || lr < 2) return 0;
+  if constexpr (MODE == kSmall) return lr <= 5 ? lr : 0;
+  return lr <= 3 ? lr : 0;
 }
 
-// log2(N / 4096) for which the single fused kernel is used; 0 = none.  Off by default for the 64-bit modes
-// (HEXL_B200_FUSED=1 enables it).  One H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit q, coefficient arrays in
-// registers, ms vs the default path: N = 2^16 forward 3.04 vs 3.47, inverse 3.10 vs 3.71; N = 2^17 inverse 3.91 vs
-// 3.71.  Like the pipelined N = 2^16 forward, the 2^16 gain is not yet confirmed on the benchmark's whole step.
+// log2(N / 4096) for which the single fused kernel is used; 0 = none.  The 64-bit modes use it at N = 2^16 (the
+// inverse, and the forward of batches too shallow for the pipelined kernel; timings at dsmem_log_r);
+// HEXL_B200_FUSED=1 enables it at N = 2^14..2^17, 0 disables it.  One H100 80GB HBM3 (power limit not recorded),
+// 2^28 coefficients, 55-bit q: N = 2^17 inverse 3.91 vs 3.71 ms for the split.
 template <int MODE>
 int fused_log_r(int log_n) {
-  static const bool enabled = MODE == kSmall ? env_int("HEXL_B200_FUSED_SMALL", 1) != 0 : env_int("HEXL_B200_FUSED", 0) != 0;
+  static const int mode = MODE == kSmall ? env_int("HEXL_B200_FUSED_SMALL", 1) : env_int("HEXL_B200_FUSED", -1);
   const int lr = log_n - FusedCfg<2>::LOGC;
-  return (enabled && lr >= 2 && lr <= 5) ? lr : 0;
+  if (mode == 0 || lr < 2 || lr > 5) return 0;
+  return (mode > 0 || log_n == 16) ? lr : 0;
 }
 
 template <int MODE>
@@ -275,8 +298,7 @@ template <int MODE>
 cudaError_t forward_impl(const NttDeviceTables& t, u64* result, const u64* operand, int out_mf,
                          u64 batch, cudaStream_t stream) {
   if (const int lr = pipe_log_r<MODE>(t.log_n, batch, true)) return launch_pipe_dyn<MODE>(lr, true, t, result, operand, batch, out_mf, stream);
-  if constexpr (MODE == kSmall)
-    if (const int lr = dsmem_log_r(t.log_n)) return launch_dsmem_dyn(lr, true, t, result, operand, batch, out_mf, stream);
+  if (const int lr = dsmem_log_r<MODE>(t.log_n)) return launch_dsmem_dyn<MODE>(lr, true, t, result, operand, batch, out_mf, stream);
   if (const int lr = fused_log_r<MODE>(t.log_n)) return launch_fused_dyn<MODE>(lr, true, t, result, operand, batch, out_mf, stream);
   const int log_c = pick_row_log(t.log_n);
   int radices[8];
@@ -296,8 +318,7 @@ template <int MODE>
 cudaError_t inverse_impl(const NttDeviceTables& t, u64* result, const u64* operand, int out_mf,
                          u64 batch, cudaStream_t stream) {
   if (const int lr = pipe_log_r<MODE>(t.log_n, batch, false)) return launch_pipe_dyn<MODE>(lr, false, t, result, operand, batch, out_mf, stream);
-  if constexpr (MODE == kSmall)
-    if (const int lr = dsmem_log_r(t.log_n)) return launch_dsmem_dyn(lr, false, t, result, operand, batch, out_mf, stream);
+  if (const int lr = dsmem_log_r<MODE>(t.log_n)) return launch_dsmem_dyn<MODE>(lr, false, t, result, operand, batch, out_mf, stream);
   if (const int lr = fused_log_r<MODE>(t.log_n)) return launch_fused_dyn<MODE>(lr, false, t, result, operand, batch, out_mf, stream);
   const int log_c = pick_row_log(t.log_n);
   int radices[8];

@@ -712,7 +712,9 @@ struct RowCfg {
 // Global-memory access policies for coefficients.  Streaming (evict-first) for
 // data touched once; L2 variants for the intermediate a fused kernel hands from
 // its column phase to its row phase (written by one CTA, read by another).
-enum : int { kStream = 0, kViaL2 = 1, kSmemRow = 2 };  // kSmemRow: the "global" side is a row of E in shared memory
+// kSmemRow: the "global" side is a row of E in shared memory; kSmemRowPad: the same in the padded layout of the 64-bit
+// exchanges (element j at j + j / 16), so that the row can double as its own exchange buffer
+enum : int { kStream = 0, kViaL2 = 1, kSmemRow = 2, kSmemRowPad = 3 };
 template <int POLICY>
 __device__ __forceinline__ u64 ld_coef(const u64* p) {
   return POLICY == kViaL2 ? __ldcg(p) : __ldcs(p);
@@ -730,6 +732,8 @@ template <int POLICY, typename E>
 __device__ __forceinline__ E ld_row(const void* base, unsigned idx) {
   if constexpr (POLICY == kSmemRow)
     return static_cast<const E*>(base)[idx];
+  else if constexpr (POLICY == kSmemRowPad)
+    return static_cast<const E*>(base)[idx + (idx >> 4)];
   else
     return (E)ld_coef<POLICY>(static_cast<const u64*>(base) + idx);
 }
@@ -737,6 +741,8 @@ template <int POLICY, typename E>
 __device__ __forceinline__ void st_row(void* base, unsigned idx, E v) {
   if constexpr (POLICY == kSmemRow)
     static_cast<E*>(base)[idx] = v;
+  else if constexpr (POLICY == kSmemRowPad)
+    static_cast<E*>(base)[idx + (idx >> 4)] = v;
   else
     st_coef<POLICY>(static_cast<u64*>(base) + idx, v);
 }
@@ -769,7 +775,7 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
     else
       v[e] = ld_row<LD, E>(in, reg_index<LB0>(u, e));
   });
-  if constexpr (LD != kSmemRow && sizeof(E) == 8) {
+  if constexpr (LD < kSmemRow && sizeof(E) == 8) {
     if (reduce_in) {  // NttMulti::gather: the input is a value of ANOTHER modulus
       static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = reduce_any(v[e], m); });
     }
@@ -815,7 +821,7 @@ __device__ __forceinline__ void row_inv_body(void* out, const void* in, typename
   constexpr int LB_IN = LB0 < 4 ? LB0 : 4;  // 16 lanes read one 128-byte line per instruction
   Tw* stab = cta_stab ? cta_stab : reinterpret_cast<Tw*>(srow + row_elems<E>(LOGC));
   static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, reg_index<LB_IN>(u, e)); });
-  if constexpr (LD != kSmemRow && sizeof(E) == 8) {
+  if constexpr (LD < kSmemRow && sizeof(E) == 8) {
     if (prod) {  // NttMulti::mul: the transform of a point-wise product, multiplied on load
       static_for<0, 16>([&](auto I) {
         constexpr int e = I;
@@ -1207,15 +1213,15 @@ __global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MO
 }
 
 // ------------------------------------- fused kernels through distributed shared memory
-// SMALL mode only (32-bit words): the whole polynomial fits in the shared memory of its
-// cluster -- N * 4 bytes spread over K CTAs -- so the intermediate between the column phase
-// and the row phase never leaves the SMs.  CTA `rank` owns rows rank, rank + K, ... of the
-// R x 4096 matrix.  Forward: the column phase of every CTA scatters its results straight
-// into the owners' shared memory (st.shared::cluster, 128 contiguous bytes per warp and
-// row), one cluster barrier, then every CTA transforms its own rows from local shared
-// memory to HBM.  Inverse: rows first into local shared memory, barrier, the column phase
-// gathers from the owners (ld.shared::cluster), a last barrier keeps every CTA's memory
-// alive until its peers have read it.  HBM sees 8N bytes in and 8N bytes out, L2 nothing.
+// The whole polynomial fits in the shared memory of its cluster -- N words spread over K CTAs
+// -- so the intermediate between the column phase and the row phase never leaves the SMs.
+// CTA `rank` owns rows rank, rank + K, ... of the R x 4096 matrix.  Forward: the column
+// phase of every CTA scatters its results straight into the owners' shared memory
+// (st.shared::cluster, 128 or 256 contiguous bytes per warp and row), one cluster barrier,
+// then every CTA transforms its own rows from local shared memory to HBM.  Inverse: rows
+// first into local shared memory, barrier, the column phase gathers from the owners
+// (ld.shared::cluster), a last barrier keeps every CTA's memory alive until its peers have
+// read it.  HBM sees 8N bytes in and 8N bytes out, L2 nothing.
 __device__ __forceinline__ unsigned dsmem_address(const void* local_smem, unsigned cta_rank) {
   const unsigned a = (unsigned)__cvta_generic_to_shared(local_smem);
   unsigned r;
@@ -1225,32 +1231,60 @@ __device__ __forceinline__ unsigned dsmem_address(const void* local_smem, unsign
 __device__ __forceinline__ void dsmem_store(unsigned addr, unsigned v) {
   asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
-__device__ __forceinline__ unsigned dsmem_load(unsigned addr) {
-  unsigned v;
-  asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+__device__ __forceinline__ void dsmem_store(unsigned addr, u64 v) {
+  asm volatile("st.shared::cluster.u64 [%0], %1;" ::"r"(addr), "l"(v) : "memory");
+}
+template <typename E>
+__device__ __forceinline__ E dsmem_load(unsigned addr) {
+  E v;
+  if constexpr (sizeof(E) == 8)
+    asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(addr) : "memory");
+  else
+    asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
 
-template <int LOGR>
+// K = min(R, 8) CTAs per cluster (8 is the portable maximum), R / K rows each.  32-bit words: the owned rows are
+// unpadded and the row phase has one exchange buffer of its own.  64-bit words: the owned rows are stored in the
+// padded layout of the row kernels' exchanges, and each row is its own exchange buffer once it is in registers, so
+// even two rows per CTA (N = 2^16: 72 KiB with the twiddle tables; 106 KiB with a separate buffer) leave room for the
+// 3 CTAs per SM the 64-bit row kernels are tuned to.  One 64-bit row per CTA in clusters of 16 (non-portable) fits
+// 3 CTAs per SM as well, but an H100 80GB HBM3 (400 W) schedules only 21 such clusters (336 of 396 CTA slots,
+// cudaOccupancyMaxActiveClusters) against 45 clusters of 8, and at N = 2^16, 55-bit q, 2^28 coefficients, it took
+// 3.86 / 4.27 ms forward / inverse against 3.97 / 4.36 for the two-kernel split.  ntt.cu (dsmem_log_r) launches the
+// 64-bit kernels at N = 2^14 and 2^15 only.
+template <int LOGR, int MODE = kSmall>
 struct DsmemCfg {
+  using E = typename Ar<MODE>::E;
+  using Tw = typename Ar<MODE>::Tw;
   static constexpr int LOGC = 12, C = 1 << LOGC, R = 1 << LOGR;
   static constexpr int K = R < 8 ? R : 8;            // CTAs per cluster
   static constexpr int RPC = R / K;                  // rows owned by one CTA
   static constexpr int THREADS = 256;
   static constexpr int COLS = C / K;                 // columns one CTA runs in the column phase
-  // owned rows + exchange buffer (32-bit words) + the row kernel's twiddle tables
-  static constexpr size_t SMEM = (size_t)(RPC + 1) * C * sizeof(unsigned) + kRowTwEntries * sizeof(Twiddle32);
-  static constexpr int MIN_BLOCKS = SMEM <= 56 * 1024 ? 4 : (SMEM <= 75 * 1024 ? 3 : 2);
+  static constexpr bool PAD = sizeof(E) == 8;        // owned rows in the padded exchange layout
+  static constexpr int ROW_POLICY = PAD ? kSmemRowPad : kSmemRow;
+  static constexpr unsigned ROW = row_elems<E>(LOGC);  // elements from one owned row to the next
+  // owned rows (+ the exchange buffer of 32-bit words) + the row kernel's twiddle tables
+  static constexpr size_t SMEM = (size_t)(RPC + (PAD ? 0 : 1)) * ROW * sizeof(E) + kRowTwEntries * sizeof(Tw);
+  // 64-bit words: the row kernels' 3 CTAs per SM (80 registers) at every R
+  static constexpr int MIN_BLOCKS = PAD ? HEXL_B200_ROW_MIN_BLOCKS : (SMEM <= 56 * 1024 ? 4 : (SMEM <= 75 * 1024 ? 3 : 2));
+  // where coefficient j of an owned row is stored
+  static __device__ __forceinline__ unsigned slot(unsigned j) { return PAD ? j + (j >> 4) : j; }
 };
 
-template <int LOGR>
-__global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_BLOCKS)
-    ntt_dsmem_fwd(u64* result, const u64* operand, const Twiddle32* __restrict__ tw, const Mod m, int out_mf) {
-  using Cfg = DsmemCfg<LOGR>;
+template <int MODE, int LOGR>
+__global__ void __launch_bounds__(DsmemCfg<LOGR, MODE>::THREADS, DsmemCfg<LOGR, MODE>::MIN_BLOCKS)
+    ntt_dsmem_fwd(u64* result, const u64* operand, const typename Ar<MODE>::Tw* __restrict__ tw, const Mod m,
+                  int out_mf) {
+  using Cfg = DsmemCfg<LOGR, MODE>;
+  using E = typename Ar<MODE>::E;
+  using Tw = typename Ar<MODE>::Tw;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  unsigned* rows = reinterpret_cast<unsigned*>(smem_raw);  // [RPC][C]
-  unsigned* xbuf = rows + Cfg::RPC * Cfg::C;               // exchange buffer, twiddle tables behind it
-  __shared__ Twiddle32 stw[Cfg::R];
+  E* rows = reinterpret_cast<E*>(smem_raw);  // [RPC][ROW]
+  E* xbuf = rows + Cfg::RPC * Cfg::ROW;      // 32-bit words: exchange buffer, twiddle tables behind it
+  Tw* const ctab = Cfg::PAD ? reinterpret_cast<Tw*>(xbuf) : nullptr;  // 64-bit words: the twiddle tables
+  __shared__ Tw stw[Cfg::R];
   const unsigned rank = blockIdx.x % Cfg::K;
   const u64 poly_off = (u64)(blockIdx.x / Cfg::K) << (Cfg::LOGC + LOGR);
   // a CTA's shared memory may only be written by its peers once it is known to be running:
@@ -1266,15 +1300,15 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_B
 #pragma unroll 1
   for (int c = threadIdx.x; c < Cfg::COLS; c += Cfg::THREADS) {
     const unsigned col = rank * Cfg::COLS + c;
-    unsigned v[Cfg::R];
+    E v[Cfg::R];
     static_for<0, Cfg::R>([&](auto I) {
       constexpr int e = I;
-      v[e] = (unsigned)ld_coef<kStream>(operand + poly_off + ((u64)e << Cfg::LOGC) + col);
+      v[e] = (E)ld_coef<kStream>(operand + poly_off + ((u64)e << Cfg::LOGC) + col);
     });
-    col_stages<kSmall, LOGR, true>(v, stw, m, false, Twiddle32{}, Twiddle32{});
+    col_stages<MODE, LOGR, true>(v, stw, m, false, Tw{}, Tw{});
     static_for<0, Cfg::R>([&](auto I) {  // row e lives in CTA e % K, slot e / K
       constexpr int e = I;
-      dsmem_store(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::C + col) * 4u, v[e]);
+      dsmem_store(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::ROW + Cfg::slot(col)) * (unsigned)sizeof(E), v[e]);
     });
   }
   cluster_barrier();
@@ -1282,21 +1316,26 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_B
 #pragma unroll 1
   for (int lr = 0; lr < Cfg::RPC; ++lr) {
     const unsigned r = rank + lr * Cfg::K;
-    row_fwd_body<kSmall, Cfg::LOGC, kSmemRow, kStream>(result + poly_off + (u64)r * Cfg::C, rows + lr * Cfg::C, xbuf,
-                                                       threadIdx.x, (u64)Cfg::R + r, tw, m, out_mf, true);
+    E* row = rows + lr * Cfg::ROW;
+    row_fwd_body<MODE, Cfg::LOGC, Cfg::ROW_POLICY, kStream>(result + poly_off + (u64)r * Cfg::C, row,
+                                                            Cfg::PAD ? row : xbuf, threadIdx.x, (u64)Cfg::R + r, tw, m,
+                                                            out_mf, true, ctab);
     if (lr + 1 < Cfg::RPC) __syncthreads();  // the next row reuses the exchange buffer and tables
   }
 }
 
-template <int LOGR>
-__global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_BLOCKS)
-    ntt_dsmem_inv(u64* result, const u64* operand, const Twiddle32* __restrict__ tw, const Mod m, int out_mf,
-                  Twiddle32 inv_n, Twiddle32 inv_n_w) {
-  using Cfg = DsmemCfg<LOGR>;
+template <int MODE, int LOGR>
+__global__ void __launch_bounds__(DsmemCfg<LOGR, MODE>::THREADS, DsmemCfg<LOGR, MODE>::MIN_BLOCKS)
+    ntt_dsmem_inv(u64* result, const u64* operand, const typename Ar<MODE>::Tw* __restrict__ tw, const Mod m,
+                  int out_mf, typename Ar<MODE>::Tw inv_n, typename Ar<MODE>::Tw inv_n_w) {
+  using Cfg = DsmemCfg<LOGR, MODE>;
+  using E = typename Ar<MODE>::E;
+  using Tw = typename Ar<MODE>::Tw;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  unsigned* rows = reinterpret_cast<unsigned*>(smem_raw);
-  unsigned* xbuf = rows + Cfg::RPC * Cfg::C;
-  __shared__ Twiddle32 stw[Cfg::R];
+  E* rows = reinterpret_cast<E*>(smem_raw);
+  E* xbuf = rows + Cfg::RPC * Cfg::ROW;
+  Tw* const ctab = Cfg::PAD ? reinterpret_cast<Tw*>(xbuf) : nullptr;
+  __shared__ Tw stw[Cfg::R];
   const unsigned rank = blockIdx.x % Cfg::K;
   const u64 poly_off = (u64)(blockIdx.x / Cfg::K) << (Cfg::LOGC + LOGR);
   for (int l = threadIdx.x; l < Cfg::R; l += Cfg::THREADS)
@@ -1305,9 +1344,12 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_B
 #pragma unroll 1
   for (int lr = 0; lr < Cfg::RPC; ++lr) {
     const unsigned r = rank + lr * Cfg::K;
-    row_inv_body<kSmall, Cfg::LOGC, kStream, kSmemRow>(rows + lr * Cfg::C, operand + poly_off + (u64)r * Cfg::C, xbuf,
-                                                       threadIdx.x, (u64)Cfg::R + r, tw, m, out_mf, false, inv_n,
-                                                       inv_n_w, true);
+    // 64-bit words: the row is its own exchange buffer; the last exchange leaves every thread holding exactly the
+    // slots it then stores to, so no thread overwrites a slot another one has still to read
+    E* row = rows + lr * Cfg::ROW;
+    row_inv_body<MODE, Cfg::LOGC, kStream, Cfg::ROW_POLICY>(row, operand + poly_off + (u64)r * Cfg::C,
+                                                            Cfg::PAD ? row : xbuf, threadIdx.x, (u64)Cfg::R + r, tw, m,
+                                                            out_mf, false, inv_n, inv_n_w, true, ctab);
     __syncthreads();
   }
   cluster_barrier();
@@ -1317,12 +1359,12 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR>::THREADS, DsmemCfg<LOGR>::MIN_B
 #pragma unroll 1
   for (int c = threadIdx.x; c < Cfg::COLS; c += Cfg::THREADS) {
     const unsigned col = rank * Cfg::COLS + c;
-    unsigned v[Cfg::R];
+    E v[Cfg::R];
     static_for<0, Cfg::R>([&](auto I) {
       constexpr int e = I;
-      v[e] = dsmem_load(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::C + col) * 4u);
+      v[e] = dsmem_load<E>(owner_base[e % Cfg::K] + ((e / Cfg::K) * Cfg::ROW + Cfg::slot(col)) * (unsigned)sizeof(E));
     });
-    col_stages<kSmall, LOGR, false>(v, stw, m, true, inv_n, inv_n_w);
+    col_stages<MODE, LOGR, false>(v, stw, m, true, inv_n, inv_n_w);
     static_for<0, Cfg::R>([&](auto I) {
       constexpr int e = I;
       st_coef<kStream>(result + poly_off + ((u64)e << Cfg::LOGC) + col, inv_out(v[e], m, out_mf));
