@@ -18,12 +18,9 @@ from concurrent.futures import ThreadPoolExecutor
 PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
-# experiments: HEXL_B200_BUILD_SUFFIX=_x HEXL_B200_BUILD_FLAGS="-DFOO=1" builds lib/libhexl_b200_x.so
-SUFFIX = os.environ.get("HEXL_B200_BUILD_SUFFIX", "")
-EXTRA_FLAGS = os.environ.get("HEXL_B200_BUILD_FLAGS", "").split()
-OBJ = os.path.join(PKG, "_obj" + SUFFIX)
+OBJ = os.path.join(PKG, "_obj")
 LIB_DIR = os.path.join(PKG, "lib")
-LIB = os.path.join(LIB_DIR, f"libhexl_b200{SUFFIX}.so")
+LIB = os.path.join(LIB_DIR, "libhexl_b200.so")
 
 SOURCES = ["capi.cu", "ntt.cu", "ntt_multi.cu", "eltwise.cu", "seal.cu", "numtheory.cpp"]
 HEADERS = ["internal.h", "modarith.cuh", "ntt_kernels.cuh", "numtheory.h", os.path.join(ROOT, "include", "hexl_b200.h")]
@@ -56,7 +53,7 @@ def _compile(src: str, force: bool) -> str:
     deps = [path] + [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HEADERS]
     if not force and _newer(obj, deps):
         return obj
-    cmd = [nvcc()] + NVCC_FLAGS + EXTRA_FLAGS + ["-c", path, "-o", obj]
+    cmd = [nvcc()] + NVCC_FLAGS + ["-c", path, "-o", obj]
     res = subprocess.run(cmd, capture_output=True, text=True)
     with open(obj + ".log", "w") as f:  # ptxas -v output: registers / spills per kernel
         f.write(res.stdout + res.stderr)

@@ -1,6 +1,4 @@
 // Single-modulus NTT launchers (the kernels are in ntt_kernels.cuh).
-#include <algorithm>
-
 #include "ntt_kernels.cuh"
 
 namespace hexl_b200 {
@@ -36,7 +34,7 @@ cudaError_t launch_row_dyn(int log_c, bool fwd, const NttDeviceTables& t, u64* r
 #define ROW_CASE(L) \
   case L: return launch_row<MODE, L>(fwd, t, result, operand, batch, out_mf, fold, stream);
     ROW_CASE(4) ROW_CASE(5) ROW_CASE(6) ROW_CASE(7) ROW_CASE(8) ROW_CASE(9) ROW_CASE(10)
-    ROW_CASE(11) ROW_CASE(12) ROW_CASE(13) ROW_CASE(14)
+    ROW_CASE(11) ROW_CASE(12) ROW_CASE(13)
 #undef ROW_CASE
   }
   return cudaErrorInvalidValue;
@@ -67,8 +65,6 @@ cudaError_t launch_col_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* r
                            const u64* operand, u64 batch, int log_s, int out_mf, int fold,
                            cudaStream_t stream) {
   switch (log_r) {
-    case 1: return launch_col<MODE, 1>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
-    case 2: return launch_col<MODE, 2>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
     case 3: return launch_col<MODE, 3>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
     case 4: return launch_col<MODE, 4>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
     case 5: return launch_col<MODE, 5>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
@@ -100,7 +96,7 @@ cudaError_t simple_transform(bool fwd, const NttDeviceTables& t, u64* result, co
 template <int MODE, int LOGR>
 cudaError_t launch_fused(bool fwd, const NttDeviceTables& t, u64* result, const u64* operand, u64 batch,
                          int out_mf, cudaStream_t stream) {
-  using Cfg = FusedCfg<LOGR, MODE>;
+  using Cfg = FusedCfg<LOGR>;
   const Mod m = make_mod(t);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(batch * Cfg::K));
@@ -124,74 +120,12 @@ cudaError_t launch_fused(bool fwd, const NttDeviceTables& t, u64* result, const 
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-// The persistent pipelined kernel: one launch, work items from a global counter (ntt_kernels.cuh).
-// HEXL_B200_PIPE: see pipe_log_r below; HEXL_B200_PIPE_LOOKAHEAD = polynomials
-// between a producer block and its consumers (default 16, chosen for the H100's 50 MB L2: at N = 2^17 that is 16 MiB
-// of intermediate), HEXL_B200_PIPE_CTAS = CTAs per SM (default: the
-// kernel's launch bound).
+// The persistent pipelined kernel: one launch, work items from a global counter (ntt_kernels.cuh).  Forward only.
 template <int MODE, int LOGR>
-cudaError_t launch_pipe(bool fwd, const NttDeviceTables& t, u64* result, const u64* operand, u64 batch, int out_mf,
+cudaError_t launch_pipe(const NttDeviceTables& t, u64* result, const u64* operand, u64 batch, int out_mf,
                         cudaStream_t stream) {
-  using Cfg = PipeCfg<LOGR, MODE>;
-  static const int lookahead_env = env_int("HEXL_B200_PIPE_LOOKAHEAD", 16);
-  static const int ctas_env = env_int("HEXL_B200_PIPE_CTAS", 0);
-  const Mod m = make_mod(t);
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const unsigned lookahead = (unsigned)std::max(1, lookahead_env);
-  const u64 items = (batch + lookahead) * Cfg::SLOTS;
-  const int per_sm = ctas_env > 0 ? ctas_env : Cfg::MIN_BLOCKS;
-  const unsigned grid = (unsigned)std::min<u64>((u64)sms * per_sm, items);
-  unsigned* state = nullptr;  // [0] = work counter, [1 + p] = producers of polynomial p that have finished
-  const size_t bytes = (size_t)(batch + 1) * sizeof(unsigned);
-  cudaError_t e = scratch_alloc_async(reinterpret_cast<void**>(&state), bytes, stream);
-  if (e != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(state, 0, bytes, stream)) != cudaSuccess) return e;
-  if (fwd) {
-    if ((e = ensure_dynamic_smem<ntt_pipe_fwd<MODE, LOGR>>(Cfg::SMEM)) != cudaSuccess) return e;
-    ntt_pipe_fwd<MODE, LOGR><<<grid, Cfg::THREADS, Cfg::SMEM, stream>>>(result, operand, Tab<MODE>::fwd(t), m, out_mf,
-                                                                        (unsigned)batch, lookahead, state, state + 1);
-  } else {
-    if ((e = ensure_dynamic_smem<ntt_pipe_inv<MODE, LOGR>>(Cfg::SMEM)) != cudaSuccess) return e;
-    ntt_pipe_inv<MODE, LOGR><<<grid, Cfg::THREADS, Cfg::SMEM, stream>>>(result, operand, Tab<MODE>::inv(t), m, out_mf,
-                                                                        Tab<MODE>::inv_n(t), Tab<MODE>::inv_n_w(t),
-                                                                        (unsigned)batch, lookahead, state, state + 1);
-  }
-  count_launch();
-  e = cudaGetLastError();
-  scratch_free_async(state, stream);
-  return e;
-}
-
-template <int MODE>
-cudaError_t launch_pipe_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* result, const u64* operand, u64 batch,
-                            int out_mf, cudaStream_t stream) {
-  switch (log_r) {
-    case 2: return launch_pipe<MODE, 2>(fwd, t, result, operand, batch, out_mf, stream);
-    case 3: return launch_pipe<MODE, 3>(fwd, t, result, operand, batch, out_mf, stream);
-    case 4: return launch_pipe<MODE, 4>(fwd, t, result, operand, batch, out_mf, stream);
-    case 5: return launch_pipe<MODE, 5>(fwd, t, result, operand, batch, out_mf, stream);
-  }
-  return cudaErrorInvalidValue;
-}
-
-// log2(N / 4096) for which the pipelined kernel is used; 0 = none.  HEXL_B200_PIPE: 1 = always (N = 2^14..2^17),
-// 0 = never, unset = the 64-bit modes' forward at N = 2^15..2^17.  One H100 80GB HBM3 (power limit not recorded), 2^28
-// coefficients, 55-bit q (tools/tune_split.py, ms, pipelined vs the two-kernel split), with the coefficient arrays in
-// registers: N = 2^17 forward 3.10 vs 3.67, inverse 3.58 vs 3.71.  (Before, with the arrays in local memory: 2^17
-// forward 14.9 vs 17.2, inverse 15.5 vs 15.4.)  At N = 2^14..2^16 see dsmem_log_r for every candidate: the pipelined
-// forward is the fastest at 2^15 and 2^16, its inverse never is.  32-bit words use the distributed-shared-memory
-// kernel instead.  A batch of fewer polynomials than the pipeline is deep gains nothing from it.
-template <int MODE>
-inline int pipe_log_r(int log_n, u64 batch, bool forward) {
-  static const int mode = env_int("HEXL_B200_PIPE", -1);
-  static const int min_batch = env_int("HEXL_B200_PIPE_MIN_BATCH", 64);
-  const int lr = log_n - 12;
-  if (mode == 0 || lr < 2 || lr > 5 || batch < (u64)min_batch || batch >= (1ull << 31)) return 0;
-  if (mode > 0) return lr;
-  const bool wins = MODE != kSmall && forward && log_n >= 15;
-  return wins ? lr : 0;
+  return launch_pipelined<ntt_pipe_fwd<MODE, LOGR>, PipeCfg<LOGR>>(batch, stream, result, operand, Tab<MODE>::fwd(t),
+                                                                  make_mod(t), out_mf);
 }
 
 // The single kernel that keeps the intermediate in the cluster's shared memory
@@ -225,71 +159,83 @@ cudaError_t launch_dsmem(bool fwd, const NttDeviceTables& t, u64* result, const 
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-template <int MODE>
-cudaError_t launch_dsmem_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* result, const u64* operand,
-                             u64 batch, int out_mf, cudaStream_t stream) {
-  switch (log_r) {
-    case 2: return launch_dsmem<MODE, 2>(fwd, t, result, operand, batch, out_mf, stream);
-    case 3: return launch_dsmem<MODE, 3>(fwd, t, result, operand, batch, out_mf, stream);
-  }
-  if constexpr (MODE == kSmall) {
-    if (log_r == 4) return launch_dsmem<MODE, 4>(fwd, t, result, operand, batch, out_mf, stream);
-    if (log_r == 5) return launch_dsmem<MODE, 5>(fwd, t, result, operand, batch, out_mf, stream);
-  }
-  return cudaErrorInvalidValue;
-}
-
-// log2(N / 4096) for which the distributed-shared-memory kernel is used; 0 = none.  HEXL_B200_DSMEM=0 disables it.
-// SMALL mode (32-bit words):
-// One H100 SXM at 400 W, 2^28 coefficients, 29-bit q, forward / inverse ms vs the cluster kernel that keeps the
-// intermediate in L2: N = 2^14 6.41 / 6.69 vs 6.90 / 7.26, 2^15 6.42 / 6.77 vs 6.83 / 7.29, 2^16 7.54 / 7.84 vs
-// 7.99 / 8.15, 2^17 7.81 / 8.10 vs 8.25 / 8.42 (and vs 7.79 / 8.23, 8.10 / 8.30 for the pipelined kernel at 2^16 /
-// 2^17), so it is the default at every size.  Re-timed on an H100 80GB HBM3 (power limit not recorded) with the
-// coefficient arrays in registers: N = 2^16 1.76 / 1.79 vs 1.97 / 1.94, 2^17 1.94 / 2.08 vs 2.22 / 2.13 (pipelined
-// 2.05 / 2.15).
+// ------------------------------------------------------------------------------------------------ launch choice
+// Which kernel transforms a batch of polynomials of N = 2^log_n >= 16 coefficients: a single-pass kernel with
+// R = N / 4096 = 2^log_r, or the split (column passes of plan_col_passes, then rows of pick_row_log; a single row
+// kernel up to N = 2^13).  "Deep" is 64 <= batch < 2^31.
+//
+//   N      64-bit modes (FAST, WIDE, GENERIC)                                          SMALL (q < 2^30)
+//   2^14   distributed shared memory                                                  distributed shared memory
+//   2^15   forward: pipelined if deep, else distributed shared memory;                distributed shared memory
+//          inverse: distributed shared memory
+//   2^16   forward: pipelined if deep, else fused through L2; inverse: fused          distributed shared memory
+//   2^17   forward: pipelined if deep, else split; inverse: split                     distributed shared memory
+//   else   split                                                                      split
+//
+// SMALL mode (32-bit words), distributed shared memory vs the fused kernel that keeps the intermediate in L2, forward /
+// inverse ms, 2^28 coefficients, 29-bit q.  One H100 SXM at 400 W: N = 2^14 6.41 / 6.69 vs 6.90 / 7.26, 2^15 6.42 /
+// 6.77 vs 6.83 / 7.29, 2^16 7.54 / 7.84 vs 7.99 / 8.15, 2^17 7.81 / 8.10 vs 8.25 / 8.42 (and vs 7.79 / 8.23, 8.10 /
+// 8.30 for the pipelined kernel at 2^16 / 2^17), so it is the default at every size.  Re-timed on an H100 80GB HBM3
+// (power limit not recorded) with the coefficient arrays in registers: N = 2^16 1.76 / 1.79 vs 1.97 / 1.94, 2^17 1.94
+// / 2.08 vs 2.22 / 2.13 (pipelined 2.05 / 2.15).
 // 64-bit words, one H100 80GB HBM3 at 700 W (1980 MHz maximum SM clock), 2^28 coefficients, q of 55 (FAST) / 60 (WIDE)
-// / 61 (GENERIC) bits, forward / inverse ms, this kernel | the fused kernel through L2 | pipelined | two-kernel split:
+// / 61 (GENERIC) bits, forward / inverse ms, distributed shared memory | fused through L2 | pipelined | two-kernel
+// split:
 //   N = 2^14  FAST 2.96 / 2.75 | 3.01 / 2.90 | 3.20 / 5.92 | 3.49 / 3.71   WIDE 3.45 / 3.24 | 3.28 / 3.32 | 3.43 / 6.26
 //             GENERIC 3.35 / 3.37 | 3.41 / 3.57 | 3.48 / 6.54
 //   N = 2^15  FAST 3.02 / 2.93 | 3.04 / 2.93 | 2.95 / 4.38 | 3.49 / 3.73   WIDE 3.51 / 3.43 | 3.35 / 3.47 | 3.24 / 4.70
 //             GENERIC 3.46 / 3.60 | 3.46 / 3.67 | 3.28 / 4.98
 //   N = 2^16  FAST 3.23 / 3.43 | 3.07 / 3.13 | 2.88 / 3.54 | 3.49 / 3.73   WIDE 3.57 / 4.01 | 3.41 / 3.56 | 3.26 / 3.87
 //             GENERIC 3.71 / 4.20 | 3.54 / 3.82 | 3.27 / 4.07
-// So the 64-bit modes use it at N = 2^14 (except where the WIDE forward is 5 % behind the fused kernel, kept for one
-// rule per size) and for the 2^15 inverse (the 2^15 forward takes the pipelined kernel when the batch is deep enough
-// for it, this one otherwise).  At 2^16 it loses both ways -- its column phase stores to the peers' shared memory in
-// 8-byte words, and each CTA's phases are serialised at the cluster barrier -- to the pipelined forward and the fused
-// inverse.  On the benchmark's step (8192 polynomials at 2^16, 55-bit) this kernel in both directions took 13.2 ms
-// against 14.4 ms for the split.
+// So the 64-bit modes use distributed shared memory at N = 2^14 (except where the WIDE forward is 5 % behind the fused
+// kernel, kept for one rule per size) and for the 2^15 inverse (the 2^15 forward takes the pipelined kernel when the
+// batch is deep enough for it, this one otherwise).  At 2^16 it loses both ways -- its column phase stores to the
+// peers' shared memory in 8-byte words, and each CTA's phases are serialised at the cluster barrier -- to the
+// pipelined forward and the fused inverse.  On the benchmark's step (8192 polynomials at 2^16, 55-bit) the distributed-
+// shared-memory kernel in both directions took 13.2 ms against 14.4 ms for the split.
+// N = 2^17, one H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit q, against the two-kernel split,
+// with the coefficient arrays in registers: pipelined forward 3.10 vs 3.67, pipelined inverse 3.58 vs 3.71, fused
+// inverse 3.91 vs 3.71.  (Before, with the arrays in local memory: pipelined forward 14.9 vs 17.2, inverse 15.5 vs
+// 15.4.)  A batch of fewer polynomials than the pipeline is deep gains nothing from it.
+enum : int { kSplit, kPipe, kFused, kDsmem };
+struct SinglePass {
+  int kernel, log_r;
+};
 template <int MODE>
-int dsmem_log_r(int log_n) {
-  static const int mode = env_int("HEXL_B200_DSMEM", 1);
-  const int lr = log_n - DsmemCfg<2>::LOGC;
-  if (mode == 0 || lr < 2) return 0;
-  if constexpr (MODE == kSmall) return lr <= 5 ? lr : 0;
-  return lr <= 3 ? lr : 0;
+SinglePass plan_single_pass(int log_n, u64 batch, bool forward) {
+  const int lr = log_n - 12;
+  if (lr < 2 || lr > 5) return {kSplit, 0};
+  if (MODE == kSmall) return {kDsmem, lr};
+  if (forward && lr >= 3 && batch >= 64 && batch < (1ull << 31)) return {kPipe, lr};
+  if (lr <= 3) return {kDsmem, lr};
+  if (lr == 4) return {kFused, lr};
+  return {kSplit, 0};
 }
 
-// log2(N / 4096) for which the single fused kernel is used; 0 = none.  The 64-bit modes use it at N = 2^16 (the
-// inverse, and the forward of batches too shallow for the pipelined kernel; timings at dsmem_log_r);
-// HEXL_B200_FUSED=1 enables it at N = 2^14..2^17, 0 disables it.  One H100 80GB HBM3 (power limit not recorded),
-// 2^28 coefficients, 55-bit q: N = 2^17 inverse 3.91 vs 3.71 ms for the split.
+// Only what plan_single_pass returns is instantiated.
 template <int MODE>
-int fused_log_r(int log_n) {
-  static const int mode = MODE == kSmall ? env_int("HEXL_B200_FUSED_SMALL", 1) : env_int("HEXL_B200_FUSED", -1);
-  const int lr = log_n - FusedCfg<2>::LOGC;
-  if (mode == 0 || lr < 2 || lr > 5) return 0;
-  return (mode > 0 || log_n == 16) ? lr : 0;
-}
-
-template <int MODE>
-cudaError_t launch_fused_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* result, const u64* operand,
-                             u64 batch, int out_mf, cudaStream_t stream) {
-  switch (log_r) {
-    case 2: return launch_fused<MODE, 2>(fwd, t, result, operand, batch, out_mf, stream);
-    case 3: return launch_fused<MODE, 3>(fwd, t, result, operand, batch, out_mf, stream);
-    case 4: return launch_fused<MODE, 4>(fwd, t, result, operand, batch, out_mf, stream);
-    case 5: return launch_fused<MODE, 5>(fwd, t, result, operand, batch, out_mf, stream);
+cudaError_t launch_single_pass(SinglePass p, bool fwd, const NttDeviceTables& t, u64* result, const u64* operand,
+                               u64 batch, int out_mf, cudaStream_t stream) {
+  if constexpr (MODE == kSmall) {
+    switch (p.log_r) {
+      case 2: return launch_dsmem<MODE, 2>(fwd, t, result, operand, batch, out_mf, stream);
+      case 3: return launch_dsmem<MODE, 3>(fwd, t, result, operand, batch, out_mf, stream);
+      case 4: return launch_dsmem<MODE, 4>(fwd, t, result, operand, batch, out_mf, stream);
+      case 5: return launch_dsmem<MODE, 5>(fwd, t, result, operand, batch, out_mf, stream);
+    }
+  } else if (p.kernel == kPipe && fwd) {
+    switch (p.log_r) {
+      case 3: return launch_pipe<MODE, 3>(t, result, operand, batch, out_mf, stream);
+      case 4: return launch_pipe<MODE, 4>(t, result, operand, batch, out_mf, stream);
+      case 5: return launch_pipe<MODE, 5>(t, result, operand, batch, out_mf, stream);
+    }
+  } else if (p.kernel == kFused && p.log_r == 4) {
+    return launch_fused<MODE, 4>(fwd, t, result, operand, batch, out_mf, stream);
+  } else if (p.kernel == kDsmem) {
+    switch (p.log_r) {
+      case 2: return launch_dsmem<MODE, 2>(fwd, t, result, operand, batch, out_mf, stream);
+      case 3: return launch_dsmem<MODE, 3>(fwd, t, result, operand, batch, out_mf, stream);
+    }
   }
   return cudaErrorInvalidValue;
 }
@@ -297,9 +243,8 @@ cudaError_t launch_fused_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64*
 template <int MODE>
 cudaError_t forward_impl(const NttDeviceTables& t, u64* result, const u64* operand, int out_mf,
                          u64 batch, cudaStream_t stream) {
-  if (const int lr = pipe_log_r<MODE>(t.log_n, batch, true)) return launch_pipe_dyn<MODE>(lr, true, t, result, operand, batch, out_mf, stream);
-  if (const int lr = dsmem_log_r<MODE>(t.log_n)) return launch_dsmem_dyn<MODE>(lr, true, t, result, operand, batch, out_mf, stream);
-  if (const int lr = fused_log_r<MODE>(t.log_n)) return launch_fused_dyn<MODE>(lr, true, t, result, operand, batch, out_mf, stream);
+  const SinglePass sp = plan_single_pass<MODE>(t.log_n, batch, true);
+  if (sp.kernel != kSplit) return launch_single_pass<MODE>(sp, true, t, result, operand, batch, out_mf, stream);
   const int log_c = pick_row_log(t.log_n);
   int radices[8];
   const int ncol = plan_col_passes(t.log_n - log_c, radices);
@@ -317,9 +262,8 @@ cudaError_t forward_impl(const NttDeviceTables& t, u64* result, const u64* opera
 template <int MODE>
 cudaError_t inverse_impl(const NttDeviceTables& t, u64* result, const u64* operand, int out_mf,
                          u64 batch, cudaStream_t stream) {
-  if (const int lr = pipe_log_r<MODE>(t.log_n, batch, false)) return launch_pipe_dyn<MODE>(lr, false, t, result, operand, batch, out_mf, stream);
-  if (const int lr = dsmem_log_r<MODE>(t.log_n)) return launch_dsmem_dyn<MODE>(lr, false, t, result, operand, batch, out_mf, stream);
-  if (const int lr = fused_log_r<MODE>(t.log_n)) return launch_fused_dyn<MODE>(lr, false, t, result, operand, batch, out_mf, stream);
+  const SinglePass sp = plan_single_pass<MODE>(t.log_n, batch, false);
+  if (sp.kernel != kSplit) return launch_single_pass<MODE>(sp, false, t, result, operand, batch, out_mf, stream);
   const int log_c = pick_row_log(t.log_n);
   int radices[8];
   const int ncol = plan_col_passes(t.log_n - log_c, radices);

@@ -14,7 +14,7 @@
 //     of node k is table[k] (for the forward table that IS the reference's
 //     bit-reversed power layout).  A sub-transform rooted at node b over a
 //     contiguous block of S elements uses node (b << s) + i in its stage s.
-//   * "Row" kernel: one CTA owns a contiguous block of C = 2^c <= 16384
+//   * "Row" kernel: one CTA owns a contiguous block of C = 2^c <= 8192
 //     coefficients (a whole polynomial when N <= C, else one of N/C rows rooted
 //     at node N/C + r).  Each thread holds 16 coefficients in registers and runs
 //     4 butterfly stages per pass with no data movement; passes are separated by
@@ -28,18 +28,12 @@
 //
 // No tensor cores: this is 64-bit integer modular arithmetic (IMAD-bound).
 #pragma once
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
 
 #include "internal.h"
-
-// Timing-only ablations of the row kernels (results are WRONG when any bit is set; used by tools/ablate.sh to
-// attribute the kernel's time): 1 = no global loads, 2 = no global stores, 4 = last-pass twiddles not from L2,
-// 8 = no shared-memory exchanges, 16 = no twiddle tables in shared memory (and no barrier for them)
-#ifndef HEXL_B200_ABLATE
-#define HEXL_B200_ABLATE 0
-#endif
 
 namespace hexl_b200 {
 namespace {
@@ -119,7 +113,6 @@ constexpr int kFastBound = 8;  // FAST inverse: every value is < 8q at a pass bo
 struct Mod {
   u64 q, two_q, four_q, mu;  // mu = floor(2^64 / q)
   unsigned n0, n1;           // low / high word of 2^64 - q
-  u64 bias;                  // kQuotBias * q mod 2^64 (FP64-assisted quotient, see TwH)
 };
 
 __device__ __forceinline__ unsigned lo32(u64 x) { return (unsigned)x; }
@@ -204,94 +197,6 @@ __device__ __forceinline__ u64 mul_tw(u64 x, const Twiddle w, const Mod& m) {
 __device__ __forceinline__ u64 mul_tw_exact(u64 x, const Twiddle w, const Mod& m) {
   return mad_chain(x, w.w, mulhi(x, w.wp), m);
 }
-
-// ---- FP64-assisted quotient estimate (FAST mode, HEXL_B200_FP64Q).
-// The FMA-heavy pipe (IMAD / IMAD.WIDE) bounds the butterflies while the FP64 pipe idles.  Of the three
-// 32x32 products of mulhi_approx, the two cross terms  cross = (x1*b0 + x0*b1) / 2^32  (b = w') only
-// need ~33 significant bits, which two fused multiply-adds in binary64 deliver:
-//   A0 = 2^52 + x0, A1 = 2^52 + x1      bit patterns {0x43300000 : word}, no arithmetic
-//   beta_i = b_i / 2^32 (exact),   K = 2^52 + 2 - 2^20 (b0 + b1) (exact integer, |K| < 2^53)
-//   u = RD(A0*beta1 + K)      = x0*b1/2^32 + 2^52 + 2 - 2^20 b0 - [0,1)         in (0, 2^52 + 2^32 + 2]
-//   R = RD(A1*beta0 + u)      = 2^52 + 2 + cross - [0,2)                         in [2^52, 2^52 + 2^33 + 2]
-// so bits(R) = kQuotBias + c with c an integer in (cross - 2, cross]: Q = x1*b1 + c is low by 0, 1 or 2
-// exactly like mulhi_approx (tools/fp64_quot_model.py checks this with exact rationals).  The constant
-// kQuotBias rides along in Q; kQuotBias*q is added back through the accumulator of the first product of
-// the multiply-add chain (Mod::bias), so it costs nothing.
-constexpr u64 kQuotBias = 0x4330000000000002ull;
-struct TwH {
-  u64 w;
-  double beta0, beta1, K;
-  unsigned b1;
-};
-__device__ __forceinline__ double fma_rd(double a, double b, double c) {
-  double r;
-  asm("fma.rm.f64 %0, %1, %2, %3;" : "=d"(r) : "d"(a), "d"(b), "d"(c));
-  return r;
-}
-#ifndef HEXL_B200_FP64Q
-#define HEXL_B200_FP64Q 0
-#endif
-// HEXL_B200_FP64Q: 1 = operand words and twiddle words enter binary64 as {constant : word} register pairs;
-// 2 = operand words through I2F.F64.U32 (conversion unit; K is then the constant 2^52 + 2), twiddle words as pairs;
-// 3 = I2F.F64.U32 on both sides.
-__device__ __forceinline__ TwH expand_tw(const Twiddle t) {
-  unsigned b0, b1;
-  split(t.wp, b0, b1);
-  TwH h;
-  h.w = t.w;
-  h.b1 = b1;
-#if HEXL_B200_FP64Q == 3
-  h.beta0 = __uint2double_rn(b0) * (1.0 / 4294967296.0);
-  h.beta1 = __uint2double_rn(b1) * (1.0 / 4294967296.0);
-#else
-  // {0x41300000 : b} is 2^20 + b/2^32
-  h.beta0 = __hiloint2double(0x41300000, (int)b0) - 1048576.0;
-  h.beta1 = __hiloint2double(0x41300000, (int)b1) - 1048576.0;
-#endif
-#if HEXL_B200_FP64Q == 1
-  h.K = fma(h.beta0 + h.beta1, -4503599627370496.0, 4503599627370498.0);
-#else
-  h.K = 4503599627370498.0;
-#endif
-  return h;
-}
-// x*w mod q in [0,4q) for x < 2^63
-__device__ __forceinline__ u64 mul_tw_h(u64 x, const TwH& w, const Mod& m) {
-  unsigned x0, x1, w0, w1, q0, q1, t0, t1;
-  split(x, x0, x1);
-#if HEXL_B200_FP64Q == 1
-  const double A0 = __hiloint2double(0x43300000, (int)x0), A1 = __hiloint2double(0x43300000, (int)x1);
-#else
-  const double A0 = __uint2double_rn(x0), A1 = __uint2double_rn(x1);
-#endif
-  const double R = fma_rd(A1, w.beta0, fma_rd(A0, w.beta1, w.K));
-  split(mad_wide(x1, w.b1, (u64)__double_as_longlong(R)), q0, q1);  // Q + kQuotBias
-  split(w.w, w0, w1);
-  split(mad_wide(q0, m.n0, mad_wide(x0, w0, m.bias)), t0, t1);
-  t1 = mad_lo(x0, w1, t1);
-  t1 = mad_lo(x1, w0, t1);
-  t1 = mad_lo(q0, m.n1, t1);
-  t1 = mad_lo(q1, m.n0, t1);
-  return join(t0, t1);
-}
-
-// the twiddle form a mode's butterflies consume
-template <int MODE>
-struct TwUse {
-  using T = typename Ar<MODE>::Tw;
-  static __device__ __forceinline__ T prep(const typename Ar<MODE>::Tw t) { return t; }
-};
-#if HEXL_B200_FP64Q
-template <>
-struct TwUse<kFast> {
-  using T = TwH;
-  static __device__ __forceinline__ TwH prep(const Twiddle t) { return expand_tw(t); }
-};
-template <int MODE>
-__device__ __forceinline__ u64 mul_tw(u64 x, const TwH& w, const Mod& m) {
-  return mul_tw_h(x, w, m);
-}
-#endif
 
 // any 64-bit value -> [0,2q):  x - floor(x*mu/2^64)*q, mu = floor(2^64/q)
 __device__ __forceinline__ u64 barrett_lazy(u64 x, const Mod& m) {
@@ -571,8 +476,6 @@ __device__ __forceinline__ void reg_stages(typename Ar<MODE>::E (&v)[16], unsign
     auto fetch = [&](int g) {
       if constexpr (PT::kShared)
         return sroot[(8 >> eb) + g];                // local node 2^s' + g, s' = 3 - eb
-      else if constexpr ((HEXL_B200_ABLATE & 4) != 0)
-        return stab[((8 >> eb) + g + (u & 15) * 16) & 255];
       else
         return ld_tw(tw + (base << (LOGC - 1 - beta)) + ((u64)(u >> LB) << (LB + 3 - beta)) + g);
     };
@@ -589,13 +492,12 @@ __device__ __forceinline__ void reg_stages(typename Ar<MODE>::E (&v)[16], unsign
           wt = wc[g];
         else
           wt = fetch(g);
-        const typename TwUse<MODE>::T wg = TwUse<MODE>::prep(wt);
         static_for<0, (1 << eb)>([&](auto L) {
           constexpr int e = (g << (eb + 1)) | L;
           if constexpr (FWD)
-            fwd_bfly<MODE>(v[e], v[e | (1 << eb)], wg, m);
+            fwd_bfly<MODE>(v[e], v[e | (1 << eb)], wt, m);
           else
-            inv_bfly<MODE>(v[e], v[e | (1 << eb)], wg, m, cq);
+            inv_bfly<MODE>(v[e], v[e | (1 << eb)], wt, m, cq);
         });
       });
     };
@@ -626,7 +528,6 @@ __device__ __forceinline__ void reg_stages(typename Ar<MODE>::E (&v)[16], unsign
 template <int LB_FROM, int LB_TO, typename E>
 __device__ __forceinline__ void smem_exchange(E (&v)[16], E* srow, unsigned u) {
   constexpr bool kWarpLocal = (LB_FROM > LB_TO ? LB_FROM : LB_TO) <= 5;
-  if (HEXL_B200_ABLATE & 8) return;
   if constexpr (sizeof(E) == 8) {
     const unsigned uf = reg_index<LB_FROM>(u, 0), ut = reg_index<LB_TO>(u, 0);
     E* wr = srow + (uf + (uf >> 4));
@@ -683,16 +584,9 @@ __device__ __forceinline__ void inv_passes(typename Ar<MODE>::E (&v)[16], typena
 
 // 64-bit row kernels of 256 threads: 3 CTAs per SM (80 registers).  One H100 80GB HBM3 (power limit not recorded), 2^28 coefficients, 55-bit
 // q, N = 2^16 (tools/tune_split.py): forward / inverse 3.47 / 3.71 ms, against 3.58 / 3.94 ms with 2 CTAs per SM.
-#ifndef HEXL_B200_ROW_MIN_BLOCKS
-#define HEXL_B200_ROW_MIN_BLOCKS 3
-#endif
-#ifndef HEXL_B200_ROW_MIN_BLOCKS_512
-#define HEXL_B200_ROW_MIN_BLOCKS_512 2
-#endif
-
-#ifndef HEXL_B200_ROW_MIN_BLOCKS_SMALL
-#define HEXL_B200_ROW_MIN_BLOCKS_SMALL 4
-#endif
+constexpr int kRowMinBlocks = 3;
+constexpr int kRowMinBlocks512 = 2;   // rows of 512 threads (C = 8192), both word sizes
+constexpr int kRowMinBlocksSmall = 4;  // 32-bit rows of at most 256 threads
 template <int LOGC, int MODE = kGeneric>
 struct RowCfg {
   using E = typename Ar<MODE>::E;
@@ -705,8 +599,8 @@ struct RowCfg {
   static constexpr bool TW_TABLES = LOGC >= 8;          // sub-tree twiddles staged in shared memory
   static constexpr size_t ROW_BYTES = (size_t)row_elems<E>(LOGC) * sizeof(E) + (TW_TABLES ? kRowTwEntries * sizeof(Tw) : 0);
   static constexpr size_t SMEM = (size_t)ROWS * ROW_BYTES;
-  static constexpr int MIN_BLOCKS = THREADS <= 256 ? (MODE == kSmall ? HEXL_B200_ROW_MIN_BLOCKS_SMALL : HEXL_B200_ROW_MIN_BLOCKS)
-                                                   : (THREADS == 512 ? HEXL_B200_ROW_MIN_BLOCKS_512 : 1);
+  static constexpr int MIN_BLOCKS = THREADS <= 256 ? (MODE == kSmall ? kRowMinBlocksSmall : kRowMinBlocks)
+                                                   : (THREADS == 512 ? kRowMinBlocks512 : 1);
 };
 
 // Global-memory access policies for coefficients.  Streaming (evict-first) for
@@ -768,26 +662,18 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
   // cta_stab: every row of this CTA has the same root (whole polynomials, N == C): one table
   // filled by all threads of the CTA instead of one per row
   Tw* stab = cta_stab ? cta_stab : reinterpret_cast<Tw*>(srow + row_elems<E>(LOGC));
-  static_for<0, 16>([&](auto I) {
-    constexpr int e = I;
-    if constexpr ((HEXL_B200_ABLATE & 1) != 0)
-      v[e] = (E)((u * 16 + e) * 0x9E3779B97F4A7C15ull + base) & (E)(m.q - 1);
-    else
-      v[e] = ld_row<LD, E>(in, reg_index<LB0>(u, e));
-  });
+  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, reg_index<LB0>(u, e)); });
   if constexpr (LD < kSmemRow && sizeof(E) == 8) {
     if (reduce_in) {  // NttMulti::gather: the input is a value of ANOTHER modulus
       static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = reduce_any(v[e], m); });
     }
   }
   if constexpr (RowCfg<LOGC>::TW_TABLES) {
-    if (!(HEXL_B200_ABLATE & 16)) {
-      if (cta_stab)
-        load_row_twiddles<LOGC>(stab, threadIdx.x, blockDim.x, base, tw);
-      else
-        load_row_twiddles<LOGC>(stab, u, (1u << LOGC) / 16, base, tw);
-      __syncthreads();
-    }
+    if (cta_stab)
+      load_row_twiddles<LOGC>(stab, threadIdx.x, blockDim.x, base, tw);
+    else
+      load_row_twiddles<LOGC>(stab, u, (1u << LOGC) / 16, base, tw);
+    __syncthreads();
   }
   reg_stages<MODE, LOGC, LB0, LOGC - 1, LB0, true>(v, u, base, tw, stab, m, false, Tw{}, Tw{});
   fwd_passes<MODE, LOGC, 1>(v, srow, u, base, tw, stab, m);
@@ -798,10 +684,7 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
   constexpr int LB_OUT = LB0 < 4 ? LB0 : 4;
   if constexpr (LOGC > 4) smem_exchange<0, LB_OUT>(v, srow, u);
   if (active) {
-    static_for<0, 16>([&](auto I) {
-      constexpr int e = I;
-      if (!(HEXL_B200_ABLATE & 2) || v[e] == (E)0x123456789abcdefull) st_row<ST, E>(out, reg_index<LB_OUT>(u, e), v[e]);
-    });
+    static_for<0, 16>([&](auto I) { constexpr int e = I; st_row<ST, E>(out, reg_index<LB_OUT>(u, e), v[e]); });
   }
 }
 
@@ -921,7 +804,7 @@ __device__ __forceinline__ void col_stages(typename Ar<MODE>::E (&v)[1 << LOGR],
     auto groups = [&] {
       static_for<0, (1 << s)>([&](auto GI) {
         constexpr int gi = GI;
-        const typename TwUse<MODE>::T w = TwUse<MODE>::prep(stw[(1 << s) + gi]);
+        const Tw w = stw[(1 << s) + gi];
         static_for<0, (1 << eb)>([&](auto L) {
           constexpr int e = (gi << (eb + 1)) | L;
           if constexpr (FWD)
@@ -1025,21 +908,21 @@ __device__ __forceinline__ void cluster_barrier() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <int LOGR, int MODE = kGeneric>
+// 64-bit words only
+template <int LOGR>
 struct FusedCfg {
   static constexpr int LOGC = 12, C = 1 << LOGC, R = 1 << LOGR;
   static constexpr int K = R < 8 ? R : 8;            // CTAs per cluster
   static constexpr int THREADS = 256;                // = RowCfg<12>::T
-  static constexpr int MIN_BLOCKS = MODE == kSmall ? (LOGR <= 4 ? HEXL_B200_ROW_MIN_BLOCKS_SMALL : 3)
-                                                   : (LOGR <= 4 ? HEXL_B200_ROW_MIN_BLOCKS : 2);
-  static constexpr size_t SMEM = RowCfg<LOGC, MODE>::ROW_BYTES;
+  static constexpr int MIN_BLOCKS = LOGR <= 4 ? kRowMinBlocks : 2;
+  static constexpr size_t SMEM = RowCfg<LOGC>::ROW_BYTES;
 };
 
 template <int MODE, int LOGR>
-__global__ void __launch_bounds__(FusedCfg<LOGR, MODE>::THREADS, FusedCfg<LOGR, MODE>::MIN_BLOCKS)
+__global__ void __launch_bounds__(FusedCfg<LOGR>::THREADS, FusedCfg<LOGR>::MIN_BLOCKS)
     ntt_fused_fwd(u64* result, const u64* operand, const typename Ar<MODE>::Tw* __restrict__ tw, const Mod m,
                   int out_mf) {
-  using Cfg = FusedCfg<LOGR, MODE>;
+  using Cfg = FusedCfg<LOGR>;
   using E = typename Ar<MODE>::E;
   using Tw = typename Ar<MODE>::Tw;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1067,10 +950,10 @@ __global__ void __launch_bounds__(FusedCfg<LOGR, MODE>::THREADS, FusedCfg<LOGR, 
 }
 
 template <int MODE, int LOGR>
-__global__ void __launch_bounds__(FusedCfg<LOGR, MODE>::THREADS, FusedCfg<LOGR, MODE>::MIN_BLOCKS)
+__global__ void __launch_bounds__(FusedCfg<LOGR>::THREADS, FusedCfg<LOGR>::MIN_BLOCKS)
     ntt_fused_inv(u64* result, const u64* operand, const typename Ar<MODE>::Tw* __restrict__ tw, const Mod m,
                   int out_mf, typename Ar<MODE>::Tw inv_n, typename Ar<MODE>::Tw inv_n_w) {
-  using Cfg = FusedCfg<LOGR, MODE>;
+  using Cfg = FusedCfg<LOGR>;
   using E = typename Ar<MODE>::E;
   using Tw = typename Ar<MODE>::Tw;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1101,8 +984,8 @@ __global__ void __launch_bounds__(FusedCfg<LOGR, MODE>::THREADS, FusedCfg<LOGR, 
 // N = R * 4096 as above, ONE launch per batch, HBM sees each coefficient once in and once out, and no
 // barrier wider than a CTA.  The grid is persistent (a few CTAs per SM) and pulls work items from a
 // global counter.  Items come in the order
-//     block b:  the 16 column tiles of polynomial b,  then the R rows of polynomial b - D
-// (forward; the inverse runs rows of b, then column tiles of b - D).  A column tile is 256 columns of R
+//     block b:  the 16 column tiles of polynomial b,  then the R rows of polynomial b - D.
+// A column tile is 256 columns of R
 // coefficients (the top log2 R stages in registers); a row is a 4096-point transform.  The consumer of a
 // polynomial waits on a per-polynomial counter its producers bump with release semantics -- but the
 // producers were claimed D*(16+R) items earlier, far more than the number of CTAs in flight, so the wait
@@ -1120,21 +1003,22 @@ __device__ __forceinline__ void red_release_gpu(unsigned* p, unsigned v) {
   asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-template <int LOGR, int MODE = kGeneric>
+// 64-bit words only
+template <int LOGR>
 struct PipeCfg {
   static constexpr int LOGC = 12, C = 1 << LOGC, R = 1 << LOGR;
   static constexpr int THREADS = 256;
   static constexpr int CT = C / THREADS;             // column tiles per polynomial
   static constexpr int SLOTS = CT + R;               // work items per block
-  static constexpr int MIN_BLOCKS = FusedCfg<LOGR, MODE>::MIN_BLOCKS;
-  static constexpr size_t SMEM = RowCfg<LOGC, MODE>::ROW_BYTES;
+  static constexpr int MIN_BLOCKS = FusedCfg<LOGR>::MIN_BLOCKS;
+  static constexpr size_t SMEM = RowCfg<LOGC>::ROW_BYTES;
 };
 
 template <int MODE, int LOGR>
-__global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MODE>::MIN_BLOCKS)
+__global__ void __launch_bounds__(PipeCfg<LOGR>::THREADS, PipeCfg<LOGR>::MIN_BLOCKS)
     ntt_pipe_fwd(u64* result, const u64* operand, const typename Ar<MODE>::Tw* __restrict__ tw, const Mod m,
                  int out_mf, unsigned batch, unsigned lookahead, unsigned* counter, unsigned* done) {
-  using Cfg = PipeCfg<LOGR, MODE>;
+  using Cfg = PipeCfg<LOGR>;
   using E = typename Ar<MODE>::E;
   using Tw = typename Ar<MODE>::Tw;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1166,48 +1050,6 @@ __global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MO
       __syncthreads();
       u64* row = result + ((u64)p << (Cfg::LOGC + LOGR)) + (u64)r * Cfg::C;
       row_fwd_body<MODE, Cfg::LOGC, kViaL2, kStream>(row, row, smem, threadIdx.x, (u64)Cfg::R + r, tw, m, out_mf, true);
-    }
-  }
-}
-
-template <int MODE, int LOGR>
-__global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MODE>::MIN_BLOCKS)
-    ntt_pipe_inv(u64* result, const u64* operand, const typename Ar<MODE>::Tw* __restrict__ tw, const Mod m,
-                 int out_mf, typename Ar<MODE>::Tw inv_n, typename Ar<MODE>::Tw inv_n_w, unsigned batch,
-                 unsigned lookahead, unsigned* counter, unsigned* done) {
-  using Cfg = PipeCfg<LOGR, MODE>;
-  using E = typename Ar<MODE>::E;
-  using Tw = typename Ar<MODE>::Tw;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  E* smem = reinterpret_cast<E*>(smem_raw);
-  __shared__ Tw stw[Cfg::R];
-  __shared__ unsigned s_item;
-  for (int l = threadIdx.x; l < Cfg::R; l += Cfg::THREADS)
-    if (l) stw[l] = ld_tw(tw + l);
-  const unsigned total = (batch + lookahead) * Cfg::SLOTS;
-  while (true) {
-    __syncthreads();
-    if (threadIdx.x == 0) s_item = atomicAdd(counter, 1u);
-    __syncthreads();
-    const unsigned item = s_item;
-    if (item >= total) break;
-    const unsigned blk = item / Cfg::SLOTS, j = item % Cfg::SLOTS;
-    if (j < (unsigned)Cfg::R) {                      // row j of polynomial blk
-      if (blk >= batch) continue;
-      const u64 off = ((u64)blk << (Cfg::LOGC + LOGR)) + (u64)j * Cfg::C;
-      row_inv_body<MODE, Cfg::LOGC, kStream, kViaL2>(result + off, operand + off, smem, threadIdx.x, (u64)Cfg::R + j, tw,
-                                                     m, out_mf, false, inv_n, inv_n_w, true);
-      __syncthreads();
-      if (threadIdx.x == 0) red_release_gpu(done + blk, 1u);
-    } else {                                         // column tile j - R of polynomial blk - lookahead
-      if (blk < lookahead) continue;
-      const unsigned p = blk - lookahead, t = j - Cfg::R;
-      if (threadIdx.x == 0)
-        while (ld_acquire_gpu(done + p) < (unsigned)Cfg::R) __nanosleep(100);
-      __syncthreads();
-      const u64 poly_off = (u64)p << (Cfg::LOGC + LOGR);
-      col_body<MODE, LOGR, false, kViaL2, kStream>(result, result, poly_off + t * Cfg::THREADS + threadIdx.x, Cfg::LOGC,
-                                                   stw, m, out_mf, true, inv_n, inv_n_w);
     }
   }
 }
@@ -1251,7 +1093,7 @@ __device__ __forceinline__ E dsmem_load(unsigned addr) {
 // 3 CTAs per SM the 64-bit row kernels are tuned to.  One 64-bit row per CTA in clusters of 16 (non-portable) fits
 // 3 CTAs per SM as well, but an H100 80GB HBM3 (400 W) schedules only 21 such clusters (336 of 396 CTA slots,
 // cudaOccupancyMaxActiveClusters) against 45 clusters of 8, and at N = 2^16, 55-bit q, 2^28 coefficients, it took
-// 3.86 / 4.27 ms forward / inverse against 3.97 / 4.36 for the two-kernel split.  ntt.cu (dsmem_log_r) launches the
+// 3.86 / 4.27 ms forward / inverse against 3.97 / 4.36 for the two-kernel split.  ntt.cu (plan_single_pass) launches the
 // 64-bit kernels at N = 2^14 and 2^15 only.
 template <int LOGR, int MODE = kSmall>
 struct DsmemCfg {
@@ -1268,7 +1110,7 @@ struct DsmemCfg {
   // owned rows (+ the exchange buffer of 32-bit words) + the row kernel's twiddle tables
   static constexpr size_t SMEM = (size_t)(RPC + (PAD ? 0 : 1)) * ROW * sizeof(E) + kRowTwEntries * sizeof(Tw);
   // 64-bit words: the row kernels' 3 CTAs per SM (80 registers) at every R
-  static constexpr int MIN_BLOCKS = PAD ? HEXL_B200_ROW_MIN_BLOCKS : (SMEM <= 56 * 1024 ? 4 : (SMEM <= 75 * 1024 ? 3 : 2));
+  static constexpr int MIN_BLOCKS = PAD ? kRowMinBlocks : (SMEM <= 56 * 1024 ? 4 : (SMEM <= 75 * 1024 ? 3 : 2));
   // where coefficient j of an owned row is stored
   static __device__ __forceinline__ unsigned slot(unsigned j) { return PAD ? j + (j >> 4) : j; }
 };
@@ -1423,32 +1265,44 @@ cudaError_t ensure_dynamic_smem(size_t bytes) {
   return e;
 }
 
-inline int env_int(const char* name, int dflt) {
-  const char* v = std::getenv(name);
-  return v ? std::atoi(v) : dflt;
+// One launch of a persistent pipelined kernel (ntt_pipe_fwd, ntt_pipe_multi) over `units` polynomials: a grid of
+// MIN_BLOCKS CTAs per SM (fewer if there are fewer work items) and a zeroed work counter and per-polynomial producer
+// counters, freed in stream order after the kernel.  The kernel is called with args..., then (units, lookahead,
+// counter, done).  HEXL_B200_PIPE_LOOKAHEAD = polynomials between a producer block and its consumers (default 16,
+// chosen for the H100's 50 MB L2: at N = 2^17 that is 16 MiB of intermediate).
+template <auto Kernel, typename Cfg, typename... Args>
+cudaError_t launch_pipelined(u64 units, cudaStream_t stream, Args... args) {
+  static const unsigned lookahead = [] {
+    const char* v = std::getenv("HEXL_B200_PIPE_LOOKAHEAD");
+    return (unsigned)std::max(1, v ? std::atoi(v) : 16);
+  }();
+  cudaError_t e = ensure_dynamic_smem<Kernel>(Cfg::SMEM);
+  if (e != cudaSuccess) return e;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const u64 items = (units + lookahead) * Cfg::SLOTS;
+  const unsigned grid = (unsigned)std::min<u64>((u64)sms * Cfg::MIN_BLOCKS, items);
+  unsigned* state = nullptr;  // [0] = work counter, [1 + p] = producers of polynomial p that have finished
+  const size_t bytes = (size_t)(units + 1) * sizeof(unsigned);
+  if ((e = scratch_alloc_async(reinterpret_cast<void**>(&state), bytes, stream)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(state, 0, bytes, stream)) == cudaSuccess) {
+    Kernel<<<grid, Cfg::THREADS, Cfg::SMEM, stream>>>(args..., (unsigned)units, lookahead, state, state + 1);
+    count_launch();
+    e = cudaGetLastError();
+  }
+  scratch_free_async(state, stream);
+  return e;
 }
 
-// log2 of the row length used for a transform of size 2^log_n
-inline int pick_row_log(int log_n) {
-  static const int max_row = [] {
-    int v = env_int("HEXL_B200_MAX_ROW_LOG", 13);
-    return v < 4 ? 4 : (v > 14 ? 14 : v);
-  }();
-  static const int split_row = [] {
-    int v = env_int("HEXL_B200_SPLIT_ROW_LOG", 12);
-    return v < 4 ? 4 : (v > 14 ? 14 : v);
-  }();
-  if (log_n <= max_row) return log_n;
-  return split_row;
-}
+// log2 of the row length used for a transform of size 2^log_n: the whole polynomial up to 8192 coefficients, else
+// 4096-point rows after the column passes
+inline int pick_row_log(int log_n) { return log_n <= 13 ? log_n : 12; }
 
 inline int pick_mode(u64 q) {
-  static const bool force_generic = env_int("HEXL_B200_FORCE_GENERIC", 0) != 0;
-  if (force_generic) return kGeneric;
   if (q < kSmallModulusLimit) return kSmall;
   if (q < kFastModulusLimit && q >= (1ull << 32)) return kFast;
-  static const bool no_wide = env_int("HEXL_B200_NO_WIDE", 0) != 0;
-  return (q >= kFastModulusLimit && q < kWideModulusLimit && !no_wide) ? kWide : kGeneric;
+  return (q >= kFastModulusLimit && q < kWideModulusLimit) ? kWide : kGeneric;
 }
 
 // the tables of a mode
@@ -1476,7 +1330,6 @@ __host__ __device__ inline Mod make_mod(u64 q, u64 mu) {
   const u64 negq = 0 - q;
   m.n0 = (unsigned)negq;
   m.n1 = (unsigned)(negq >> 32);
-  m.bias = kQuotBias * q;
   return m;
 }
 inline Mod make_mod(const NttDeviceTables& t) { return make_mod(t.q, t.mu); }

@@ -80,20 +80,19 @@ __global__ void __launch_bounds__(256)
                                               FWD ? nullptr : &mir, FWD && gather != 0);
 }
 
-// The persistent pipelined single kernel of ntt_kernels.cuh (ntt_pipe_fwd / _inv) for RNS batches: the same work
-// queue, producer/consumer counters and L2-resident intermediate; the modulus record of a work item comes from the
+// The persistent pipelined forward kernel of ntt_kernels.cuh (ntt_pipe_fwd) for RNS batches: the same work queue,
+// producer/consumer counters and L2-resident intermediate; the modulus record of a work item comes from the
 // polynomial it belongs to, and the root sub-tree twiddles are re-staged when a CTA's next item has another modulus.
-template <int MODE, int LOGR, bool FWD>
-__global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MODE>::MIN_BLOCKS)
+template <int MODE, int LOGR>
+__global__ void __launch_bounds__(PipeCfg<LOGR>::THREADS, PipeCfg<LOGR>::MIN_BLOCKS)
     ntt_pipe_multi(u64* result, const u64* operand, const __grid_constant__ NttMulti multi, int out_mf, unsigned units,
                    unsigned lookahead, unsigned* counter, unsigned* done) {
-  using Cfg = PipeCfg<LOGR, MODE>;
+  using Cfg = PipeCfg<LOGR>;
   using E = typename Ar<MODE>::E;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   E* smem = reinterpret_cast<E*>(smem_raw);
   __shared__ Twiddle stw[Cfg::R];
   __shared__ unsigned s_item;
-  constexpr unsigned kProd = FWD ? Cfg::CT : Cfg::R;  // producer items per polynomial (column tiles / rows)
   const unsigned total = (units + lookahead) * Cfg::SLOTS;
   unsigned staged = ~0u;                              // modulus entry whose root twiddles sit in stw
   while (true) {
@@ -103,93 +102,38 @@ __global__ void __launch_bounds__(PipeCfg<LOGR, MODE>::THREADS, PipeCfg<LOGR, MO
     const unsigned item = s_item;
     if (item >= total) break;
     const unsigned blk = item / Cfg::SLOTS, j = item % Cfg::SLOTS;
-    const bool producer = j < kProd;
+    const bool producer = j < (unsigned)Cfg::CT;      // column tile j of polynomial blk, else row j - CT of blk - D
     if (producer ? blk >= units : blk < lookahead) continue;
     const unsigned poly = producer ? blk : blk - lookahead;
     const unsigned entry = poly / multi.group;
     const NttDeviceParams P = *multi.p[entry];
     const Mod m = make_mod(P.q, P.mu);
-    const Twiddle* tw = FWD ? P.fwd : P.inv;
     if (entry != staged) {                            // uniform across the CTA
       for (int l = threadIdx.x; l < Cfg::R; l += Cfg::THREADS)
-        if (l) stw[l] = ld_tw(tw + l);
+        if (l) stw[l] = ld_tw(P.fwd + l);
       staged = entry;
       __syncthreads();
     }
     const u64 poly_off = (u64)poly << (Cfg::LOGC + LOGR);
     if (!producer) {
       if (threadIdx.x == 0)
-        while (ld_acquire_gpu(done + poly) < kProd) __nanosleep(100);
+        while (ld_acquire_gpu(done + poly) < (unsigned)Cfg::CT) __nanosleep(100);
       __syncthreads();
     }
-    if (FWD) {
-      if (producer) {
-        col_body<MODE, LOGR, true, kStream, kViaL2>(result, operand, poly_off + j * Cfg::THREADS + threadIdx.x, Cfg::LOGC,
-                                                    stw, m, out_mf, false, Twiddle{}, Twiddle{});
-      } else {
-        const unsigned r = j - Cfg::CT;
-        u64* row = result + poly_off + (u64)r * Cfg::C;
-        row_fwd_body<MODE, Cfg::LOGC, kViaL2, kStream>(row, row, smem, threadIdx.x, (u64)Cfg::R + r, tw, m, out_mf, true);
-      }
+    if (producer) {
+      col_body<MODE, LOGR, true, kStream, kViaL2>(result, operand, poly_off + j * Cfg::THREADS + threadIdx.x, Cfg::LOGC,
+                                                  stw, m, out_mf, false, Twiddle{}, Twiddle{});
     } else {
-      if (producer) {
-        const u64 off = poly_off + (u64)j * Cfg::C;
-        row_inv_body<MODE, Cfg::LOGC, kStream, kViaL2>(result + off, operand + off, smem, threadIdx.x, (u64)Cfg::R + j, tw,
-                                                       m, out_mf, false, P.inv_n, P.inv_n_w, true);
-      } else {
-        const MirrorList mir{multi.mirror, multi.mirrors, 0};
-        col_body<MODE, LOGR, false, kViaL2, kStream>(result, result, poly_off + (j - Cfg::R) * Cfg::THREADS + threadIdx.x,
-                                                     Cfg::LOGC, stw, m, out_mf, true, P.inv_n, P.inv_n_w,
-                                                     &mir);
-      }
+      const unsigned r = j - Cfg::CT;
+      u64* row = result + poly_off + (u64)r * Cfg::C;
+      row_fwd_body<MODE, Cfg::LOGC, kViaL2, kStream>(row, row, smem, threadIdx.x, (u64)Cfg::R + r, P.fwd, m, out_mf,
+                                                     true);
     }
     if (producer) {
       __syncthreads();
       if (threadIdx.x == 0) red_release_gpu(done + poly, 1u);
     }
   }
-}
-
-template <int MODE, int LOGR>
-cudaError_t launch_pipe_multi(bool fwd, const NttMulti& multi, u64* result, const u64* operand, u64 units, int out_mf,
-                              cudaStream_t stream) {
-  using Cfg = PipeCfg<LOGR, MODE>;
-  static const int lookahead_env = env_int("HEXL_B200_PIPE_LOOKAHEAD", 16);
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const unsigned lookahead = (unsigned)(lookahead_env < 1 ? 1 : lookahead_env);
-  const u64 items = (units + lookahead) * Cfg::SLOTS;
-  const u64 want = (u64)sms * Cfg::MIN_BLOCKS;
-  const unsigned grid = (unsigned)(want < items ? want : items);
-  unsigned* state = nullptr;
-  const size_t bytes = (size_t)(units + 1) * sizeof(unsigned);
-  cudaError_t e = scratch_alloc_async(reinterpret_cast<void**>(&state), bytes, stream);
-  if (e != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(state, 0, bytes, stream)) != cudaSuccess) return e;
-  if (fwd) {
-    if ((e = ensure_dynamic_smem<ntt_pipe_multi<MODE, LOGR, true>>(Cfg::SMEM)) != cudaSuccess) return e;
-    ntt_pipe_multi<MODE, LOGR, true><<<grid, Cfg::THREADS, Cfg::SMEM, stream>>>(result, operand, multi, out_mf, (unsigned)units,
-                                                                                lookahead, state, state + 1);
-  } else {
-    if ((e = ensure_dynamic_smem<ntt_pipe_multi<MODE, LOGR, false>>(Cfg::SMEM)) != cudaSuccess) return e;
-    ntt_pipe_multi<MODE, LOGR, false><<<grid, Cfg::THREADS, Cfg::SMEM, stream>>>(result, operand, multi, out_mf, (unsigned)units,
-                                                                                 lookahead, state, state + 1);
-  }
-  count_launch();
-  e = cudaGetLastError();
-  scratch_free_async(state, stream);
-  return e;
-}
-
-// forced by HEXL_B200_PIPE=1, off with =0 (as ntt.cu:pipe_log_r), else the forward transform at N = 2^17
-inline int pipe_multi_log_r(int log_n, u64 units, bool forward) {
-  static const int mode = env_int("HEXL_B200_PIPE", -1);
-  static const int min_batch = env_int("HEXL_B200_PIPE_MIN_BATCH", 64);
-  const int lr = log_n - 12;
-  if (mode == 0 || lr < 2 || lr > 5 || units < (u64)min_batch || units >= (1ull << 31)) return 0;
-  if (mode > 0) return lr;
-  return (forward && log_n == 17) ? lr : 0;
 }
 
 // N = 2^LOGN < 16: one thread per polynomial, everything in registers (launch-bound shapes only)
@@ -272,7 +216,7 @@ cudaError_t launch_row_multi_dyn(int log_c, bool fwd, const NttMulti& multi, int
 #define ROW_CASE(L) \
   case L: return launch_row_multi<MODE, L>(fwd, multi, log_n, result, operand, units, out_mf, fold, stream, gather);
     ROW_CASE(4) ROW_CASE(5) ROW_CASE(6) ROW_CASE(7) ROW_CASE(8) ROW_CASE(9) ROW_CASE(10)
-    ROW_CASE(11) ROW_CASE(12) ROW_CASE(13) ROW_CASE(14)
+    ROW_CASE(11) ROW_CASE(12) ROW_CASE(13)
 #undef ROW_CASE
   }
   return cudaErrorInvalidValue;
@@ -302,7 +246,7 @@ cudaError_t launch_col_multi_dyn(int log_r, bool fwd, const NttMulti& multi, int
   switch (log_r) {
 #define COL_CASE(L) \
   case L: return launch_col_multi<MODE, L>(fwd, multi, log_n, result, operand, units, log_s, out_mf, fold, stream, gather);
-    COL_CASE(1) COL_CASE(2) COL_CASE(3) COL_CASE(4) COL_CASE(5)
+    COL_CASE(2) COL_CASE(3) COL_CASE(4) COL_CASE(5)
 #undef COL_CASE
   }
   return cudaErrorInvalidValue;
@@ -312,14 +256,10 @@ template <int MODE>
 cudaError_t multi_impl(bool fwd, const NttMulti& multi, int log_n, u64* result, const u64* operand, int out_mf,
                        u64 units, cudaStream_t stream) {
   const unsigned gather = fwd ? multi.gather : 0u;
-  if (const int lr = (gather || multi.mul) ? 0 : pipe_multi_log_r(log_n, units, fwd)) {
-    switch (lr) {
-      case 2: return launch_pipe_multi<MODE, 2>(fwd, multi, result, operand, units, out_mf, stream);
-      case 3: return launch_pipe_multi<MODE, 3>(fwd, multi, result, operand, units, out_mf, stream);
-      case 4: return launch_pipe_multi<MODE, 4>(fwd, multi, result, operand, units, out_mf, stream);
-      case 5: return launch_pipe_multi<MODE, 5>(fwd, multi, result, operand, units, out_mf, stream);
-    }
-  }
+  // the pipelined kernel: the forward transform at N = 2^17 of a batch deep enough for the pipeline, without gather
+  // (multiply-on-load is inverse only)
+  if (fwd && !gather && log_n == 17 && units >= 64 && units < (1ull << 31))
+    return launch_pipelined<ntt_pipe_multi<MODE, 5>, PipeCfg<5>>(units, stream, result, operand, multi, out_mf);
   const int log_c = pick_row_log(log_n);
   int radices[8];
   const int ncol = plan_col_passes(log_n - log_c, radices);
@@ -370,11 +310,9 @@ cudaError_t launch_ntt_multi(bool forward, const NttMulti& multi, int log_n, u64
   }
   // FAST needs every modulus in [2^32, 2^56), WIDE every modulus below 2^61 (its doubled lazy ranges
   // are valid for any smaller q as well), GENERIC runs everything
-  static const bool force_generic = env_int("HEXL_B200_FORCE_GENERIC", 0) != 0;
-  static const bool no_wide = env_int("HEXL_B200_NO_WIDE", 0) != 0;
-  if (!force_generic && min_q >= (1ull << 32) && max_q < kFastModulusLimit)
+  if (min_q >= (1ull << 32) && max_q < kFastModulusLimit)
     return multi_impl<kFast>(forward, multi, log_n, result, operand, out_mf, units, stream);
-  if (!force_generic && !no_wide && max_q < kWideModulusLimit)
+  if (max_q < kWideModulusLimit)
     return multi_impl<kWide>(forward, multi, log_n, result, operand, out_mf, units, stream);
   return multi_impl<kGeneric>(forward, multi, log_n, result, operand, out_mf, units, stream);
 }

@@ -80,6 +80,59 @@ def test_c4_poly_multiply_16_moduli_n17(hb, checker):
     assert (host(x) == conv[lo:hi]).all()
 
 
+# The multi-modulus forward transform at N = 2^17 of 64 or more units is the pipelined kernel, one launch; below 64 units
+# it is the split, a column pass and a row pass.  C4 in bench.py (16 moduli x 32 polynomials) takes the pipelined kernel;
+# these cases run it at 64 units under one modulus set per arithmetic mode: (name, mode, [(count, bits, first)], group).
+PIPE_SETS = [("c4_60bit", "wide", [(16, 60, True)], 4),
+             ("50_55bit", "fast", [(4, 50, True), (4, 55, True)], 8),
+             ("below_2_62", "generic", [(8, 61, False)], 8)]
+PIPE_SPREAD = [0, 1, 7, 8, 30, 31, 32, 45, 62, 63]  # units compared with the checker
+
+
+def _multi_mode(mods):
+    """the arithmetic mode launch_ntt_multi picks for a list of moduli"""
+    if min(mods) >= 1 << 32 and max(mods) < 1 << 56:
+        return "fast"
+    return "wide" if max(mods) < 1 << 61 else "generic"
+
+
+@pytest.mark.parametrize("name,mode,primes,group", PIPE_SETS, ids=[s[0] for s in PIPE_SETS])
+def test_multi_forward_n17_pipelined(hb, checker, name, mode, primes, group):
+    """ComputeForwardMulti (canonical and lazy outputs) and PolyMultiplyMulti, whose forward transforms take the same
+    kernel; PolyMultiplyMulti needs q < 2^61, so not under the GENERIC set."""
+    n = 1 << 17
+    mods = [q for count, bits, first in primes for q in hb.GeneratePrimes(count, bits, first, n)]
+    assert len(set(mods)) == len(mods) and len(mods) * group == 64 and _multi_mode(mods) == mode
+    ntts = [hb.NTT(n, q).Prepare() for q in mods]
+    sz = n * group
+    a = np.concatenate([uniform_below(43 * i + 1, sz, q) for i, q in enumerate(mods)])
+    b = np.concatenate([uniform_below(43 * i + 2, sz, q) for i, q in enumerate(mods)])
+    da, db = dev(a), dev(b)
+    o = torch.zeros_like(da)
+    launches = hb.launch_count()
+    hb.ComputeForwardMulti(ntts, o, da, 1, 1, batch_per_modulus=group)
+    assert hb.launch_count() - launches == 1
+    got = host(o)
+    exp_f = {u: checker.ntt_forward(a[u * n:(u + 1) * n], n, mods[u // group]) for u in PIPE_SPREAD}
+    for u in PIPE_SPREAD:
+        assert (got[u * n:(u + 1) * n] == exp_f[u]).all(), ("fwd", name, u)
+    hb.ComputeForwardMulti(ntts, o, da, 1, 4, batch_per_modulus=group)
+    got = host(o)
+    for u in PIPE_SPREAD:
+        q = np.uint64(mods[u // group])
+        g = got[u * n:(u + 1) * n]
+        assert (g % q == exp_f[u]).all() and (g < np.uint64(4) * q).all(), ("fwd lazy", name, u)
+    if mode == "generic":
+        return
+    hb.PolyMultiplyMulti(ntts, o, da, db, group)
+    got = host(o)
+    for u in PIPE_SPREAD:
+        q = mods[u // group]
+        fb = checker.ntt_forward(b[u * n:(u + 1) * n], n, q)
+        exp = checker.ntt_inverse(checker.mult_mod(exp_f[u], fb, q), n, q)
+        assert (got[u * n:(u + 1) * n] == exp).all(), ("poly multiply", name, u)
+
+
 def _c5_case(hb, n, decomp, bits, kcc=2):
     kms = rns = decomp + 1
     mods = hb.GeneratePrimes(kms, bits, True, n)

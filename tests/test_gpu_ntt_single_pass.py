@@ -1,12 +1,13 @@
-"""The single-pass transforms of 64-bit moduli at N = 2^14..2^16, at the launch choice the library makes by default.
+"""The single-pass transforms of 64-bit moduli at N = 2^14..2^17, at the launch choice the library makes by default.
 
-At these degrees each transform is one kernel: the one that keeps the whole polynomial in its cluster's shared memory
-(N = 2^14, the 2^15 inverse, the 2^15 forward of shallow batches), the pipelined one (the 2^15 and 2^16 forward of deep
-batches) or the cluster kernel whose intermediate goes through L2 (the 2^16 inverse, and the forward of shallow
-batches).  These tests hold those paths to the checker at the edges of every 64-bit arithmetic mode (FAST just
-above 2^32 and just below 2^56, WIDE, GENERIC just below 2^62), for lazy and extreme inputs, in place, for a single
-polynomial, a few, and a grid many clusters deep, and at the benchmark's own shape; and they hold the kernels to
-registers in the ptxas report.
+At N = 2^14..2^16 each transform is one kernel: the one that keeps the whole polynomial in its cluster's shared memory
+(N = 2^14, the 2^15 inverse, the 2^15 forward of shallow batches), the pipelined one (the 2^15 and 2^16 forward of
+batches of 64 or more) or the cluster kernel whose intermediate goes through L2 (the 2^16 inverse, and the forward of
+shallow batches).  At N = 2^17 the forward of 64 or more polynomials is the pipelined kernel too; the 2^17 inverse, and
+the forward of shallow batches, are the two-kernel split.  These tests hold those paths to the checker at the edges of
+every 64-bit arithmetic mode (FAST just above 2^32 and just below 2^56, WIDE, GENERIC just below 2^62), for lazy and
+extreme inputs, in place, for a single polynomial, a few, and a grid many waves deep (where the 2^15..2^17 forward
+is one pipelined launch), and at the benchmark's own shape; and they hold the kernels to registers in the ptxas report.
 """
 import numpy as np
 import pytest
@@ -99,17 +100,20 @@ def test_single_pass_extreme_inputs(hb, checker, logn, name, bits, first):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("logn", LOGNS)
+@pytest.mark.parametrize("logn", LOGNS + [17])
 @pytest.mark.parametrize("name,bits,first", MODULI, ids=[m[0] for m in MODULI])
 def test_single_pass_many_waves(hb, checker, logn, name, bits, first):
-    """1000 polynomials: a grid several waves of clusters deep"""
+    """1000 polynomials: a grid several waves deep.  The forward is one launch (the pipelined kernel from N = 2^15 on;
+    at 2^17 the split would be two)."""
     n, batch = 1 << logn, 1000
     q = modulus(hb, n, bits, first)
-    t = hb.NTT(n, q)
+    t = hb.NTT(n, q).Prepare()
     g = torch.Generator(device="cuda").manual_seed(logn * 1000 + bits)
     x = torch.randint(0, q, (batch, n), dtype=torch.int64, device="cuda", generator=g)
     y = torch.empty_like(x)
+    launches = hb.launch_count()
     t.ComputeForward(y, x, 1, 1)
+    assert hb.launch_count() - launches == 1, ("fwd launches", name, logn)
     xs = host(x[SPREAD]).reshape(-1)
     assert (host(y[SPREAD]).reshape(-1) == checker.ntt_forward(xs, n, q)).all(), ("fwd", name, logn)
     z = torch.empty_like(x)

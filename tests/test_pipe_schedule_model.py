@@ -1,6 +1,6 @@
-"""Host-side model of the persistent pipelined transform's work queue (ntt_kernels.cuh:ntt_pipe_fwd / _inv,
+"""Host-side model of the persistent pipelined forward transform's work queue (ntt_kernels.cuh:ntt_pipe_fwd,
 ntt_multi.cu:ntt_pipe_multi): item -> (polynomial, role) mapping, coverage, and freedom from deadlock with any number of
-resident CTAs.  No GPU: the kernels' control flow is restated with a cooperative scheduler that lets CTAs claim items
+resident CTAs.  The 16 column tiles of a polynomial produce, its R rows consume.  No GPU: the kernels' control flow is restated with a cooperative scheduler that lets CTAs claim items
 in counter order and run or block exactly as the device code does."""
 import random
 
@@ -16,12 +16,12 @@ def item_of(i, slots, kprod, units, lookahead):
     return ("prod", blk, j) if producer else ("cons", blk - lookahead, j - kprod)
 
 
-@pytest.mark.parametrize("logr,fwd", [(2, True), (2, False), (4, True), (5, False)])
+@pytest.mark.parametrize("logr", [2, 3, 4, 5])
 @pytest.mark.parametrize("units,lookahead", [(1, 1), (3, 1), (5, 2), (7, 48), (64, 48)])
-def test_every_work_unit_exactly_once_and_producers_first(logr, fwd, units, lookahead):
+def test_every_work_unit_exactly_once_and_producers_first(logr, units, lookahead):
     ct, r = 4096 // 256, 1 << logr
     slots = ct + r
-    kprod = ct if fwd else r                      # forward: column tiles produce, rows consume; inverse: the reverse
+    kprod = ct
     ncons = slots - kprod
     total = (units + lookahead) * slots
     seen = {}

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Time forward/inverse NTT for a list of log2(N) under the current HEXL_B200_* environment
-(one process per setting: the knobs are read once).  python tools/tune_split.py 13 14 [bits]"""
+"""Time forward/inverse NTT for a list of log2(N), 2^28 coefficients per call, at the library's default launch choice
+(ntt.cu:plan_single_pass).  python tools/tune_split.py 13 14 [bits]"""
 import os
 import sys
 
