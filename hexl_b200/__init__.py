@@ -112,6 +112,7 @@ _sig("hexl_b200_eltwise_cmp_sub_mod", _int, [_vp, _vp, _u64, _u64, _int, _u64, _
 _sig("hexl_b200_ntt_get_cached", _int, [C.POINTER(_vp), _u64, _u64])
 _sig("hexl_b200_dyadic_multiply", _int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp])
 _sig("hexl_b200_key_switch", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _vp])
+_sig("hexl_b200_divide_and_round_q_last", _int, [_vp, _vp, _u64, _vp, _u64, _u64, _int, _vp])
 
 _sig("hexl_b200_hensel_lemma_2adic_root", _u64, [C.c_uint32, _u64])
 _sig("hexl_b200_montgomery_reduce", _u64, [_u64, _u64, _u64, _int, _u64])
@@ -495,6 +496,19 @@ def KeySwitch(result, t_target_iter_ptr, n, decomp_modulus_size, key_modulus_siz
     _check(_lib.hexl_b200_key_switch(rp, tp, n, decomp_modulus_size, key_modulus_size, rns_modulus_size,
                                      key_component_count, mods.ctypes.data, key_ptrs, ms.ctypes.data,
                                      _stream(stream, rc or tc)))
+    return result
+
+
+def DivideAndRoundQLast(result, operand, n, moduli, rns_modulus_size, count=1, ntt_form=True, stream=None):
+    """Rescale `count` polynomials of rns_modulus_size limbs (n words each) by their last modulus
+    (hexl_b200_divide_and_round_q_last; SEAL's divide_and_round_q_last(_ntt)_inplace).  Limbs 0..L-1 of every
+    polynomial of result are written, limb L is not; result may be operand."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); op, on, oc = _buf(operand)
+    _need("moduli", mods.size, rns_modulus_size)
+    _need("result", rn, count * rns_modulus_size * n); _need("operand", on, count * rns_modulus_size * n)
+    _check(_lib.hexl_b200_divide_and_round_q_last(rp, op, n, mods.ctypes.data, rns_modulus_size, count,
+                                                  int(bool(ntt_form)), _stream(stream, rc or oc)))
     return result
 
 

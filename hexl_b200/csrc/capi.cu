@@ -20,7 +20,9 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <numeric>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/hexl_b200.h"
@@ -270,10 +272,12 @@ StageCtx* stage_for(int dev) {
 // A host-pointer job: `total` elements, processed in chunks that are multiples
 // of `unit` elements.  a is always present; b optional; result may alias a or b.
 // launch(dev_result, dev_a, dev_b, off, elems, stream) enqueues the kernel(s) for the
-// elements [off, off + elems) of the whole job (`base` = offset of this device's block).
+// elements [off, off + elems) of the whole job (`base` = offset of this device's block);
+// it returns a cudaError_t, or an int error code whose message it has already set.
+// unit_out (non-zero): only the first unit_out elements of every unit are copied back.
 template <class Launch>
 int run_host_on_device(int dev, u64* result, const u64* a, const u64* b, u64 total, u64 unit,
-                       Launch&& launch, bool wait, u64 base = 0) {
+                       Launch&& launch, bool wait, u64 base = 0, u64 unit_out = 0) {
   DeviceGuard g;
   if (int rc = g.enter(dev)) return rc;
   StageCtx* st = stage_for(dev);
@@ -291,9 +295,17 @@ int run_host_on_device(int dev, u64* result, const u64* a, const u64* b, u64 tot
     cudaStream_t s = st->stream[slot];
     CU(cudaMemcpyAsync(st->buf[slot][0], a + off, bytes, cudaMemcpyHostToDevice, s));
     if (b) CU(cudaMemcpyAsync(st->buf[slot][1], b + off, bytes, cudaMemcpyHostToDevice, s));
-    cudaError_t e = launch(st->buf[slot][0], st->buf[slot][0], b ? st->buf[slot][1] : nullptr, base + off, elems, s);
-    if (e != cudaSuccess) return cuda_fail(e, "kernel launch");
-    CU(cudaMemcpyAsync(result + off, st->buf[slot][0], bytes, cudaMemcpyDeviceToHost, s));
+    const auto e = launch(st->buf[slot][0], st->buf[slot][0], b ? st->buf[slot][1] : nullptr, base + off, elems, s);
+    if constexpr (std::is_same_v<std::decay_t<decltype(e)>, int>) {
+      if (e) return e;
+    } else if (e != cudaSuccess) {
+      return cuda_fail(e, "kernel launch");
+    }
+    if (unit_out && unit_out < unit)
+      CU(cudaMemcpy2DAsync(result + off, unit * sizeof(u64), st->buf[slot][0], unit * sizeof(u64),
+                           unit_out * sizeof(u64), elems / unit, cudaMemcpyDeviceToHost, s));
+    else
+      CU(cudaMemcpyAsync(result + off, st->buf[slot][0], bytes, cudaMemcpyDeviceToHost, s));
   }
   if (wait)
     for (int s = 0; s < kSlots; ++s) CU(cudaStreamSynchronize(st->stream[s]));
@@ -318,7 +330,7 @@ std::vector<int> host_devices() {
 // Split a host-pointer job over the configured devices by contiguous blocks of
 // whole units (no inter-GPU traffic), enqueue everything, then wait.
 template <class MakeLaunch>
-int run_host(u64* result, const u64* a, const u64* b, u64 total, u64 unit, MakeLaunch&& make) {
+int run_host(u64* result, const u64* a, const u64* b, u64 total, u64 unit, MakeLaunch&& make, u64 unit_out = 0) {
   std::vector<int> devs = host_devices();
   if (devs.empty() || total / unit < 2) {
     int cur = 0;
@@ -326,7 +338,7 @@ int run_host(u64* result, const u64* a, const u64* b, u64 total, u64 unit, MakeL
     if (!devs.empty()) cur = devs[0];
     auto launch = make(cur, (u64)0, total);
     if (!launch.ok) return launch.rc;
-    return run_host_on_device(cur, result, a, b, total, unit, launch, true);
+    return run_host_on_device(cur, result, a, b, total, unit, launch, true, 0, unit_out);
   }
   const u64 units = total / unit;
   const u64 ndev = devs.size() < units ? devs.size() : units;
@@ -338,7 +350,8 @@ int run_host(u64* result, const u64* a, const u64* b, u64 total, u64 unit, MakeL
       rc = launch.rc;  // fall through: copies already enqueued on other devices still target `result`
       break;
     }
-    rc = run_host_on_device(devs[d], result + lo, a + lo, b ? b + lo : nullptr, hi - lo, unit, launch, false, lo);
+    rc = run_host_on_device(devs[d], result + lo, a + lo, b ? b + lo : nullptr, hi - lo, unit, launch, false, lo,
+                            unit_out);
   }
   for (u64 d = 0; d < ndev; ++d) {
     int rc2 = sync_stage(devs[d]);
@@ -739,6 +752,47 @@ static uint64_t ks_mac_digits_per_launch(const KsModuli& mods, uint64_t count) {
   return (uint64_t)std::min<unsigned __int128>(kParamBlock, ~(unsigned __int128)0 / largest_product);
 }
 
+// Mod-down of `group` polynomials by their last modulus q_last = h_last->q, every step batched over the target moduli
+// (key-switch-internal.cpp:134-198; SEAL's divide_and_round_q_last_ntt_inplace):
+//   t_last: the polynomials' last part in NTT form, [p][n] contiguous, < 2 q_last; inverse-transformed in place;
+//   for each block of at most kParamBlock target moduli i (h_targets[i], q_i, factors[i] = q_last^-1 mod q_i):
+//     ks_round into tmp ([e][p][n], room for one block), one lazy multi-modulus forward transform of tmp, and
+//     ks_finish: result[n (res_stride p + i) + l] (+)= (in - tmp) * factors[i] mod q_i.
+// `in`, in_like_result and accumulate are those of launch_ks_finish (modulus-major `in` starts at target 0).
+// About 1 + 3 launches per block, whatever `group` is.  Device pointers on the current device, asynchronous on s.
+int mod_down_on_device(int dev, uint64_t* result, uint64_t res_stride, const uint64_t* in, bool in_like_result,
+                       bool accumulate, uint64_t* t_last, uint64_t* tmp, uint64_t n, uint64_t group,
+                       hexl_b200_ntt* h_last, hexl_b200_ntt* const* h_targets, const uint64_t* target_moduli,
+                       const uint64_t* factors, uint64_t targets, cudaStream_t s) {
+#define LAUNCH(expr)                                                    \
+  do {                                                                  \
+    cudaError_t e__ = (expr);                                           \
+    if (e__ != cudaSuccess) return cuda_fail(e__, "mod-down: " #expr); \
+  } while (0)
+  const uint64_t q_last = h_last->q, mu_last = nt::multiply_factor(1, 64, q_last);
+  {
+    NttDeviceTables tl;
+    if (int rc = device_tables(h_last, dev, &tl, s)) return rc;
+    LAUNCH(launch_ntt_inverse(tl, t_last, t_last, 2, 2, group, s));
+  }
+  for (uint64_t i0 = 0; i0 < targets; i0 += kParamBlock) {
+    const uint64_t cnt = std::min<uint64_t>(kParamBlock, targets - i0);
+    KsModuli round_mods, fin_mods;
+    for (uint64_t e = 0; e < cnt; ++e) {
+      const uint64_t qi = target_moduli[i0 + e], mu_i = nt::multiply_factor(1, 64, qi);
+      round_mods.m[e] = KsModulus{qi, mu_i, qi - ((q_last >> 1) % qi), 0, 0};
+      const Twiddle ms = make_twiddle(factors[i0 + e] % qi, qi);
+      fin_mods.m[e] = KsModulus{qi, mu_i, ms.w, ms.wp, 0};
+    }
+    LAUNCH(launch_ks_round(tmp, t_last, n, group, q_last, mu_last, cnt, round_mods, s));
+    if (int rc = ntt_multi_on_device(true, dev, h_targets + i0, cnt, tmp, tmp, 4, group, s)) return rc;
+    LAUNCH(launch_ks_finish(result, in_like_result ? in : in + i0 * group * n, tmp, n, group, res_stride, i0, cnt,
+                            fin_mods, in_like_result, accumulate, s));
+  }
+#undef LAUNCH
+  return 0;
+}
+
 // key-switch-internal.cpp:25-201 as a short chain of launches on the caller's stream, every
 // step batched over the RNS moduli (multi-modulus NTTs + the glue kernels of seal.cu): about a
 // dozen launches whatever the number of moduli, instead of ~10 per modulus.  Every pointer is
@@ -771,8 +825,8 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
   uint64_t *t_coef = nullptr, *ops = nullptr, *prod = nullptr, *tmp = nullptr;
   if (int rc = ws.get(&t_coef, per_mod)) return rc;
   if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;
-  if (int rc = ws.get(&prod, rns * kcc * n)) return rc;   // [i][k][n]
-  if (int rc = ws.get(&tmp, decomp * kcc * n)) return rc;  // [i][k][n]
+  if (int rc = ws.get(&prod, rns * kcc * n)) return rc;                                       // [i][k][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(decomp, kParamBlock) * kcc * n)) return rc;  // [i][k][n], one block
 #define LAUNCH(expr)                                                    \
   do {                                                                  \
     cudaError_t e__ = (expr);                                           \
@@ -805,29 +859,11 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
                            j0 != 0, s));
     }
   }
-  // 3. mod-down by the special prime and accumulate into result (:134-198)
-  const uint64_t q_last = moduli[key_modulus_size - 1], mu_last = nt::multiply_factor(1, 64, q_last);
-  uint64_t* t_last = prod + decomp * kcc * n;  // [k][n], contiguous
-  {
-    NttDeviceTables tl;
-    if (int rc = device_tables(h[key_modulus_size - 1], dev, &tl, s)) return rc;
-    LAUNCH(launch_ntt_inverse(tl, t_last, t_last, 2, 2, kcc, s));
-  }
-  for (uint64_t i0 = 0; i0 < decomp; i0 += kParamBlock) {
-    const uint64_t cnt = std::min<uint64_t>(kParamBlock, decomp - i0);
-    KsModuli round_mods, fin_mods;
-    for (uint64_t e = 0; e < cnt; ++e) {
-      const uint64_t qi = moduli[i0 + e], mu_i = nt::multiply_factor(1, 64, qi);
-      round_mods.m[e] = KsModulus{qi, mu_i, qi - ((q_last >> 1) % qi), 0, 0};
-      const Twiddle ms = make_twiddle(modswitch[i0 + e] % qi, qi);
-      fin_mods.m[e] = KsModulus{qi, mu_i, ms.w, ms.wp, 0};
-    }
-    uint64_t* tmp_c = tmp + i0 * kcc * n;
-    LAUNCH(launch_ks_round(tmp_c, t_last, n, kcc, q_last, mu_last, cnt, round_mods, s));
-    if (int rc = ntt_multi_on_device(true, dev, h.data() + i0, cnt, tmp_c, tmp_c, 4, kcc, s)) return rc;
-    LAUNCH(launch_ks_finish(result, prod + i0 * kcc * n, tmp_c, n, kcc, decomp, i0, cnt, fin_mods, s));
-  }
 #undef LAUNCH
+  // 3. mod-down by the special prime and accumulate into result (:134-198); prod's last part is [k][n], contiguous
+  if (int rc = mod_down_on_device(dev, result, decomp, prod, false, true, prod + decomp * kcc * n, tmp, n, kcc,
+                                  h[key_modulus_size - 1], h.data(), moduli, modswitch, decomp, s))
+    return rc;
   return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
 }
 
@@ -1782,7 +1818,8 @@ static int key_switch_sharded(uint64_t* result, const uint64_t* t_target, uint64
         uint64_t* tmp_c = z.tmp + e0 * kcc * n;
         if (cu(launch_ks_round(tmp_c, z.t_last, n, kcc, q_last, mu_last, c, round_mods, z.stream), "ks_round")) break;
         if (bad(ntt_multi_on_device(true, z.device, h.data() + z.lo + e0, c, tmp_c, tmp_c, 4, kcc, z.stream))) break;
-        cu(launch_ks_finish(z.res, z.prod + e0 * kcc * n, tmp_c, n, kcc, nd, e0, c, fin_mods, z.stream), "ks_finish");
+        cu(launch_ks_finish(z.res, z.prod + e0 * kcc * n, tmp_c, n, kcc, nd, e0, c, fin_mods, false, true, z.stream),
+           "ks_finish");
       }
       if (!rc) cu(cudaMemcpy2DAsync(result + z.lo * n, row, z.res, nd * n * 8, nd * n * 8, kcc, cudaMemcpyDeviceToHost, z.stream), "D2H result");
     }
@@ -1959,6 +1996,119 @@ int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, ui
                                        modswitch_factors, 1);
   hexl_b200_keys_release(tmp);
   return rc;
+}
+
+// ---------------------------------------------------------------- rescale by the last modulus
+// `count` polynomials of rns limbs x n words (limb i under moduli[i]), device pointers on the current device; limbs
+// [0, rns - 1) of result get floor((X + q_last/2) / q_last) mod q_i.  NTT form: the gathered last limbs of a chunk of
+// polynomials run through the shared mod-down (mod_down_on_device); coefficient form: one fused kernel per block of
+// moduli.  h: the cached transforms of every modulus (NTT form only).
+static int divide_and_round_on_device(int dev, uint64_t* result, const uint64_t* operand, uint64_t n,
+                                      const uint64_t* moduli, uint64_t rns, uint64_t count, bool ntt_form,
+                                      hexl_b200_ntt* const* h, cudaStream_t s) {
+  const uint64_t L = rns - 1, q_last = moduli[L], mu_last = nt::multiply_factor(1, 64, q_last);
+  std::vector<uint64_t> inv(L);
+  for (uint64_t i = 0; i < L; ++i) inv[i] = nt::inverse_mod(q_last % moduli[i], moduli[i]);
+  if (!ntt_form) {
+    for (uint64_t i0 = 0; i0 < L; i0 += kParamBlock) {
+      const uint64_t cnt = std::min<uint64_t>(kParamBlock, L - i0);
+      KsModuli mods;
+      for (uint64_t e = 0; e < cnt; ++e) {
+        const uint64_t qi = moduli[i0 + e];
+        const Twiddle f = make_twiddle(inv[i0 + e], qi);
+        mods.m[e] = KsModulus{qi, nt::multiply_factor(1, 64, qi), f.w, f.wp, qi - ((q_last >> 1) % qi)};
+      }
+      cudaError_t e = launch_rescale_coef(result, operand, n, rns, i0, cnt, count, q_last, mu_last, mods, s);
+      if (e != cudaSuccess) return cuda_fail(e, "DivideAndRoundQLast launch");
+    }
+    return 0;
+  }
+  // polynomials per round: the last limbs plus one block of rounded limbs stay within ~256 MiB of scratch
+  const uint64_t block = std::min<uint64_t>(L, kParamBlock);
+  uint64_t chunk = std::max<uint64_t>(1, (256ull << 20) / ((block + 1) * n * 8));
+  chunk = std::min(chunk, count);
+  Scratch ws(s);
+  uint64_t *t_last = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&t_last, chunk * n)) return rc;        // [p][n]
+  if (int rc = ws.get(&tmp, block * chunk * n)) return rc;   // [e][p][n]
+  for (uint64_t p0 = 0; p0 < count; p0 += chunk) {
+    const uint64_t cnt = std::min(chunk, count - p0);
+    const uint64_t* op = operand + p0 * rns * n;
+    CU(cudaMemcpy2DAsync(t_last, n * 8, op + L * n, rns * n * 8, n * 8, cnt, cudaMemcpyDeviceToDevice, s));
+    if (int rc = mod_down_on_device(dev, result + p0 * rns * n, rns, op, true, false, t_last, tmp, n, cnt, h[L], h,
+                                    moduli, inv.data(), L, s))
+      return rc;
+  }
+  return 0;  // ~Scratch returns the buffers to the pool in stream order
+}
+
+int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                                      uint64_t rns_modulus_size, uint64_t count, int ntt_form, void* stream) {
+  REQUIRE(result && operand && moduli, "Require result, operand, moduli != nullptr");
+  REQUIRE(rns_modulus_size >= 2, "Require rns_modulus_size >= 2");
+  REQUIRE(ntt_form == 0 || ntt_form == 1, "Require ntt_form = 0 or 1");
+  const uint64_t rns = rns_modulus_size, L = rns - 1, q_last = moduli[L];
+  for (uint64_t i = 0; i < rns; ++i)
+    // the lazy sums of the round and finish steps (< 8q) need q < 2^61
+    REQUIRE(moduli[i] > 1 && moduli[i] < (1ull << 61), "Require 1 < moduli[%llu] < 2^61", (unsigned long long)i);
+  for (uint64_t i = 0; i < L; ++i)
+    REQUIRE(std::gcd(moduli[i], q_last) == 1, "Require moduli[%llu] coprime to the last modulus",
+            (unsigned long long)i);
+  if (ntt_form) {
+    REQUIRE(n >= 2 && n <= (1ull << 20) && !(n & (n - 1)), "Require n a power of two in [2, 2^20]");
+    for (uint64_t i = 0; i < rns; ++i) {
+      const char* why = "";
+      REQUIRE(check_ntt_arguments(n, moduli[i], &why), "moduli[%llu]: %s", (unsigned long long)i, why);
+    }
+  } else {
+    REQUIRE(n >= 1, "Require n >= 1");
+  }
+  if (count == 0) return 0;
+  const uint64_t unit = rns * n, total = count * unit;
+  REQUIRE(result == operand || result + total <= operand || operand + total <= result,
+          "result and operand must be the same buffer or not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, operand}, &pi)) return rc;
+  std::vector<hexl_b200_ntt*> h(ntt_form ? rns : 0, nullptr);
+  struct Release {
+    std::vector<hexl_b200_ntt*>& v;
+    ~Release() {
+      for (auto* p : v)
+        if (p) hexl_b200_ntt_release(p);
+    }
+  } release{h};
+  for (uint64_t i = 0; i < h.size(); ++i)
+    if (int rc = cached_ntt(&h[i], n, moduli[i])) return rc;
+  if (g_debug.load())
+    for (uint64_t p = 0; p < count; ++p)
+      for (uint64_t i = 0; i < rns; ++i)
+        if (int rc = check_bounds(operand + p * unit + i * n, n, moduli[i], pi, "operand")) return rc;
+  const bool ntt = ntt_form != 0;
+  if (pi.where == Where::Device) {
+    DeviceGuard g;
+    if (int rc = g.enter(pi.device)) return rc;
+    if (int rc = divide_and_round_on_device(pi.device, result, operand, n, moduli, rns, count, ntt, h.data(),
+                                            (cudaStream_t)stream))
+      return rc;
+    return finish_device_call(pi, stream);
+  }
+  // host pointers: whole polynomials through the staging slots (split over the host devices when set); only limbs
+  // [0, L) of each polynomial are copied back, so limb L of result is left as it was
+  struct Launch {
+    bool ok = true;
+    int rc = 0;
+    int dev;
+    uint64_t n, rns, unit;
+    const uint64_t* moduli;
+    bool ntt;
+    hexl_b200_ntt* const* h;
+    int operator()(u64* r, const u64* a, const u64*, u64, u64 elems, cudaStream_t s) const {
+      return divide_and_round_on_device(dev, r, a, n, moduli, rns, elems / unit, ntt, h, s);
+    }
+  };
+  return run_host(result, operand, nullptr, total, unit,
+                  [&](int dev, u64, u64) { return Launch{true, 0, dev, n, rns, unit, moduli, ntt, h.data()}; },
+                  L * n);
 }
 
 }  // extern "C"

@@ -128,6 +128,7 @@ cudaError_t launch_rns_eltwise(int op, u64* result, const u64* a, const u64* b, 
 // describes modulus i0 + e).  KsModulus.a/b/c mean, per kernel:
 //   reduce: -            mac: a,b = 2^64 mod q and its Shoup factor, c = slot of q in the key
 //   round:  a = q - (q_last/2 mod q)        finish: a,b = mod-switch factor and its Shoup factor
+//   rescale_coef: a,b = q_last^-1 mod q and its Shoup factor, c = q - (q_last/2 mod q)
 struct KsModulus {
   u64 q, mu, a, b, c;
 };
@@ -141,9 +142,16 @@ cudaError_t launch_ks_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPo
 // tmp[e][k][l] = ((t_last[k][l] + q_last/2) mod q_last) mod q_e + a_e
 cudaError_t launch_ks_round(u64* tmp, const u64* t_last, u64 n, u64 kcc, u64 q_last, u64 mu_last, u64 count,
                             const KsModuli& mods, cudaStream_t stream);
-// result[k][i0+e][l] = (result + (prod[e][k][l] + 4 q_e - tmp[e][k][l]) * a_e) mod q_e ; result has `decomp` moduli per k
-cudaError_t launch_ks_finish(u64* result, const u64* prod, const u64* tmp, u64 n, u64 kcc, u64 decomp, u64 i0,
-                             u64 count, const KsModuli& mods, cudaStream_t stream);
+// result[k][i0+e][l] = ([result +] (in + 4 q_e - tmp[e][k][l]) * a_e) mod q_e ; result has `res_stride` moduli per k.
+// in: in[e][k][l] (modulus-major, like tmp), or in[k][i0+e][l] laid out like result when in_like_result (may be result).
+// accumulate: add into result (KeySwitch) or store (DivideAndRoundQLast).
+cudaError_t launch_ks_finish(u64* result, const u64* in, const u64* tmp, u64 n, u64 kcc, u64 res_stride, u64 i0,
+                             u64 count, const KsModuli& mods, bool in_like_result, bool accumulate,
+                             cudaStream_t stream);
+// DivideAndRoundQLast in coefficient form, fused: `polys` polynomials of rns limbs x n words; limbs [i0, i0 + count)
+// of result = round(limb rns-1) and finish(limb i0+e) of operand, one pass; limb rns-1 of result is not written
+cudaError_t launch_rescale_coef(u64* result, const u64* operand, u64 n, u64 rns, u64 i0, u64 count, u64 polys,
+                                u64 q_last, u64 mu_last, const KsModuli& mods, cudaStream_t stream);
 
 // Stream-ordered scratch from the library's own memory pool (capi.cu): kept warm between calls, capturable.
 cudaError_t scratch_alloc_async(void** p, size_t bytes, cudaStream_t stream);

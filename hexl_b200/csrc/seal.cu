@@ -1,9 +1,11 @@
 // Device kernels for the SEAL-shaped composites that sit directly on top of the
-// hot path (SURVEY.md 8(f)-1/-2): DyadicMultiply and the element-wise glue of
-// CKKS KeySwitch.  The NTTs inside KeySwitch are the kernels of ntt.cu; what is
-// here is memory-bound streaming work.
+// hot path (SURVEY.md 8(f)-1/-2): DyadicMultiply, the element-wise glue of
+// CKKS KeySwitch, and the rescale (DivideAndRoundQLast) that shares KeySwitch's
+// mod-down.  The NTTs inside them are the kernels of ntt.cu; what is here is
+// memory-bound streaming work.
 //   DyadicMultiply   hexl/experimental/seal/dyadic-multiply-internal.cpp:17-73
 //   KeySwitch        hexl/experimental/seal/key-switch-internal.cpp:25-201
+//   rescale          SEAL's RNSTool::divide_and_round_q_last(_ntt)_inplace
 #include "internal.h"
 
 namespace hexl_b200 {
@@ -154,8 +156,22 @@ __global__ void __launch_bounds__(kThreads)
   prod[g] = v;
 }
 
-// :148-178: the special prime's part (coefficient form, [0, 2 q_last)), rounded and moved
-// into modulus e:  t = (x + q_last/2) mod q_last;  out = (t mod q_e) + (q_e - (q_last/2 mod q_e))
+// The two halves of the mod-down by the last modulus, shared by the kernels below.
+// round: a coefficient of the last modulus's part (coefficient form, [0, 2 q_last)) rounded and moved into modulus q:
+//   t = (x + q_last/2) mod q_last;  out = (t mod q) + add,  add = q - (q_last/2 mod q);  out < 2q
+__device__ __forceinline__ u64 round_into(u64 x, u64 q_last, u64 mu_last, u64 q, u64 mu, u64 add) {
+  x += q_last >> 1;
+  x = csub(barrett64_lazy(x, q_last, mu_last), q_last);
+  if (q_last > q) x = csub(barrett64_lazy(x, q, mu), q);
+  return x + add;
+}
+// finish: (x + 4q - t) * factor mod q, canonical, for x < 4q and t < 4q (the operand is < 8q, so q < 2^61)
+__device__ __forceinline__ u64 finish_value(u64 x, u64 t, u64 q, u64 w, u64 wp) {
+  x = reduce_from<8>(x + (q << 2) - t, q);
+  return csub(shoup_lazy(x, w, wp, q), q);
+}
+
+// :148-178: the special prime's part, rounded and moved into modulus e
 __global__ void __launch_bounds__(kThreads)
     ks_round_kernel(u64* tmp, const u64* t_last, u64 per_mod /* kcc*n */, u64 q_last, u64 mu_last, u64 count,
                     const __grid_constant__ KsModuli mods) {
@@ -163,27 +179,41 @@ __global__ void __launch_bounds__(kThreads)
   if (g >= per_mod * count) return;
   const u64 e = g / per_mod, r = g - e * per_mod;
   const KsModulus& md = mods.m[e];
-  u64 x = t_last[r] + (q_last >> 1);
-  x = csub(barrett64_lazy(x, q_last, mu_last), q_last);
-  if (q_last > md.q) x = csub(barrett64_lazy(x, md.q, md.mu), md.q);
-  tmp[g] = x + md.a;
+  tmp[g] = round_into(t_last[r], q_last, mu_last, md.q, md.mu, md.a);
 }
 
-// :183-197:  r = (prod + 4 q_e - t_ntt) * modswitch mod q_e (operand < 8 q_e);  result += r mod q_e
+// :183-197:  v = (in + 4 q_e - t_ntt) * modswitch mod q_e;  result[n (res_stride k + i0 + e) + l] (+)= v mod q_e.
+// `in` is either modulus-major like tmp (KeySwitch's prod) or, with in_like_result, laid out like result (the operand
+// of DivideAndRoundQLast, which may be result itself).  accumulate: add into result (KeySwitch) or store (rescale).
 __global__ void __launch_bounds__(kThreads)
-    ks_finish_kernel(u64* result, const u64* prod, const u64* tmp, u64 n, u64 kcc, u64 decomp, u64 i0, u64 count,
-                     const __grid_constant__ KsModuli mods) {
+    ks_finish_kernel(u64* result, const u64* in, const u64* tmp, u64 n, u64 kcc, u64 res_stride, u64 i0, u64 count,
+                     const __grid_constant__ KsModuli mods, int in_like_result, int accumulate) {
   const u64 per_mod = kcc * n;
   const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
   if (g >= per_mod * count) return;
   const u64 e = g / per_mod, r = g - e * per_mod;
   const u64 k = r / n, l = r - k * n;
   const KsModulus& md = mods.m[e];
-  u64 x = prod[g] + (md.q << 2) - tmp[g];
-  x = reduce_from<8>(x, md.q);
-  const u64 v = csub(shoup_lazy(x, md.a, md.b, md.q), md.q);
-  u64* dst = result + n * (decomp * k + i0 + e) + l;
-  *dst = csub(*dst + v, md.q);
+  const u64 d = n * (res_stride * k + i0 + e) + l;
+  const u64 v = finish_value(in[in_like_result ? d : g], tmp[g], md.q, md.a, md.b);
+  result[d] = accumulate ? csub(result[d] + v, md.q) : v;
+}
+
+// DivideAndRoundQLast in coefficient form: polynomial p of `polys` holds rns limbs of n words; every thread reads limb
+// rns-1 and limb i0+e of one coefficient, rounds and finishes in registers and stores limb i0+e.  Limb rns-1 is never
+// written, so result may be operand.  mods.m[e]: a, b = q_last^-1 mod q and its Shoup factor, c = the round's `add`.
+__global__ void __launch_bounds__(kThreads)
+    rescale_coef_kernel(u64* result, const u64* operand, u64 n, u64 rns, u64 i0, u64 count, u64 polys, u64 q_last,
+                        u64 mu_last, const __grid_constant__ KsModuli mods) {
+  const u64 per_poly = count * n;
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= per_poly * polys) return;
+  const u64 p = g / per_poly, r = g - p * per_poly;
+  const u64 e = r / n, l = r - e * n;
+  const KsModulus& md = mods.m[e];
+  const u64 base = p * rns * n + l, d = base + (i0 + e) * n;
+  const u64 t = round_into(operand[base + (rns - 1) * n], q_last, mu_last, md.q, md.mu, md.c);
+  result[d] = finish_value(operand[d], t, md.q, md.a, md.b);
 }
 
 unsigned blocks_for(u64 items) { return (unsigned)((items + kThreads - 1) / kThreads); }
@@ -252,10 +282,19 @@ cudaError_t launch_ks_round(u64* tmp, const u64* t_last, u64 n, u64 kcc, u64 q_l
   return cudaGetLastError();
 }
 
-cudaError_t launch_ks_finish(u64* result, const u64* prod, const u64* tmp, u64 n, u64 kcc, u64 decomp, u64 i0,
-                             u64 count, const KsModuli& mods, cudaStream_t stream) {
-  ks_finish_kernel<<<blocks_for(kcc * n * count), kThreads, 0, stream>>>(result, prod, tmp, n, kcc, decomp, i0, count,
-                                                                        mods);
+cudaError_t launch_ks_finish(u64* result, const u64* in, const u64* tmp, u64 n, u64 kcc, u64 res_stride, u64 i0,
+                             u64 count, const KsModuli& mods, bool in_like_result, bool accumulate,
+                             cudaStream_t stream) {
+  ks_finish_kernel<<<blocks_for(kcc * n * count), kThreads, 0, stream>>>(result, in, tmp, n, kcc, res_stride, i0, count,
+                                                                        mods, in_like_result, accumulate);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rescale_coef(u64* result, const u64* operand, u64 n, u64 rns, u64 i0, u64 count, u64 polys,
+                                u64 q_last, u64 mu_last, const KsModuli& mods, cudaStream_t stream) {
+  rescale_coef_kernel<<<blocks_for(count * n * polys), kThreads, 0, stream>>>(result, operand, n, rns, i0, count, polys,
+                                                                             q_last, mu_last, mods);
   count_launch();
   return cudaGetLastError();
 }

@@ -585,6 +585,15 @@ inline void KeySwitch(uint64_t* result, const uint64_t* t_target_iter_ptr, uint6
                                           modswitch_factors, stream));
 }
 
+// extension: rescale by the last RNS modulus, SEAL's RNSTool::divide_and_round_q_last(_ntt)_inplace batched over
+// `count` polynomials of rns_modulus_size limbs each (hexl_b200_divide_and_round_q_last in include/hexl_b200.h has the
+// layout and the argument rules).  Limb rns_modulus_size - 1 of result is not written; result may be operand.
+inline void DivideAndRoundQLast(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                                uint64_t rns_modulus_size, uint64_t count, bool ntt_form, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_divide_and_round_q_last(result, operand, n, moduli, rns_modulus_size, count,
+                                                       ntt_form ? 1 : 0, stream));
+}
+
 // extension: key-switch keys resident on the GPU(s).  The reference reads the keys from caller memory on every
 // call (key-switch.hpp:34-39); a host caller uploads them once here and then switches any number of
 // ciphertexts (`batch` of them back to back per call) without the keys crossing PCIe again.

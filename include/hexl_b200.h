@@ -251,6 +251,21 @@ int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, ui
                          const uint64_t* const* k_switch_keys, const uint64_t* modswitch_factors,
                          void* stream);
 
+/* Rescale by the last RNS modulus (extension; SEAL's RNSTool::divide_and_round_q_last_inplace and
+ * divide_and_round_q_last_ntt_inplace): the CKKS rescale after every multiplication, and BFV modulus switching.
+ * operand holds `count` polynomials back to back, each of rns_modulus_size = L + 1 limbs of n words; limb i of
+ * polynomial p is at (p * (L + 1) + i) * n and lies under moduli[i]; q_L = moduli[L] is the modulus dropped (the two
+ * components of a ciphertext are two consecutive polynomials).  result has the same layout: limbs 0..L-1 of every
+ * polynomial get floor((X + floor(q_L / 2)) / q_L) mod q_i, canonical, with X the CRT lift of the coefficient's limbs
+ * in [0, q_0 ... q_L); limb L is not written.  result == operand is allowed; otherwise the buffers must not overlap.
+ * ntt_form = 1 (CKKS): input and output limbs are in the forward-NTT form of GetNTT(n, q_i), as KeySwitch takes them;
+ * ntt_form = 0: plain coefficients.  Inputs must be below their modulus (checked under hexl_b200_set_debug(1)).
+ * HEXL_B200_ERR_INVALID_ARG unless every modulus is in (1, 2^61) and coprime to q_L, and in NTT form n is a power of
+ * two in [2, 2^20] and every modulus NTT-friendly for n (n >= 1 in coefficient form).  count = 0 does nothing.  The
+ * library computes q_L^-1 mod q_i itself.  Host buffers are staged by whole polynomials. */
+int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                                      uint64_t rns_modulus_size, uint64_t count, int ntt_form, void* stream);
+
 /* Key-switch keys resident on the GPU.  The reference keeps the keys in caller memory and reads them on every
  * call (key-switch.hpp:34-39); a host caller of hexl_b200_key_switch therefore pays decomp x key_component_count
  * x key_modulus_size x n words of PCIe traffic per call.  hexl_b200_keys_upload copies the `decomp` key buffers
