@@ -11,12 +11,14 @@
 namespace hexl_b200 {
 namespace {
 
+// Each thread loads the record of its own polynomial.  A column CTA lies inside one sub-block of one polynomial, but a
+// row CTA can span several: below N = 4096 a polynomial is one row of N / 16 threads and a CTA holds 4096 / N rows, so
+// with a small group its rows belong to polynomials under different moduli.
 __device__ __forceinline__ NttDeviceParams load_params(const NttMulti& multi, u64 poly) {
-  return *multi.p[poly / multi.group];  // uniform across the CTA (a CTA never spans two polynomials' moduli)
+  return *multi.p[poly / multi.group];
 }
 
-// rows of one CTA must share a modulus: ROWS divides rows_per_poly * group or the launcher
-// falls back to one row per ... (see launch_row_multi: grid is built per polynomial row set)
+// each row takes the modulus of its own polynomial (load_params per row), so a CTA may span moduli
 // MUL (inverse only): multiply by multi.mul on load -- a separate instantiation, so the plain inverse keeps its code
 template <int MODE, int LOGC, bool FWD, bool MUL = false>
 __global__ void __launch_bounds__(RowCfg<LOGC, MODE>::THREADS, RowCfg<LOGC, MODE>::MIN_BLOCKS)

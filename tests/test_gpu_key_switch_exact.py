@@ -8,7 +8,9 @@
 on the shapes the older tests never reach: moduli just below 2^61 with more digits than a 128-bit sum of lazy
 products can hold (where the reference's own accumulator wraps, so only the exact model knows the answer), more digits
 than one parameter block, a SEAL-style chain whose first digit prime is larger than the special prime, and moduli of
-all three word classes in one switch.  Every comparison is bit for bit."""
+all three word classes in one switch.  The last two also run at the degrees CKKS uses, N = 2^14, 2^16 and 2^17 (SEAL's
+largest), and a uniform chain at 2^18, where the transforms inside the switch take two column passes.  Every
+comparison is bit for bit."""
 import numpy as np
 import pytest
 
@@ -20,6 +22,11 @@ torch = pytest.importorskip("torch")
 
 GPU_CASES = ("wrap_keys", "wrap_blocks", "seal_chain", "word_classes")
 ENTRY_POINTS = ("device", "host", "resident", "sharded")
+# (case, log2 n) beyond each case's default degree: device and host pointers at each, every entry point at 2^17
+DEGREES = [(name, logn) for logn in (14, 16, 17) for name in ("seal_chain", "word_classes")] + [("uniform", 18)]
+CASES = ([(name, None, entry) for name in GPU_CASES for entry in ENTRY_POINTS]
+         + [(name, logn, entry) for name, logn in DEGREES
+            for entry in (ENTRY_POINTS if logn == 17 else ("device", "host"))])
 
 
 def dev(a):
@@ -39,17 +46,17 @@ def _need_cuda(hb):
 _cache = {}
 
 
-def _prepared(port, checker, name):
-    """(case, [(result, t_target)] x 2, [exact result] x 2), computed once per case"""
-    if name not in _cache:
-        case = ks_exact.make_case(port, name)
+def _prepared(port, checker, name, logn):
+    """(case, [(result, t_target)] x 2, [exact result] x 2), computed once per case and degree"""
+    if (name, logn) not in _cache:
+        case = ks_exact.make_case(port, name, None if logn is None else 1 << logn)
         cts = [ks_exact.ciphertext(case, seed) for seed in (1, 2)]
         exp = [ks_exact.expected(port, case, r, t) for r, t in cts]
         if not case.wraps:   # where the checker's accumulator cannot wrap, it must agree with the model
             r, t = cts[0]
             assert (checker.key_switch(r.copy(), t, *case.shape, case.keys, case.modswitch) == exp[0]).all(), name
-        _cache[name] = case, cts, exp
-    return _cache[name]
+        _cache[name, logn] = case, cts, exp
+    return _cache[name, logn]
 
 
 def _check(got, exp, what):
@@ -57,10 +64,11 @@ def _check(got, exp, what):
     assert wrong == 0, f"{what}: {wrong} of {exp.size} words differ from the exact key switch"
 
 
-@pytest.mark.parametrize("entry", ENTRY_POINTS)
-@pytest.mark.parametrize("name", GPU_CASES)
-def test_key_switch_equals_exact_model(hb, port, checker, name, entry):
-    case, cts, exp = _prepared(port, checker, name)
+@pytest.mark.parametrize("name,logn,entry", CASES,
+                         ids=[f"{name}{'' if logn is None else f'_n{logn}'}-{entry}" for name, logn, entry in CASES])
+def test_key_switch_equals_exact_model(hb, port, checker, name, logn, entry):
+    case, cts, exp = _prepared(port, checker, name, logn)
+    name = f"{name} n={case.n}"
     (r0, t0), (r1, t1) = cts
     if entry == "device":
         d = dev(r0)

@@ -30,6 +30,9 @@ SHAPES = {
     "tiny2": (2, "seal", 6, 3),
     "tiny4": (4, "seal", 6, 3),
     "tiny8": (8, "seal", 6, 3),
+    "seal_n16": (1 << 16, "seal", 31, 2),        # DESIGN §6's shape
+    "classes_n18": (1 << 18, "classes", 4, 2),  # from 2^18 on, the transforms take two column passes
+    "seal_n20": (1 << 20, "seal", 6, 1),        # the largest degree accepted
 }
 
 
