@@ -67,8 +67,10 @@ cudaError_t launch_col_dyn(int log_r, bool fwd, const NttDeviceTables& t, u64* r
   switch (log_r) {
     case 3: return launch_col<MODE, 3>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
     case 4: return launch_col<MODE, 4>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
-    case 5: return launch_col<MODE, 5>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
   }
+  // a radix-32 pass splits N = 2^17 only, where SMALL takes its distributed-shared-memory kernel instead
+  if constexpr (MODE != kSmall)
+    if (log_r == 5) return launch_col<MODE, 5>(fwd, t, result, operand, batch, log_s, out_mf, fold, stream);
   return cudaErrorInvalidValue;
 }
 

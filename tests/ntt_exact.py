@@ -1,4 +1,5 @@
-"""The negacyclic NTT in Python integers for the tests, and the moduli lists and inputs the multi-modulus tests run.
+"""The negacyclic NTT in Python integers for the tests, and the moduli and inputs the single- and multi-modulus tests
+run.
 
 forward() and inverse() are the transforms the library computes (hexl/ntt/ntt-internal.cpp): natural order in,
 bit-reversed order out, X[k] = sum_j x_j psi^((2 brv(k) + 1) j) with psi the minimal primitive 2N-th root of unity (or
@@ -11,6 +12,8 @@ tests/test_ntt_exact.py checks the model against the O(N^2) definition and pins 
 the GPU tests then compare against the faster checkers.
 """
 from __future__ import annotations
+
+import functools
 
 import numpy as np
 
@@ -29,6 +32,52 @@ MODULUS_LISTS = [
     ("generic_mixed", [(61, False), (29, False), (49, True)]),            # just below 2^62, below 2^30, 50 bits
 ]
 KINDS = ("top", "alternating", "uniform")
+
+# Primes of the single-modulus tests, GeneratePrimes(1, bits, first, 2^20) as above: the prime on each side of every
+# boundary of pick_mode (SMALL below 2^30, GENERIC in [2^30, 2^32), FAST in [2^32, 2^56), WIDE in [2^56, 2^61), GENERIC
+# from 2^61), the largest GENERIC prime, and one mid-range prime per mode.  single_primes() adds, per degree, the
+# smallest prime that is 1 mod 2N.
+SINGLE_PRIMES = [
+    ("below_2^30", (29, False)), ("above_2^30", (30, True)),
+    ("below_2^32", (31, False)), ("above_2^32", (32, True)),
+    ("below_2^56", (55, False)), ("above_2^56", (56, True)),
+    ("below_2^61", (60, False)), ("above_2^61", (61, True)),
+    ("below_2^62", (61, False)),
+    ("small_25bit", (24, True)), ("fast_50bit", (49, True)), ("wide_60bit", (59, True)),
+]
+SINGLE_NAMES = [name for name, _ in SINGLE_PRIMES] + ["smallest"]
+
+
+def smallest_prime(n):
+    """the smallest prime q = 1 mod 2n"""
+    q = 2 * n + 1
+    while any(q % d == 0 for d in range(2, int(q ** 0.5) + 1)):
+        q += 2 * n
+    return q
+
+
+@functools.lru_cache(maxsize=None)
+def _fixed_primes(primes):
+    return tuple((name, int(primes(1, bits, first, 1 << MAX_LOGN)[0])) for name, (bits, first) in SINGLE_PRIMES)
+
+
+def single_primes(primes, logn):
+    """[(name, q)] of SINGLE_NAMES for N = 2^logn; primes(num, bits, first, n) is GeneratePrimes"""
+    return list(_fixed_primes(primes)) + [("smallest", smallest_prime(1 << logn))]
+
+
+def single_polynomial(kind, seed, n, q, in_mf):
+    """n values below in_mf * q whose residues mod q do not depend on in_mf, so one transform of the model serves
+    every input factor: all at in_mf * q - 1, 0 alternating with that value, or uniform below q plus a uniform multiple
+    of q below in_mf * q"""
+    if kind != "uniform":
+        return polynomial(kind, seed, n, in_mf * q)
+    return uniform_below(seed, n, q) + U64(q) * uniform_below(seed + 1, n, in_mf)
+
+
+def single_operand(seed, n, q, batch, in_mf):
+    """`batch` polynomials under one modulus, polynomial u of kind KINDS[u % 3] and seed seed + 2u"""
+    return np.concatenate([single_polynomial(KINDS[u % 3], seed + 2 * u, n, q, in_mf) for u in range(batch)])
 
 
 def moduli(primes, spec):

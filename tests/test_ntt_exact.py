@@ -4,7 +4,8 @@ inputs of the multi-modulus GPU tests.  CPU only.
 The GPU tests of the multi-modulus transforms compare against the checkers (the C restatement, or the compiled
 reference), so the checkers are pinned here: at every moduli list those tests use, from N = 2 to N = 2^20, on inputs
 at in_mf * q - 1, 0 alternating with that value, and uniform below in_mf * q, their canonical outputs equal the model's
-word for word."""
+word for word.  The same holds at the primes of the single-modulus GPU tests (ntt_exact.SINGLE_PRIMES) that the lists
+do not hold, on those tests' inputs."""
 import numpy as np
 import pytest
 
@@ -89,3 +90,38 @@ def test_checkers_equal_the_model_at_two_column_passes(request, port, checker_ki
     chk = _checker(request, port, checker_kind)
     _check(chk, port, name, logn, 1, True, 4)
     _check(chk, port, name, logn, 1, False, 2)
+
+
+# the primes of the single-modulus GPU tests that no moduli list above holds
+SINGLE_PINNED = ["above_2^30", "above_2^56", "above_2^61", "smallest"]
+_single_model = {}
+
+
+def _single_expected(q, logn, kind, fwd):
+    """the model's transform of one polynomial of `kind`; its residues, hence the model, do not depend on in_mf"""
+    key = q, logn, kind, fwd
+    if key not in _single_model:
+        n = 1 << logn
+        x = nx.single_polynomial(kind, logn, n, q, 1)
+        _single_model[key] = (nx.forward if fwd else nx.inverse)(x, n, q)
+    return _single_model[key]
+
+
+@pytest.mark.parametrize("checker_kind", ["port", "ref"])
+@pytest.mark.parametrize("logn", range(1, nx.MAX_LOGN + 1))
+def test_checkers_equal_the_model_at_single_primes(request, port, checker_kind, logn):
+    """tests/test_gpu_ntt_degrees.py's inputs: every input factor and kind at every degree"""
+    chk = _checker(request, port, checker_kind)
+    n = 1 << logn
+    primes = dict(nx.single_primes(port.generate_primes, logn))
+    for name in SINGLE_PINNED:
+        q = primes[name]
+        for fwd, in_mfs in ((True, (1, 2, 4)), (False, (1, 2))):
+            run = chk.ntt_forward if fwd else chk.ntt_inverse
+            for kind in nx.KINDS:
+                exp = _single_expected(q, logn, kind, fwd)
+                for in_mf in in_mfs:
+                    got = run(nx.single_polynomial(kind, logn, n, q, in_mf), n, q, in_mf, 1)
+                    wrong = int((got != exp).sum())
+                    assert wrong == 0, (f"{chk.kind} {'fwd' if fwd else 'inv'} {name} q={q} n=2^{logn} {kind} "
+                                        f"in_mf={in_mf}: {wrong} words")
