@@ -113,6 +113,7 @@ _sig("hexl_b200_ntt_get_cached", _int, [C.POINTER(_vp), _u64, _u64])
 _sig("hexl_b200_dyadic_multiply", _int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp])
 _sig("hexl_b200_key_switch", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _vp])
 _sig("hexl_b200_divide_and_round_q_last", _int, [_vp, _vp, _u64, _vp, _u64, _u64, _int, _vp])
+_sig("hexl_b200_apply_galois", _int, [_vp, _vp, _u64, _vp, _u64, _u64, _u64, _int, _vp])
 
 _sig("hexl_b200_hensel_lemma_2adic_root", _u64, [C.c_uint32, _u64])
 _sig("hexl_b200_montgomery_reduce", _u64, [_u64, _u64, _u64, _int, _u64])
@@ -123,6 +124,7 @@ _sig("hexl_b200_keys_upload", _int, [C.POINTER(_vp), _vp, _u64, _u64, _u64, _u64
 _sig("hexl_b200_keys_upload_sharded", _int, [C.POINTER(_vp), _vp, _u64, _u64, _u64, _u64])
 _sig("hexl_b200_keys_release", None, [_vp])
 _sig("hexl_b200_key_switch_resident", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp])
+_sig("hexl_b200_apply_galois_key_switch", _int, [_vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -551,3 +553,31 @@ def KeySwitchResident(result, t_target_iter_ptr, n, decomp_modulus_size, key_mod
                                               key_component_count, mods.ctypes.data, keys._h, ms.ctypes.data, batch,
                                               _stream(stream, rc or tc)))
     return result
+
+
+def ApplyGalois(result, operand, n, moduli, rns_modulus_size, count, galois_elt, ntt_form=True, stream=None):
+    """The Galois automorphism a(X) -> a(X^galois_elt) of `count` polynomials of rns_modulus_size limbs (n words each),
+    in NTT or coefficient form (hexl_b200_apply_galois); result may be operand."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); op, on, oc = _buf(operand)
+    _need("moduli", mods.size, rns_modulus_size)
+    _need("result", rn, count * rns_modulus_size * n); _need("operand", on, count * rns_modulus_size * n)
+    _check(_lib.hexl_b200_apply_galois(rp, op, n, mods.ctypes.data, rns_modulus_size, count, galois_elt,
+                                       int(bool(ntt_form)), _stream(stream, rc or oc)))
+    return result
+
+
+def ApplyGaloisKeySwitch(ciphertexts, n, decomp_modulus_size, key_modulus_size, rns_modulus_size, key_component_count,
+                         moduli, galois_keys: KeySwitchKeys, modswitch_factors, galois_elt, batch=1, stream=None):
+    """Rotation or conjugation of `batch` ciphertexts in place (hexl_b200_apply_galois_key_switch): ciphertext c is
+    ciphertexts[c * 2*decomp*n:], c0 <- sigma(c0) + KS_0(sigma(c1)), c1 <- KS_1(sigma(c1))."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    ms = np.ascontiguousarray(modswitch_factors, dtype=np.uint64)
+    cp, cn, cc = _buf(ciphertexts)
+    _need("moduli", mods.size, key_modulus_size); _need("modswitch_factors", ms.size, decomp_modulus_size)
+    _need("ciphertexts", cn, batch * key_component_count * decomp_modulus_size * n)
+    _check(_lib.hexl_b200_apply_galois_key_switch(cp, n, decomp_modulus_size, key_modulus_size, rns_modulus_size,
+                                                  key_component_count, mods.ctypes.data,
+                                                  galois_keys._h if galois_keys is not None else None, ms.ctypes.data,
+                                                  galois_elt, batch, _stream(stream, cc)))
+    return ciphertexts

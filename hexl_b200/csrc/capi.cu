@@ -1568,13 +1568,32 @@ int hexl_b200_dyadic_multiply(uint64_t* result, const uint64_t* operand1, const 
   return 0;
 }
 
+// The rotation of one ciphertext (two components of decomp limbs in NTT form, device memory): sigma_g of both
+// components into perm (2 x decomp x n words of scratch) in one launch, then c0 <- sigma_g(c0), c1 <- 0 by stream
+// copies and the key switch of t_target = sigma_g(c1), which accumulates KS(sigma_g(c1)) into both components.
+static int galois_key_switch_on_device(int dev, uint64_t* ct, uint64_t* perm, uint64_t n, uint64_t decomp,
+                                       uint64_t key_modulus_size, uint64_t rns, const uint64_t* moduli,
+                                       const uint64_t* const* d_key_ptrs_host, const uint64_t* modswitch,
+                                       uint64_t galois_elt, cudaStream_t s) {
+  const uint64_t comp = decomp * n;
+  const cudaError_t e = launch_galois_ntt(perm, ct, floor_log2(n), 2 * decomp, galois_elt, s);
+  if (e != cudaSuccess) return cuda_fail(e, "ApplyGaloisKeySwitch: automorphism launch");
+  CU(cudaMemcpyAsync(ct, perm, comp * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+  CU(cudaMemsetAsync(ct + comp, 0, comp * sizeof(uint64_t), s));
+  return key_switch_on_device(dev, ct, perm + comp, n, decomp, key_modulus_size, rns, 2, moduli, d_key_ptrs_host,
+                              modswitch, s);
+}
+
 // One or more key switches on HOST buffers against keys already on the devices: ciphertext c occupies
 // result[c * kcc*decomp*n ...] and t_target[c * decomp*n ...].  Each ciphertext runs on one of the rotating
 // staging streams (digits in, result in, ~12 kernels, result out), so the copies of one ciphertext overlap the
 // kernels of its neighbours; with host devices set the batch is split across the GPUs holding the keys.
+// galois_elt != 0: the rotation of ApplyGaloisKeySwitch instead (kcc = 2, t_target unused): only the ciphertext
+// crosses PCIe, and the slot's second buffer holds both permuted components.
 static int key_switch_host_batch(uint64_t* result, const uint64_t* t_target, uint64_t n, uint64_t decomp,
                                  uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
-                                 const hexl_b200_keys* keys, const uint64_t* modswitch, uint64_t batch) {
+                                 const hexl_b200_keys* keys, const uint64_t* modswitch, uint64_t batch,
+                                 uint64_t galois_elt = 0) {
   std::vector<int> devs = host_devices();
   if (devs.empty()) {
     int cur = 0;
@@ -1600,16 +1619,22 @@ static int key_switch_host_batch(uint64_t* result, const uint64_t* t_target, uin
     int slot = 0;
     for (u64 c = c_lo; c < c_hi && !rc; ++c, slot = (slot + 1) % kSlots) {
       if ((rc = st->reserve(slot, 0, res_elems * 8))) break;
-      if ((rc = st->reserve(slot, 1, t_elems * 8))) break;
+      if ((rc = st->reserve(slot, 1, (galois_elt ? 2 : 1) * t_elems * 8))) break;
       cudaStream_t sx = st->stream[slot];
       u64 *d_res = st->buf[slot][0], *d_t = st->buf[slot][1];
-      cudaError_t e = cudaMemcpyAsync(d_t, t_target + c * t_elems, t_elems * 8, cudaMemcpyHostToDevice, sx);
+      cudaError_t e = cudaSuccess;
+      if (!galois_elt) e = cudaMemcpyAsync(d_t, t_target + c * t_elems, t_elems * 8, cudaMemcpyHostToDevice, sx);
       if (e == cudaSuccess) e = cudaMemcpyAsync(d_res, result + c * res_elems, res_elems * 8, cudaMemcpyHostToDevice, sx);
       if (e != cudaSuccess) {
         rc = cuda_fail(e, "KeySwitch H2D");
         break;
       }
-      rc = key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, kcc, moduli, dk.data(), modswitch, sx);
+      if (galois_elt)
+        rc = galois_key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, moduli, dk.data(),
+                                         modswitch, galois_elt, sx);
+      else
+        rc = key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, kcc, moduli, dk.data(), modswitch,
+                                  sx);
       if (rc) break;
       e = cudaMemcpyAsync(result + c * res_elems, d_res, res_elems * 8, cudaMemcpyDeviceToHost, sx);
       if (e != cudaSuccess) rc = cuda_fail(e, "KeySwitch D2H");
@@ -2109,6 +2134,144 @@ int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand,
   return run_host(result, operand, nullptr, total, unit,
                   [&](int dev, u64, u64) { return Launch{true, 0, dev, n, rns, unit, moduli, ntt, h.data()}; },
                   L * n);
+}
+
+// ---------------------------------------------------------------- Galois automorphisms
+static int galois_elt_check(uint64_t n, uint64_t galois_elt) {
+  REQUIRE(galois_elt % 2 == 1 && galois_elt < 2 * n, "Require galois_elt odd and in [1, 2n)");
+  return 0;
+}
+
+// g^-1 mod 2n (g odd): Newton's iteration doubles the correct low bits of an inverse mod 2^64 (g is its own inverse
+// mod 8), so five steps give all 64
+static uint64_t galois_inverse(uint64_t g, uint64_t n) {
+  uint64_t inv = g;
+  for (int i = 0; i < 5; ++i) inv *= 2 - g * inv;
+  return inv & (2 * n - 1);
+}
+
+// `count` polynomials of rns limbs x n words, device pointers on the current device.  NTT form: one launch over every
+// limb; coefficient form: one launch per block of kParamBlock moduli.  In place, the polynomials are first copied into
+// pool scratch (at most ~256 MiB at a time, whole polynomials) and permuted from there back into result.
+static int apply_galois_on_device(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                                  uint64_t rns, uint64_t count, uint64_t galois_elt, bool ntt_form, cudaStream_t s) {
+  const int log_n = floor_log2(n);
+  const uint64_t g_inv = galois_inverse(galois_elt, n), unit = rns * n;
+  auto permute = [&](uint64_t* r, const uint64_t* a, uint64_t polys) -> int {
+    if (ntt_form) {
+      cudaError_t e = launch_galois_ntt(r, a, log_n, polys * rns, galois_elt, s);
+      if (e != cudaSuccess) return cuda_fail(e, "ApplyGalois launch");
+      return 0;
+    }
+    for (uint64_t i0 = 0; i0 < rns; i0 += kParamBlock) {
+      const uint64_t cnt = std::min<uint64_t>(kParamBlock, rns - i0);
+      GaloisModuli mods;
+      for (uint64_t e = 0; e < cnt; ++e) mods.q[e] = moduli[i0 + e];
+      cudaError_t e = launch_galois_coef(r, a, log_n, rns, i0, cnt, polys, g_inv, mods, s);
+      if (e != cudaSuccess) return cuda_fail(e, "ApplyGalois launch");
+    }
+    return 0;
+  };
+  if (result != operand) return permute(result, operand, count);
+  const uint64_t chunk = std::min<uint64_t>(count, std::max<uint64_t>(1, (256ull << 20) / (unit * 8)));
+  Scratch ws(s);
+  uint64_t* copy = nullptr;
+  if (int rc = ws.get(&copy, chunk * unit)) return rc;
+  for (uint64_t p0 = 0; p0 < count; p0 += chunk) {
+    const uint64_t cnt = std::min(chunk, count - p0);
+    CU(cudaMemcpyAsync(copy, result + p0 * unit, cnt * unit * 8, cudaMemcpyDeviceToDevice, s));
+    if (int rc = permute(result + p0 * unit, copy, cnt)) return rc;
+  }
+  return 0;  // ~Scratch returns the copy to the pool in stream order
+}
+
+int hexl_b200_apply_galois(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                           uint64_t rns_modulus_size, uint64_t count, uint64_t galois_elt, int ntt_form, void* stream) {
+  REQUIRE(result && operand && moduli, "Require result, operand, moduli != nullptr");
+  REQUIRE(rns_modulus_size >= 1, "Require rns_modulus_size >= 1");
+  REQUIRE(ntt_form == 0 || ntt_form == 1, "Require ntt_form = 0 or 1");
+  REQUIRE(n >= 2 && n <= (1ull << 20) && !(n & (n - 1)), "Require n a power of two in [2, 2^20]");
+  const uint64_t rns = rns_modulus_size;
+  for (uint64_t i = 0; i < rns; ++i)
+    REQUIRE(moduli[i] > 1 && moduli[i] < (1ull << 62), "Require 1 < moduli[%llu] < 2^62", (unsigned long long)i);
+  if (int rc = galois_elt_check(n, galois_elt)) return rc;
+  if (count == 0) return 0;
+  const uint64_t unit = rns * n, total = count * unit;
+  REQUIRE(result == operand || result + total <= operand || operand + total <= result,
+          "result and operand must be the same buffer or not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, operand}, &pi)) return rc;
+  if (g_debug.load())
+    for (uint64_t p = 0; p < count; ++p)
+      for (uint64_t i = 0; i < rns; ++i)
+        if (int rc = check_bounds(operand + p * unit + i * n, n, moduli[i], pi, "operand")) return rc;
+  const bool ntt = ntt_form != 0;
+  if (pi.where == Where::Device) {
+    DeviceGuard g;
+    if (int rc = g.enter(pi.device)) return rc;
+    if (int rc = apply_galois_on_device(result, operand, n, moduli, rns, count, galois_elt, ntt, (cudaStream_t)stream))
+      return rc;
+    return finish_device_call(pi, stream);
+  }
+  // host pointers: whole polynomials through the staging slots (split over the host devices when set); the staged
+  // polynomials are permuted in place on the device
+  struct Launch {
+    bool ok = true;
+    int rc = 0;
+    uint64_t n, rns, unit, galois_elt;
+    const uint64_t* moduli;
+    bool ntt;
+    int operator()(u64* r, const u64* a, const u64*, u64, u64 elems, cudaStream_t s) const {
+      return apply_galois_on_device(r, a, n, moduli, rns, elems / unit, galois_elt, ntt, s);
+    }
+  };
+  return run_host(result, operand, nullptr, total, unit,
+                  [&](int, u64, u64) { return Launch{true, 0, n, rns, unit, galois_elt, moduli, ntt}; });
+}
+
+int hexl_b200_apply_galois_key_switch(uint64_t* ciphertexts, uint64_t n, uint64_t decomp_modulus_size,
+                                      uint64_t key_modulus_size, uint64_t rns_modulus_size,
+                                      uint64_t key_component_count, const uint64_t* moduli,
+                                      const hexl_b200_keys* galois_keys, const uint64_t* modswitch_factors,
+                                      uint64_t galois_elt, uint64_t batch, void* stream) {
+  const uint64_t decomp = decomp_modulus_size, rns = rns_modulus_size, kcc = key_component_count;
+  if (int rc = key_switch_check(ciphertexts, ciphertexts, n, decomp, key_modulus_size, rns, kcc, moduli,
+                                modswitch_factors))
+    return rc;
+  REQUIRE(kcc == 2, "Require key_component_count == 2 (a ciphertext of two components)");
+  REQUIRE(n <= (1ull << 20), "Require n <= 2^20");
+  if (int rc = galois_elt_check(n, galois_elt)) return rc;
+  REQUIRE(galois_keys != nullptr, "Require galois_keys != nullptr");
+  REQUIRE(galois_keys->n == n && galois_keys->decomp >= decomp && galois_keys->kcc == kcc &&
+              galois_keys->kms == key_modulus_size,
+          "the key handle was uploaded for another shape");
+  REQUIRE(galois_keys->shards.empty(),
+          "ApplyGaloisKeySwitch does not take keys sharded by modulus: upload them with hexl_b200_keys_upload");
+  if (batch == 0) return 0;
+  PtrInfo pi;
+  if (int rc = classify_all({ciphertexts}, &pi)) return rc;
+  const uint64_t comp = decomp * n;
+  if (g_debug.load())
+    for (uint64_t c = 0; c < 2 * batch; ++c)
+      for (uint64_t i = 0; i < decomp; ++i)
+        if (int rc = check_bounds(ciphertexts + c * comp + i * n, n, moduli[i], pi, "ciphertexts")) return rc;
+  if (pi.where == Where::Host)
+    return key_switch_host_batch(ciphertexts, nullptr, n, decomp, key_modulus_size, rns, kcc, moduli, galois_keys,
+                                 modswitch_factors, batch, galois_elt);
+  auto it = galois_keys->dev.find(pi.device);
+  if (it == galois_keys->dev.end())
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "the key handle holds no copy on the device of the ciphertexts");
+  DeviceGuard g;
+  if (int rc = g.enter(pi.device)) return rc;
+  Scratch ws((cudaStream_t)stream);
+  uint64_t* perm = nullptr;
+  if (int rc = ws.get(&perm, 2 * comp)) return rc;
+  for (uint64_t c = 0; c < batch; ++c)
+    if (int rc = galois_key_switch_on_device(pi.device, ciphertexts + c * 2 * comp, perm, n, decomp, key_modulus_size,
+                                             rns, moduli, it->second.data(), modswitch_factors, galois_elt,
+                                             (cudaStream_t)stream))
+      return rc;
+  return finish_device_call(pi, stream);
 }
 
 }  // extern "C"

@@ -153,6 +153,18 @@ cudaError_t launch_ks_finish(u64* result, const u64* in, const u64* tmp, u64 n, 
 cudaError_t launch_rescale_coef(u64* result, const u64* operand, u64 n, u64 rns, u64 i0, u64 count, u64 polys,
                                 u64 q_last, u64 mu_last, const KsModuli& mods, cudaStream_t stream);
 
+// Galois automorphism sigma_g (galois.cu).  NTT form: `polys` polynomials of 2^log_n words, one launch, words move
+// unchanged (result[j] = operand[pi_g(j)]).  Coefficient form: limbs [i0, i0 + cnt) of `polys` polynomials of rns
+// limbs each, limb i0 + e under mods.q[e]; galois_inv = g^-1 mod 2n.  result and operand must not overlap.
+constexpr u64 kGaloisSmemMaxN = 1ull << 14;  // coefficient form: a limb is staged in shared memory up to this degree
+struct GaloisModuli {
+  u64 q[kParamBlock];
+};
+cudaError_t launch_galois_ntt(u64* result, const u64* operand, int log_n, u64 polys, u64 galois_elt,
+                              cudaStream_t stream);
+cudaError_t launch_galois_coef(u64* result, const u64* operand, int log_n, u64 rns, u64 i0, u64 cnt, u64 polys,
+                               u64 galois_inv, const GaloisModuli& mods, cudaStream_t stream);
+
 // Stream-ordered scratch from the library's own memory pool (capi.cu): kept warm between calls, capturable.
 cudaError_t scratch_alloc_async(void** p, size_t bytes, cudaStream_t stream);
 void scratch_free_async(void* p, cudaStream_t stream);

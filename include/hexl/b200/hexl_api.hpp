@@ -632,5 +632,29 @@ inline void KeySwitch(uint64_t* result, const uint64_t* t_target_iter_ptr, uint6
                                                    modswitch_factors, batch, stream));
 }
 
+// extension: the Galois automorphism a(X) -> a(X^galois_elt) of `count` polynomials of rns_modulus_size limbs each,
+// in NTT or coefficient form (hexl_b200_apply_galois in include/hexl_b200.h has the layout, the formulas and the
+// argument rules); result may be operand.
+inline void ApplyGalois(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                        uint64_t rns_modulus_size, uint64_t count, uint64_t galois_elt, bool ntt_form,
+                        void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_apply_galois(result, operand, n, moduli, rns_modulus_size, count, galois_elt,
+                                            ntt_form ? 1 : 0, stream));
+}
+
+// extension: rotation or conjugation of `batch` ciphertexts in NTT form, in place -- SEAL's apply_galois_inplace:
+// c0 <- sigma(c0) + KS_0(sigma(c1)), c1 <- KS_1(sigma(c1)) with the Galois keys of galois_elt
+// (hexl_b200_apply_galois_key_switch).  key_component_count must be 2; sharded key handles are refused.
+inline void ApplyGaloisKeySwitch(uint64_t* ciphertexts, uint64_t n, uint64_t decomp_modulus_size,
+                                 uint64_t key_modulus_size, uint64_t rns_modulus_size, uint64_t key_component_count,
+                                 const uint64_t* moduli, const b200::KeySwitchKeys& galois_keys,
+                                 const uint64_t* modswitch_factors, uint64_t galois_elt, uint64_t batch = 1,
+                                 void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_apply_galois_key_switch(ciphertexts, n, decomp_modulus_size, key_modulus_size,
+                                                       rns_modulus_size, key_component_count, moduli,
+                                                       galois_keys.Handle(), modswitch_factors, galois_elt, batch,
+                                                       stream));
+}
+
 }  // namespace hexl
 }  // namespace intel

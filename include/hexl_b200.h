@@ -266,6 +266,25 @@ int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, ui
 int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
                                       uint64_t rns_modulus_size, uint64_t count, int ntt_form, void* stream);
 
+/* Galois automorphism sigma_g : a(X) -> a(X^g) of RNS polynomials (extension; the permutation of SEAL's
+ * Evaluator::apply_galois_inplace, behind every rotation and conjugation of CKKS, BFV and BGV).  Layout as for
+ * hexl_b200_divide_and_round_q_last: `count` polynomials back to back, each of rns_modulus_size limbs of n words, limb
+ * i under moduli[i].  galois_elt = g is odd with 1 <= g < 2n; n is a power of two in [2, 2^20].
+ *   ntt_form = 0 (coefficients): coefficient i moves to k = i g mod 2n; result[k] = operand[i] if k < n, otherwise
+ *     result[k - n] = (q - operand[i]) mod q.  Inputs must be below q; outputs are canonical.
+ *   ntt_form = 1 (the forward-NTT order of GetNTT(n, q), slot j holding a(psi^(2 rev(j) + 1))):
+ *     result[j] = operand[pi_g(j)], pi_g(j) = rev(((g (2 rev(j) + 1)) mod 2n - 1) / 2), rev the bit reversal on
+ *     log2 n bits.  Words move unchanged; pi_g depends neither on q nor on the root, so the moduli are read only by
+ *     the range check.
+ * Inputs are checked below their modulus under hexl_b200_set_debug(1).  HEXL_B200_ERR_INVALID_ARG unless every
+ * pointer is non-null, every modulus is in (1, 2^62), g is as above and result == operand or the buffers do not
+ * overlap.  count = 0 does nothing.  NTT form is one launch for the whole call; coefficient form one per block of 64
+ * moduli.  In place (result == operand) the polynomials are first copied into library scratch and permuted from
+ * there: one device copy of the data more than out of place.  Host buffers are staged by whole polynomials (and
+ * permuted in place on the device) and split by polynomial over the devices of hexl_b200_set_host_devices. */
+int hexl_b200_apply_galois(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                           uint64_t rns_modulus_size, uint64_t count, uint64_t galois_elt, int ntt_form, void* stream);
+
 /* Key-switch keys resident on the GPU.  The reference keeps the keys in caller memory and reads them on every
  * call (key-switch.hpp:34-39); a host caller of hexl_b200_key_switch therefore pays decomp x key_component_count
  * x key_modulus_size x n words of PCIe traffic per call.  hexl_b200_keys_upload copies the `decomp` key buffers
@@ -292,6 +311,25 @@ int hexl_b200_key_switch_resident(uint64_t* result, const uint64_t* t_target_ite
                                   uint64_t decomp_modulus_size, uint64_t key_modulus_size, uint64_t rns_modulus_size,
                                   uint64_t key_component_count, const uint64_t* moduli, const hexl_b200_keys* keys,
                                   const uint64_t* modswitch_factors, uint64_t batch, void* stream);
+
+/* Rotation or conjugation of `batch` ciphertexts in place (extension; SEAL's Evaluator::apply_galois_inplace for a
+ * ciphertext in NTT form).  Ciphertext c is at ciphertexts + c * 2 * decomp * n, laid out like KeySwitch's result:
+ * components c0 and c1 of decomp limbs in NTT form, limb i under moduli[i], every word canonical (checked under
+ * hexl_b200_set_debug(1)).  For each ciphertext:
+ *   c0 <- sigma_g(c0) + KS_0(sigma_g(c1)),  c1 <- KS_1(sigma_g(c1)),
+ * with sigma_g the NTT-form automorphism of hexl_b200_apply_galois and KS the function of hexl_b200_key_switch
+ * applied to a zero result; bit for bit the chain r = [sigma_g(c0), 0]; hexl_b200_key_switch_resident(r, sigma_g(c1)).
+ * galois_keys: the key-switch keys for g, uploaded with hexl_b200_keys_upload.  HEXL_B200_ERR_INVALID_ARG on the
+ * shape rules of hexl_b200_key_switch_resident, unless key_component_count == 2 and n <= 2^20, for g outside the
+ * rules of hexl_b200_apply_galois, and for a handle sharded by modulus (not supported here).  On the device, one
+ * automorphism launch over both components into scratch, a copy and a memset, then the key switch: one launch more
+ * per ciphertext than hexl_b200_key_switch_resident.  Host buffers cross PCIe once each way per ciphertext, pipelined
+ * and split over the devices holding the keys as for hexl_b200_key_switch_resident. */
+int hexl_b200_apply_galois_key_switch(uint64_t* ciphertexts, uint64_t n, uint64_t decomp_modulus_size,
+                                      uint64_t key_modulus_size, uint64_t rns_modulus_size,
+                                      uint64_t key_component_count, const uint64_t* moduli,
+                                      const hexl_b200_keys* galois_keys, const uint64_t* modswitch_factors,
+                                      uint64_t galois_elt, uint64_t batch, void* stream);
 
 #ifdef __cplusplus
 }
