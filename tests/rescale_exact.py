@@ -60,6 +60,36 @@ def rescale_integer(operand, n, moduli, count):
     return out.reshape(-1)
 
 
+def rescale_per_limb(operand, n, moduli, count):
+    """Coefficient form limb by limb, with Python integers: (x_i + h - ((x_L + h) mod q_L)) * q_L^-1 mod q_i.  Equal to
+    rescale_integer() where the CRT lift exists, and still defined where the q_i share factors with each other (each
+    q_i coprime to q_L)."""
+    moduli = [int(q) for q in moduli]
+    rns = len(moduli)
+    q_last, half = moduli[-1], moduli[-1] >> 1
+    x = np.asarray(operand, dtype=U64).reshape(count, rns, n)
+    out = x.copy()
+    t = (x[:, -1].astype(object) + half) % q_last
+    for i, q in enumerate(moduli[:-1]):
+        out[:, i] = ((x[:, i].astype(object) + half - t) * pow(q_last, -1, q) % q).astype(U64)
+    return out.reshape(-1)
+
+
+def edge_values(moduli, n, seed):
+    """One polynomial per edge class, as integers ([row][n]): X = 0, X = Q - 1, and X mod q_L in {h - 1, h, h + 1}
+    (a random multiple of q_L below Q added), so (X + h) / q_L falls just below, on and just above an integer"""
+    Q = 1
+    for q in moduli:
+        Q *= q
+    q_last = moduli[-1]
+    half = q_last >> 1
+    ks = [int(v) for v in uniform_below(seed, 3 * n, 1 << 63)]
+    rows = [[0] * n, [Q - 1] * n]
+    for j, off in enumerate((half - 1, half, half + 1)):
+        rows.append([(ks[j * n + l] * (Q // q_last) >> 63) * q_last + off for l in range(n)])
+    return rows
+
+
 def limbs_of(values, moduli):
     """Integers (one per coefficient, [count][n]) -> the operand layout [count][rns][n]"""
     values = [[int(v) for v in row] for row in values]

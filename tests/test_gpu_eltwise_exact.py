@@ -2,6 +2,7 @@
 to each operation's own modulus limit:
 
     MultMod, MultModMulti, DyadicMultiply    q < 2^62 (MultMod: input_mod_factor * q < 2^63)
+    AddModMulti, SubModMulti                 q < 2^62
     AddMod, SubMod (vector and scalar)       q < 2^63
     FMAMod                                   q < 2^61
     ReduceMod, CmpSubMod                     any q > 1
@@ -155,6 +156,47 @@ def test_mult_mod_multi(hb, in_mf, per_mod):
     hb.EltwiseMultModMulti(h, a, b, per_mod, moduli, in_mf)
     verdict("host pointers", h)
     _report(bad, f"EltwiseMultModMulti in_mf={in_mf} moduli={moduli}")
+
+
+# the largest prime below 2^62 and the largest modulus accepted (2^62 - 1, composite), a 60-bit, a 29-bit prime and 3
+ADDSUB_MULTI_MODULI = [ee.prime_below(1 << 62), (1 << 62) - 1, ee.prime_below(1 << 60), ee.prime_below(1 << 29), 3]
+
+
+@pytest.mark.parametrize("op", ["add", "sub"])
+@pytest.mark.parametrize("per_mod", [4096, 4099])   # 128-bit and scalar instantiations
+def test_add_sub_mod_multi(hb, op, per_mod):
+    """every edge pair of each modulus (a sum of exactly q, a difference of exactly 0 or -1) in one call"""
+    moduli = ADDSUB_MULTI_MODULI
+    fn, model = (hb.EltwiseAddModMulti, ee.add_mod) if op == "add" else (hb.EltwiseSubModMulti, ee.sub_mod)
+    a, b = _rns_operands(moduli, 1, per_mod, 80 + per_mod % 7)
+    exp = np.concatenate([model(a[i * per_mod:(i + 1) * per_mod], b[i * per_mod:(i + 1) * per_mod], q)
+                          for i, q in enumerate(moduli)])
+    total = per_mod * len(moduli)
+    bad = []
+
+    def verdict(what, got):
+        for i, q in enumerate(moduli):
+            w = ee.wrong_words(got[i * per_mod:(i + 1) * per_mod], exp[i * per_mod:(i + 1) * per_mod])
+            if w:
+                bad.append(f"{what}, q={q}: {w} of {per_mod} words wrong")
+
+    r = torch.empty(total, dtype=torch.int64, device="cuda")
+    fn(r, dev(a), dev(b), per_mod, moduli)
+    verdict("device", host(r))
+    da = dev(a)
+    fn(da, da, dev(b), per_mod, moduli)
+    verdict("in place", host(da))
+    bufs = [torch.zeros(total + 2, dtype=torch.int64, device="cuda") for _ in range(3)]
+    bufs[1][1:-1], bufs[2][1:-1] = dev(a), dev(b)
+    fn(bufs[0][1:-1], bufs[1][1:-1], bufs[2][1:-1], per_mod, moduli)
+    got = host(bufs[0])
+    verdict("offset view", got[1:-1])
+    if got[0] or got[-1]:
+        bad.append("offset view: guard word overwritten")
+    h = np.zeros(total, dtype=np.uint64)
+    fn(h, a, b, per_mod, moduli)
+    verdict("host pointers", h)
+    _report(bad, f"Eltwise{op.capitalize()}ModMulti moduli={moduli}")
 
 
 # ------------------------------------------------------------------------------------------------ DyadicMultiply

@@ -13,7 +13,6 @@ import numpy as np
 import pytest
 
 import rescale_exact as rx
-from util import uniform_below
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CHAINS = ("seal", "classes", "wide", "small")
@@ -22,20 +21,6 @@ U64 = np.uint64
 
 def _mods(port, name, n):
     return rx.chain(port.generate_primes, n, name)
-
-
-def _edge_values(moduli, n, seed):
-    """One polynomial per edge class: X = 0, X = Q - 1, and X mod q_L in {h - 1, h, h + 1} (random multiple of q_L)"""
-    Q = 1
-    for q in moduli:
-        Q *= q
-    q_last = moduli[-1]
-    half = q_last >> 1
-    ks = [int(v) for v in uniform_below(seed, 3 * n, 1 << 63)]
-    rows = [[0] * n, [Q - 1] * n]
-    for j, off in enumerate((half - 1, half, half + 1)):
-        rows.append([(ks[j * n + l] * (Q // q_last) >> 63) * q_last + off for l in range(n)])
-    return rows
 
 
 @pytest.mark.parametrize("name", CHAINS)
@@ -57,13 +42,35 @@ def test_coefficient_form_equals_integer_definition(port, name, n):
 def test_edge_inputs_equal_integer_definition(port, name):
     n = 16
     mods = _mods(port, name, n)
-    rows = _edge_values(mods, n, 5)
+    rows = rx.edge_values(mods, n, 5)
     x = rx.limbs_of(rows, mods)
     exp = rx.rescale_integer(x, n, mods, len(rows))
     assert (rx.rescale_exact(port, x, n, mods, len(rows), ntt_form=False) == exp).all()
+    assert (rx.rescale_per_limb(x, n, mods, len(rows)) == exp).all()
     # the edges themselves: X = 0 -> 0; X = Q - 1 -> floor((Q - 1 + h) / q_L) = Q / q_L, which is 0 mod every q_i
     e = exp.reshape(len(rows), len(mods), n)
     assert (e[0, :-1] == 0).all() and (e[1, :-1] == 0).all()
+    # q_L is odd: X mod q_L = h - 1 and h round down, h + 1 up; adding ceil(q_L / 2) instead of h would round h up
+    assert mods[-1] % 2 == 1
+    for row, up in zip(rows[2:], (0, 0, 1)):
+        assert all((v + (mods[-1] >> 1)) // mods[-1] == v // mods[-1] + up for v in row)
+
+
+PER_LIMB_LISTS = {
+    "tiny q_i": [2, 3, (1 << 61) - 1],
+    "tiny q_L": [(1 << 61) - 1, 2, 3],
+    "even q_L": [(1 << 61) - 1, 1000003, 1 << 40],
+    "composite": [3 * 5 * 7 * 11 * 13 * 17 * 19 * 23, 29 * 31 * 37 * 41 * 43 * 47, 53 * 59 * 61 * 67 * 71],
+}
+
+
+@pytest.mark.parametrize("name", sorted(PER_LIMB_LISTS))
+def test_per_limb_formula_equals_integer_definition(name):
+    """the GPU domain test's reference where the moduli share factors; here on pairwise coprime moduli"""
+    mods, n = PER_LIMB_LISTS[name], 16
+    x = np.concatenate([rx.limbs_of(rx.edge_values(mods, n, 3), mods), rx.random_operand(4, n, mods, 2)])
+    count = x.size // (len(mods) * n)
+    assert (rx.rescale_per_limb(x, n, mods, count) == rx.rescale_integer(x, n, mods, count)).all()
 
 
 def test_q_last_between_the_other_moduli(port):
