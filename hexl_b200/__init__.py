@@ -350,7 +350,8 @@ def EltwiseSubModMulti(result, operand1, operand2, n_per_modulus, moduli, stream
 
 
 def PolyMultiplyMulti(ntts, result, a, b, batch_per_modulus=None, stream=None):
-    """Negacyclic products InvNTT(FwdNTT(a) .* FwdNTT(b)), polynomial u under ntts[u // batch_per_modulus]"""
+    """Negacyclic products InvNTT(FwdNTT(a) .* FwdNTT(b)), polynomial u under ntts[u // batch_per_modulus]; result
+    may be a, b or a separate buffer, and a may be b (a square), with or without result."""
     rp, rn, rc = _buf(result); ap, an, ac = _buf(a); bp, bn, _ = _buf(b)
     n = ntts[0].GetDegree()
     if batch_per_modulus is None:

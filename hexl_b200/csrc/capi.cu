@@ -1462,11 +1462,11 @@ int hexl_b200_eltwise_sub_mod_multi(uint64_t* result, const uint64_t* operand1, 
   return rns_eltwise_entry(kRnsSub, result, operand1, operand2, n_per_modulus, moduli, num_moduli, 1, stream);
 }
 
-// FwdNTT(a), FwdNTT(b), point-wise product, InvNTT: all moduli per launch
+// FwdNTT(b) into scratch, FwdNTT(a) into result, point-wise product, InvNTT: all moduli per launch.  b is read before
+// result is first written, so result may be a, b or both (an in-place square)
 static int poly_multiply_on_device(int dev, hexl_b200_ntt* const* handles, uint64_t count, uint64_t* result,
                                    const uint64_t* a, const uint64_t* b, uint64_t group, cudaStream_t s) {
   const uint64_t n = handles[0]->n, total = count * group * n;
-  if (result == b) std::swap(a, b);  // the product commutes; keep the in-place transform on `result`
   Scratch ws(s);
   uint64_t* fb = nullptr;
   if (int rc = ws.get(&fb, total)) return rc;
@@ -1475,12 +1475,12 @@ static int poly_multiply_on_device(int dev, hexl_b200_ntt* const* handles, uint6
   if (product_fusion()) {
     // canonical transforms, then ONE inverse transform that multiplies on load: no MultMod kernel, and the product
     // never travels to HBM and back (dyadic-multiply-internal.cpp:17-73 folded into the transform that consumes it)
-    if (int rc = ntt_multi_on_device(true, dev, handles, count, result, a, 1, group, s)) return rc;
     if (int rc = ntt_multi_on_device(true, dev, handles, count, fb, b, 1, group, s)) return rc;
+    if (int rc = ntt_multi_on_device(true, dev, handles, count, result, a, 1, group, s)) return rc;
     return ntt_multi_on_device(false, dev, handles, count, result, result, 1, group, s, nullptr, false, fb);
   }
-  if (int rc = ntt_multi_on_device(true, dev, handles, count, result, a, 4, group, s)) return rc;
   if (int rc = ntt_multi_on_device(true, dev, handles, count, fb, b, 4, group, s)) return rc;
+  if (int rc = ntt_multi_on_device(true, dev, handles, count, result, a, 4, group, s)) return rc;
   if (int rc = rns_eltwise_on_device(kRnsMult, result, result, fb, group * n, moduli.data(), count, 4, s)) return rc;
   return ntt_multi_on_device(false, dev, handles, count, result, result, 1, group, s);
 }

@@ -370,7 +370,8 @@ class NTT {
 
   // result = InvNTT(FwdNTT(a) .* FwdNTT(b)) for count * batch_per_modulus polynomials (negacyclic
   // products, polynomial u under ntts[u / batch_per_modulus]): the FwdNTT -> EltwiseMultMod -> InvNTT
-  // pipeline as one call and a handful of launches.
+  // pipeline as one call and a handful of launches.  result may be a, b or a separate buffer, and a may be b
+  // (a square), with or without result.
   static void PolyMultiplyMulti(const NTT* const* ntts, size_t count, uint64_t* result, const uint64_t* a,
                                 const uint64_t* b, uint64_t batch_per_modulus = 1, void* stream = nullptr) {
     std::vector<hexl_b200_ntt*> hs(count);

@@ -155,7 +155,8 @@ int hexl_b200_ntt_inverse_multi(hexl_b200_ntt* const* handles, uint64_t count, u
  * polynomial u under handles[u / batch_per_modulus] (BASELINE configs[3]: FwdNTT ->
  * EltwiseMultMod -> InvNTT; the point-wise product is folded into the inverse transform,
  * which multiplies on load), 4 to 6 launches whatever `count`.  Inputs < q, outputs
- * in [0, q); result may be a, b or a separate buffer. */
+ * in [0, q); result may be a, b or a separate buffer, and a may be b (a square), with or
+ * without result. */
 int hexl_b200_eltwise_mult_mod_multi(uint64_t* result, const uint64_t* operand1, const uint64_t* operand2,
                                      uint64_t n_per_modulus, const uint64_t* moduli, uint64_t num_moduli,
                                      uint64_t input_mod_factor, void* stream);
