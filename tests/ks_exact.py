@@ -70,7 +70,7 @@ class Case(NamedTuple):
     keys: list
     modswitch: list
     digit_factor: int   # digits are drawn from [0, digit_factor * q_j)
-    wraps: bool         # the checkers' 128-bit accumulator wraps on this case
+    wraps: bool         # the checkers' 128-bit accumulator can wrap on this case (see can_wrap)
 
     @property
     def rns(self):
@@ -83,10 +83,25 @@ class Case(NamedTuple):
         return self.n, self.decomp, self.kms, self.rns, self.kcc, self.mods
 
 
+def can_wrap(mods, decomp):
+    """Whether decomp lazy products (4q - 1)(q - 1) can exceed a 128-bit sum for the largest modulus the switch uses
+    (the digits' and the special prime's; the unused key slots are never read)"""
+    q = max(mods[:decomp] + [mods[-1]])
+    return decomp * (4 * q - 1) * (q - 1) > (1 << 128) - 1
+
+
 def make_case(port, name, n=None):
     """The named configuration at degree n (default: the degree the GPU tests use).
 
     uniform       4 digits of 50-bit primes: the shape every older test has
+    kcc1, kcc3    3 digits of 50-bit primes with key_component_count 1 and 3
+    one_digit     1 digit (SEAL's level above the bottom) of a 50-bit prime, so rns_modulus_size = 2
+    slots         kcc3 with 3 unused key slots between the digits and the special prime
+                  (key_modulus_size = rns_modulus_size + 3)
+    small_special 3 digits of 50-bit primes and a 29-bit special prime, smaller than every digit: its inverse transform
+                  runs the 32-bit-word kernels, and the mod-down moves values into larger moduli
+    kcc3_wrap     17 digits just below 2^61 with key_component_count 3: one multiply-accumulate launch holds 16 digits
+                  there, so every modulus takes two launches
     seal_chain    a SEAL-style chain: first digit just below 2^61, larger than the special prime (just above 2^60),
                   then 40-bit digits, so the multi-modulus transforms run in WIDE mode; digits in [0, 2q); one unused
                   key slot between the digits and the special prime (key_modulus_size = rns_modulus_size + 1)
@@ -97,11 +112,28 @@ def make_case(port, name, n=None):
     wrap_blocks   70 digits (more than one 64-entry parameter block) of primes just below 2^61, random keys
     """
     primes = port.generate_primes
-    kcc, digit_factor, key_fill, wraps = 2, 1, None, False
+    kcc, digit_factor, key_fill = 2, 1, None
     if name == "uniform":
         n = n or 1 << 12
         mods = primes(5, 50, True, n)
         decomp = 4
+    elif name in ("kcc1", "kcc3", "slots"):
+        n = n or 1 << 12
+        decomp, kcc = 3, 1 if name == "kcc1" else 3
+        mods = primes(7 if name == "slots" else 4, 50, True, n)
+    elif name == "one_digit":
+        n = n or 1 << 12
+        decomp = 1
+        mods = primes(2, 50, True, n)
+    elif name == "small_special":
+        n = n or 1 << 12
+        decomp = 3
+        mods = primes(3, 50, True, n) + primes(1, 29, True, n)
+        assert mods[-1] < 1 << 30 and mods[-1] < min(mods[:decomp])
+    elif name == "kcc3_wrap":
+        n = n or 1 << 12
+        decomp, kcc = 17, 3
+        mods = primes(18, 60, False, n)
     elif name == "seal_chain":
         n = n or 1 << 12
         decomp = 4
@@ -118,14 +150,14 @@ def make_case(port, name, n=None):
         n = n or 1 << 12
         decomp = 29
         mods = primes(30, 60, False, n)
-        key_fill, wraps = "q-1", True
+        key_fill = "q-1"
     elif name == "wrap_blocks":
         n = n or 1 << 11
         decomp = 70
         mods = primes(71, 60, False, n)
-        wraps = True
     else:
         raise ValueError(name)
+    mods = [int(q) for q in mods]
     kms = len(mods)
     assert kms >= decomp + 1 and len(set(mods)) == kms
     seed = 1000 * sum(map(ord, name)) + n
@@ -137,7 +169,7 @@ def make_case(port, name, n=None):
 
     keys = [np.concatenate([key_word(j, k, i) for k in range(kcc) for i in range(kms)]) for j in range(decomp)]
     modswitch = [port.inverse_mod(mods[-1] % mods[i], mods[i]) for i in range(decomp)]
-    return Case(n, decomp, kms, kcc, mods, keys, modswitch, digit_factor, wraps)
+    return Case(n, decomp, kms, kcc, mods, keys, modswitch, digit_factor, can_wrap(mods, decomp))
 
 
 def ciphertext(case, seed):

@@ -311,20 +311,33 @@ def _rotation_exact(port, case, ct, g, batch):
     return np.concatenate(out)
 
 
-def _ks_prepared(port, name, g):
-    if (name, g) not in _ks_cache:
-        case = ks_exact.make_case(port, name)
+def _ks_prepared(port, name, g, n=None):
+    if (name, g, n) not in _ks_cache:
+        case = ks_exact.make_case(port, name, n)
         gg = 2 * case.n - 1 if g == "2n-1" else g
         ct = _ciphertexts(case, 3, 11)
-        _ks_cache[name, g] = case, gg, ct, _rotation_exact(port, case, ct, gg, 3)
-    return _ks_cache[name, g]
+        _ks_cache[name, g, n] = case, gg, ct, _rotation_exact(port, case, ct, gg, 3)
+    return _ks_cache[name, g, n]
 
 
 @pytest.mark.parametrize("entry", ["device", "host", "host_split"])
 @pytest.mark.parametrize("g", [3, "2n-1"])
 @pytest.mark.parametrize("name", KS_CASES)
 def test_apply_galois_key_switch_equals_exact_rotation(hb, port, name, g, entry):
-    case, g, ct, exp = _ks_prepared(port, name, g)
+    _check_rotations(hb, name, *_ks_prepared(port, name, g), entry)
+
+
+@pytest.mark.parametrize("entry", ["device", "host"])
+@pytest.mark.parametrize("g", [3, "2n-1"])
+@pytest.mark.parametrize("logn", [1, 2, 3, 6, 10])
+def test_apply_galois_key_switch_at_small_degrees(hb, port, logn, g, entry):
+    """uniform at N = 2 (where 3 = 2n - 1), 4 and 8, where the automorphism moves one or two 16-byte pairs per
+    polynomial and the transforms of the switch run one thread per polynomial, and at 64 and 2^10 (row kernels)"""
+    _check_rotations(hb, f"uniform n={1 << logn}", *_ks_prepared(port, "uniform", g, 1 << logn), entry)
+
+
+def _check_rotations(hb, name, case, g, ct, exp, entry):
+    """batch 1 and 3 through one entry point, against the exact rotation"""
     per = 2 * case.decomp * case.n
     for batch in (1, 3):
         if entry == "device":

@@ -1,7 +1,8 @@
 """DivideAndRoundQLast on the GPU across the domain it accepts, against the integer definition.
 
     chains       wide (primes just below 2^61, the limit), small (q_L < 2^30: its inverse runs the 32-bit kernels),
-                 classes and seal, at n = 2^4, 2^12 and 2^17, in both forms, on device and host pointers
+                 classes and seal, at n = 2, 4, 8, 16, 32, 2^8, 2^11, 2^12 and 2^17, in both forms, on device and
+                 host pointers
     inputs       the rounding edges of rescale_exact.edge_values (X = 0, X = Q - 1, X mod q_L in {h - 1, h, h + 1}),
                  limbs at q_i - 1 with X mod q_L = h + 1, and a uniform polynomial
     coef. form   n = 1, 3 and 4099; q_i in {2, 3}; an even q_L; composite moduli; moduli that share factors with each
@@ -24,7 +25,9 @@ torch = pytest.importorskip("torch")
 U64 = np.uint64
 SENTINEL = 0xA5A5A5A5A5A5A5A5
 CHAINS = ("wide", "small", "classes", "seal")
-LOGNS = (4, 12, 17)
+# 2, 4 and 8: the NTT form's transforms run one thread per polynomial; 16 to 2^11: one row kernel with several
+# polynomials per CTA; 2^12 and up: row and column passes
+LOGNS = (1, 2, 3, 4, 5, 8, 11, 12, 17)
 INTEGER_MAX_N = 1 << 12   # above this, rescale_exact stands in for the Python-integer definition
 
 
