@@ -125,6 +125,8 @@ _sig("hexl_b200_keys_upload_sharded", _int, [C.POINTER(_vp), _vp, _u64, _u64, _u
 _sig("hexl_b200_keys_release", None, [_vp])
 _sig("hexl_b200_key_switch_resident", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp])
 _sig("hexl_b200_apply_galois_key_switch", _int, [_vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _u64, _vp])
+_sig("hexl_b200_apply_galois_key_switch_hoisted", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -582,3 +584,26 @@ def ApplyGaloisKeySwitch(ciphertexts, n, decomp_modulus_size, key_modulus_size, 
                                                   galois_keys._h if galois_keys is not None else None, ms.ctypes.data,
                                                   galois_elt, batch, _stream(stream, cc)))
     return ciphertexts
+
+
+def ApplyGaloisKeySwitchHoisted(results, ciphertexts, n, decomp_modulus_size, key_modulus_size, rns_modulus_size,
+                                key_component_count, moduli, galois_keys, modswitch_factors, galois_elts, batch=1,
+                                stream=None):
+    """Hoisted rotations (hexl_b200_apply_galois_key_switch_hoisted): ciphertext c of `ciphertexts` (2*decomp*n words
+    each) rotated by every galois_elts[r] with galois_keys[r] (a list of KeySwitchKeys), into
+    results[(c * len(galois_elts) + r) * 2*decomp*n:], its digits decomposed once for all elements.  Not bit-identical
+    to ApplyGaloisKeySwitch: digits are lifted to signed integers under sigma_g (equal for g = 1)."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    ms = np.ascontiguousarray(modswitch_factors, dtype=np.uint64)
+    elts = np.ascontiguousarray(galois_elts, dtype=np.uint64)
+    rp, rn, rc = _buf(results); cp, cn, cc = _buf(ciphertexts)
+    per = key_component_count * decomp_modulus_size * n
+    _need("moduli", mods.size, key_modulus_size); _need("modswitch_factors", ms.size, decomp_modulus_size)
+    _need("galois_keys", len(galois_keys), elts.size)
+    _need("results", rn, batch * elts.size * per); _need("ciphertexts", cn, batch * per)
+    keys = (_vp * max(1, len(galois_keys)))(*[k._h if k is not None else None for k in galois_keys])
+    _check(_lib.hexl_b200_apply_galois_key_switch_hoisted(rp, cp, n, decomp_modulus_size, key_modulus_size,
+                                                          rns_modulus_size, key_component_count, mods.ctypes.data,
+                                                          keys, elts.ctypes.data, elts.size, ms.ctypes.data, batch,
+                                                          _stream(stream, rc or cc)))
+    return results

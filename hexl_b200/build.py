@@ -23,7 +23,7 @@ LIB_DIR = os.path.join(PKG, "lib")
 LIB = os.path.join(LIB_DIR, "libhexl_b200.so")
 
 SOURCES = ["capi.cu", "ntt.cu", "ntt_multi.cu", "eltwise.cu", "seal.cu", "galois.cu", "numtheory.cpp"]
-HEADERS = ["internal.h", "modarith.cuh", "ntt_kernels.cuh", "numtheory.h", os.path.join(ROOT, "include", "hexl_b200.h")]
+HEADERS = ["internal.h", "modarith.cuh", "ntt_kernels.cuh", "galois.cuh", "numtheory.h", os.path.join(ROOT, "include", "hexl_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

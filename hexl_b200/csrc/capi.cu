@@ -797,9 +797,15 @@ int mod_down_on_device(int dev, uint64_t* result, uint64_t res_stride, const uin
 // step batched over the RNS moduli (multi-modulus NTTs + the glue kernels of seal.cu): about a
 // dozen launches whatever the number of moduli, instead of ~10 per modulus.  Every pointer is
 // a device pointer on the current device.  Scratch layouts are [modulus][digit or component][n].
-int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, uint64_t n, uint64_t decomp,
-                         uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
-                         const uint64_t* const* d_key_ptrs_host, const uint64_t* modswitch, cudaStream_t s) {
+// `elts` switches share the digits t_target, decomposed once (steps 1 and 2's transforms): switch r multiplies them
+// with the keys d_key_ptrs[r] and accumulates into results[r].  galois_elts (the hoisted rotations; nullptr: none)
+// makes switch r read the transformed digits permuted by pi_{galois_elts[r]}.  Scratch: one round of transformed
+// digits plus elts x rns x kcc x n words of products.
+static int key_switch_elts_on_device(int dev, uint64_t* const* results, const uint64_t* t_target, uint64_t n,
+                                     uint64_t decomp, uint64_t key_modulus_size, uint64_t rns, uint64_t kcc,
+                                     const uint64_t* moduli, const uint64_t* const* const* d_key_ptrs,
+                                     const uint64_t* galois_elts, uint64_t elts, const uint64_t* modswitch,
+                                     cudaStream_t s) {
   std::vector<hexl_b200_ntt*> h(key_modulus_size, nullptr);
   struct Release {
     std::vector<hexl_b200_ntt*>& v;
@@ -825,7 +831,7 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
   uint64_t *t_coef = nullptr, *ops = nullptr, *prod = nullptr, *tmp = nullptr;
   if (int rc = ws.get(&t_coef, per_mod)) return rc;
   if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;
-  if (int rc = ws.get(&prod, rns * kcc * n)) return rc;                                       // [i][k][n]
+  if (int rc = ws.get(&prod, elts * rns * kcc * n)) return rc;                                // [r][i][k][n]
   if (int rc = ws.get(&tmp, std::min<uint64_t>(decomp, kParamBlock) * kcc * n)) return rc;  // [i][k][n], one block
 #define LAUNCH(expr)                                                    \
   do {                                                                  \
@@ -851,20 +857,33 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
     // t_coef (L2-resident) and reduces on load, instead of a reduce kernel writing decomp x cnt x n words for it
     if (int rc = ntt_multi_on_device(true, dev, hs.data(), cnt, ops, t_coef, 4, decomp, s, nullptr, true)) return rc;
     const uint64_t jmax = ks_mac_digits_per_launch(mods, cnt);
-    for (uint64_t j0 = 0; j0 < decomp; j0 += jmax) {  // key pointers ride in the kernel parameters
-      const uint64_t jc = std::min<uint64_t>(jmax, decomp - j0);
-      KeyPointers kp;
-      for (uint64_t j = 0; j < jc; ++j) kp.p[j] = d_key_ptrs_host[j0 + j];
-      LAUNCH(launch_ks_mac(prod + i0 * kcc * n, ops + j0 * n, per_mod, kp, n, jc, kcc, key_modulus_size, cnt, mods,
-                           j0 != 0, s));
+    for (uint64_t r = 0; r < elts; ++r) {
+      uint64_t* prod_r = prod + r * rns * kcc * n;
+      for (uint64_t j0 = 0; j0 < decomp; j0 += jmax) {  // key pointers ride in the kernel parameters
+        const uint64_t jc = std::min<uint64_t>(jmax, decomp - j0);
+        KeyPointers kp;
+        for (uint64_t j = 0; j < jc; ++j) kp.p[j] = d_key_ptrs[r][j0 + j];
+        LAUNCH(launch_ks_mac(prod_r + i0 * kcc * n, ops + j0 * n, per_mod, kp, n, jc, kcc, key_modulus_size, cnt,
+                             mods, j0 != 0, s, galois_elts ? galois_elts[r] : 0));
+      }
     }
   }
 #undef LAUNCH
   // 3. mod-down by the special prime and accumulate into result (:134-198); prod's last part is [k][n], contiguous
-  if (int rc = mod_down_on_device(dev, result, decomp, prod, false, true, prod + decomp * kcc * n, tmp, n, kcc,
-                                  h[key_modulus_size - 1], h.data(), moduli, modswitch, decomp, s))
-    return rc;
+  for (uint64_t r = 0; r < elts; ++r) {
+    uint64_t* prod_r = prod + r * rns * kcc * n;
+    if (int rc = mod_down_on_device(dev, results[r], decomp, prod_r, false, true, prod_r + decomp * kcc * n, tmp, n,
+                                    kcc, h[key_modulus_size - 1], h.data(), moduli, modswitch, decomp, s))
+      return rc;
+  }
   return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
+}
+
+int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, uint64_t n, uint64_t decomp,
+                         uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
+                         const uint64_t* const* d_key_ptrs_host, const uint64_t* modswitch, cudaStream_t s) {
+  return key_switch_elts_on_device(dev, &result, t_target, n, decomp, key_modulus_size, rns, kcc, moduli,
+                                   &d_key_ptrs_host, nullptr, 1, modswitch, s);
 }
 
 
@@ -1584,28 +1603,56 @@ static int galois_key_switch_on_device(int dev, uint64_t* ct, uint64_t* perm, ui
                               modswitch, s);
 }
 
+// The hoisted rotations of one ciphertext ct (device memory, as above) by num_elts elements: out + r * 2 * decomp * n
+// gets [sigma_g(c0), 0] + ModDown(sum_j pi_g(D_j) K_r[j]) for g = galois_elts[r], with the digits D_j of c1 decomposed
+// and transformed once for every element.  Per element: one automorphism launch over c0 straight into the output, a
+// memset of the output's c1, then its multiply-accumulates and mod-down inside the shared key switch.
+static int hoisted_rotations_on_device(int dev, uint64_t* out, const uint64_t* ct, uint64_t n, uint64_t decomp,
+                                       uint64_t key_modulus_size, uint64_t rns, const uint64_t* moduli,
+                                       const uint64_t* const* const* d_key_ptrs, const uint64_t* galois_elts,
+                                       uint64_t num_elts, const uint64_t* modswitch, cudaStream_t s) {
+  const uint64_t comp = decomp * n;
+  std::vector<uint64_t*> results(num_elts);
+  for (uint64_t r = 0; r < num_elts; ++r) {
+    results[r] = out + r * 2 * comp;
+    const cudaError_t e = launch_galois_ntt(results[r], ct, floor_log2(n), decomp, galois_elts[r], s);
+    if (e != cudaSuccess) return cuda_fail(e, "ApplyGaloisKeySwitchHoisted: automorphism launch");
+    CU(cudaMemsetAsync(results[r] + comp, 0, comp * sizeof(uint64_t), s));
+  }
+  return key_switch_elts_on_device(dev, results.data(), ct + comp, n, decomp, key_modulus_size, rns, 2, moduli,
+                                   d_key_ptrs, galois_elts, num_elts, modswitch, s);
+}
+
 // One or more key switches on HOST buffers against keys already on the devices: ciphertext c occupies
 // result[c * kcc*decomp*n ...] and t_target[c * decomp*n ...].  Each ciphertext runs on one of the rotating
 // staging streams (digits in, result in, ~12 kernels, result out), so the copies of one ciphertext overlap the
 // kernels of its neighbours; with host devices set the batch is split across the GPUs holding the keys.
 // galois_elt != 0: the rotation of ApplyGaloisKeySwitch instead (kcc = 2, t_target unused): only the ciphertext
 // crosses PCIe, and the slot's second buffer holds both permuted components.
+// hoisted_elts != nullptr: the num_elts hoisted rotations of ApplyGaloisKeySwitchHoisted instead (kcc = 2, keys[r] for
+// hoisted_elts[r]): t_target holds the input ciphertexts (2 x decomp x n words each); each crosses PCIe in once and
+// its num_elts rotations come back from the same slot.  The batch is split over the devices holding every key.
 static int key_switch_host_batch(uint64_t* result, const uint64_t* t_target, uint64_t n, uint64_t decomp,
                                  uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
-                                 const hexl_b200_keys* keys, const uint64_t* modswitch, uint64_t batch,
-                                 uint64_t galois_elt = 0) {
+                                 const hexl_b200_keys* const* keys, const uint64_t* modswitch, uint64_t batch,
+                                 uint64_t galois_elt = 0, const uint64_t* hoisted_elts = nullptr,
+                                 uint64_t num_elts = 1) {
   std::vector<int> devs = host_devices();
   if (devs.empty()) {
     int cur = 0;
     CU(cudaGetDevice(&cur));
     devs.push_back(cur);
   }
+  const bool hoisted = hoisted_elts != nullptr;
   std::vector<int> use;
-  for (int d : devs)
-    if (keys->dev.count(d)) use.push_back(d);
+  for (int d : devs) {
+    bool all = true;
+    for (uint64_t r = 0; r < num_elts; ++r) all = all && keys[r]->dev.count(d);
+    if (all) use.push_back(d);
+  }
   if (use.empty()) return fail(HEXL_B200_ERR_INVALID_ARG, "the key handle holds no copy on the device(s) used for host calls");
   if (use.size() > batch) use.resize(batch);
-  const u64 res_elems = kcc * decomp * n, t_elems = decomp * n;
+  const u64 res_elems = (hoisted ? num_elts : 1) * kcc * decomp * n, t_elems = (hoisted ? 2 : 1) * decomp * n;
   int rc = 0;
   for (size_t di = 0; di < use.size() && !rc; ++di) {
     const int dev = use[di];
@@ -1615,7 +1662,8 @@ static int key_switch_host_batch(uint64_t* result, const uint64_t* t_target, uin
     StageCtx* st = stage_for(dev);
     std::lock_guard<std::mutex> lk(st->mu);
     if ((rc = st->init())) break;
-    const std::vector<uint64_t*>& dk = keys->dev.at(dev);
+    std::vector<const uint64_t* const*> dk(num_elts);
+    for (uint64_t r = 0; r < num_elts; ++r) dk[r] = keys[r]->dev.at(dev).data();
     int slot = 0;
     for (u64 c = c_lo; c < c_hi && !rc; ++c, slot = (slot + 1) % kSlots) {
       if ((rc = st->reserve(slot, 0, res_elems * 8))) break;
@@ -1624,17 +1672,20 @@ static int key_switch_host_batch(uint64_t* result, const uint64_t* t_target, uin
       u64 *d_res = st->buf[slot][0], *d_t = st->buf[slot][1];
       cudaError_t e = cudaSuccess;
       if (!galois_elt) e = cudaMemcpyAsync(d_t, t_target + c * t_elems, t_elems * 8, cudaMemcpyHostToDevice, sx);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_res, result + c * res_elems, res_elems * 8, cudaMemcpyHostToDevice, sx);
+      if (e == cudaSuccess && !hoisted)
+        e = cudaMemcpyAsync(d_res, result + c * res_elems, res_elems * 8, cudaMemcpyHostToDevice, sx);
       if (e != cudaSuccess) {
         rc = cuda_fail(e, "KeySwitch H2D");
         break;
       }
-      if (galois_elt)
-        rc = galois_key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, moduli, dk.data(),
-                                         modswitch, galois_elt, sx);
+      if (hoisted)
+        rc = hoisted_rotations_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, moduli, dk.data(),
+                                         hoisted_elts, num_elts, modswitch, sx);
+      else if (galois_elt)
+        rc = galois_key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, moduli, dk[0], modswitch,
+                                         galois_elt, sx);
       else
-        rc = key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, kcc, moduli, dk.data(), modswitch,
-                                  sx);
+        rc = key_switch_on_device(dev, d_res, d_t, n, decomp, key_modulus_size, rns, kcc, moduli, dk[0], modswitch, sx);
       if (rc) break;
       e = cudaMemcpyAsync(result + c * res_elems, d_res, res_elems * 8, cudaMemcpyDeviceToHost, sx);
       if (e != cudaSuccess) rc = cuda_fail(e, "KeySwitch D2H");
@@ -1975,7 +2026,7 @@ int hexl_b200_key_switch_resident(uint64_t* result, const uint64_t* t_target_ite
     return 0;
   }
   if (pi.where == Where::Host)
-    return key_switch_host_batch(result, t_target_iter_ptr, n, decomp, key_modulus_size, rns, kcc, moduli, keys,
+    return key_switch_host_batch(result, t_target_iter_ptr, n, decomp, key_modulus_size, rns, kcc, moduli, &keys,
                                  modswitch_factors, batch);
   auto it = keys->dev.find(pi.device);
   if (it == keys->dev.end()) return fail(HEXL_B200_ERR_MIXED_POINTERS, "the key handle holds no copy on the device of result");
@@ -2017,7 +2068,7 @@ int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, ui
   // (hexl_b200_keys_upload) and calls hexl_b200_key_switch_resident.
   hexl_b200_keys* tmp = nullptr;
   if (int rc = hexl_b200_keys_upload(&tmp, k_switch_keys, n, decomp, key_modulus_size, kcc)) return rc;
-  const int rc = key_switch_host_batch(result, t_target_iter_ptr, n, decomp, key_modulus_size, rns, kcc, moduli, tmp,
+  const int rc = key_switch_host_batch(result, t_target_iter_ptr, n, decomp, key_modulus_size, rns, kcc, moduli, &tmp,
                                        modswitch_factors, 1);
   hexl_b200_keys_release(tmp);
   return rc;
@@ -2256,7 +2307,7 @@ int hexl_b200_apply_galois_key_switch(uint64_t* ciphertexts, uint64_t n, uint64_
       for (uint64_t i = 0; i < decomp; ++i)
         if (int rc = check_bounds(ciphertexts + c * comp + i * n, n, moduli[i], pi, "ciphertexts")) return rc;
   if (pi.where == Where::Host)
-    return key_switch_host_batch(ciphertexts, nullptr, n, decomp, key_modulus_size, rns, kcc, moduli, galois_keys,
+    return key_switch_host_batch(ciphertexts, nullptr, n, decomp, key_modulus_size, rns, kcc, moduli, &galois_keys,
                                  modswitch_factors, batch, galois_elt);
   auto it = galois_keys->dev.find(pi.device);
   if (it == galois_keys->dev.end())
@@ -2270,6 +2321,59 @@ int hexl_b200_apply_galois_key_switch(uint64_t* ciphertexts, uint64_t n, uint64_
     if (int rc = galois_key_switch_on_device(pi.device, ciphertexts + c * 2 * comp, perm, n, decomp, key_modulus_size,
                                              rns, moduli, it->second.data(), modswitch_factors, galois_elt,
                                              (cudaStream_t)stream))
+      return rc;
+  return finish_device_call(pi, stream);
+}
+
+int hexl_b200_apply_galois_key_switch_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                              uint64_t decomp_modulus_size, uint64_t key_modulus_size,
+                                              uint64_t rns_modulus_size, uint64_t key_component_count,
+                                              const uint64_t* moduli, const hexl_b200_keys* const* galois_keys,
+                                              const uint64_t* galois_elts, uint64_t num_elts,
+                                              const uint64_t* modswitch_factors, uint64_t batch, void* stream) {
+  const uint64_t decomp = decomp_modulus_size, rns = rns_modulus_size, kcc = key_component_count;
+  if (int rc = key_switch_check(results, ciphertexts, n, decomp, key_modulus_size, rns, kcc, moduli,
+                                modswitch_factors))
+    return rc;
+  REQUIRE(kcc == 2, "Require key_component_count == 2 (a ciphertext of two components)");
+  REQUIRE(n <= (1ull << 20), "Require n <= 2^20");
+  REQUIRE(num_elts == 0 || (galois_keys && galois_elts), "Require galois_keys, galois_elts != nullptr");
+  for (uint64_t r = 0; r < num_elts; ++r) {
+    if (int rc = galois_elt_check(n, galois_elts[r])) return rc;
+    const hexl_b200_keys* k = galois_keys[r];
+    REQUIRE(k != nullptr, "Require galois_keys[%llu] != nullptr", (unsigned long long)r);
+    REQUIRE(k->n == n && k->decomp >= decomp && k->kcc == kcc && k->kms == key_modulus_size,
+            "galois_keys[%llu] was uploaded for another shape", (unsigned long long)r);
+    REQUIRE(k->shards.empty(),
+            "ApplyGaloisKeySwitchHoisted does not take keys sharded by modulus: upload them with hexl_b200_keys_upload");
+  }
+  if (num_elts == 0 || batch == 0) return 0;
+  const uint64_t comp = decomp * n, in_total = batch * 2 * comp, out_total = batch * num_elts * 2 * comp;
+  REQUIRE(results + out_total <= ciphertexts || ciphertexts + in_total <= results,
+          "results and ciphertexts must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({results, ciphertexts}, &pi)) return rc;
+  if (g_debug.load())
+    for (uint64_t c = 0; c < 2 * batch; ++c)
+      for (uint64_t i = 0; i < decomp; ++i)
+        if (int rc = check_bounds(ciphertexts + c * comp + i * n, n, moduli[i], pi, "ciphertexts")) return rc;
+  if (pi.where == Where::Host)
+    return key_switch_host_batch(results, ciphertexts, n, decomp, key_modulus_size, rns, kcc, moduli, galois_keys,
+                                 modswitch_factors, batch, 0, galois_elts, num_elts);
+  std::vector<const uint64_t* const*> dk(num_elts);
+  for (uint64_t r = 0; r < num_elts; ++r) {
+    auto it = galois_keys[r]->dev.find(pi.device);
+    if (it == galois_keys[r]->dev.end())
+      return fail(HEXL_B200_ERR_MIXED_POINTERS, "galois_keys[%llu] holds no copy on the device of the ciphertexts",
+                  (unsigned long long)r);
+    dk[r] = it->second.data();
+  }
+  DeviceGuard g;
+  if (int rc = g.enter(pi.device)) return rc;
+  for (uint64_t c = 0; c < batch; ++c)
+    if (int rc = hoisted_rotations_on_device(pi.device, results + c * num_elts * 2 * comp, ciphertexts + c * 2 * comp,
+                                             n, decomp, key_modulus_size, rns, moduli, dk.data(), galois_elts,
+                                             num_elts, modswitch_factors, (cudaStream_t)stream))
       return rc;
   return finish_device_call(pi, stream);
 }

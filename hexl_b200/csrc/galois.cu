@@ -10,6 +10,7 @@
 //
 // V16: every buffer of the launch is 16-byte aligned, so a thread moves its output pair (2m, 2m+1) with one 16-byte
 // store (and, in NTT form, one 16-byte load); otherwise the same pairs move a word at a time.
+#include "galois.cuh"
 #include "internal.h"
 
 namespace hexl_b200 {
@@ -17,14 +18,6 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kSmemThreads = 1024;
-
-__device__ __forceinline__ unsigned rev_bits(unsigned x, int log_n) { return __brev(x) >> (32 - log_n); }
-
-// pi_g(j) for the NTT-form slot j
-__device__ __forceinline__ unsigned ntt_source(unsigned j, unsigned g, unsigned two_n_mask, int log_n) {
-  const unsigned k = (g * (2u * rev_bits(j, log_n) + 1u)) & two_n_mask;  // odd
-  return rev_bits(k >> 1, log_n);
-}
 
 template <bool V16>
 __device__ __forceinline__ void st_pair(u64* p, u64 a, u64 b) {

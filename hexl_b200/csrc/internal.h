@@ -135,10 +135,11 @@ struct KsModulus {
 struct KsModuli {
   KsModulus m[kParamBlock];
 };
-// prod[e][k][l] (+)= sum_{j < jcount} ops[e][j][l] * keys[j][k][c_e][l]  mod q_e ; ops_stride = elements between e's
+// prod[e][k][l] (+)= sum_{j < jcount} ops[e][j][l] * keys[j][k][c_e][l]  mod q_e ; ops_stride = elements between e's.
+// galois_elt = g != 0: ops[e][j][pi_g(l)] instead, pi_g the NTT-form automorphism of launch_galois_ntt.
 cudaError_t launch_ks_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPointers& keys, u64 n, u64 jcount,
                           u64 kcc, u64 key_modulus_size, u64 count, const KsModuli& mods, int accumulate,
-                          cudaStream_t stream);
+                          cudaStream_t stream, u64 galois_elt = 0);
 // tmp[e][k][l] = ((t_last[k][l] + q_last/2) mod q_last) mod q_e + a_e
 cudaError_t launch_ks_round(u64* tmp, const u64* t_last, u64 n, u64 kcc, u64 q_last, u64 mu_last, u64 count,
                             const KsModuli& mods, cudaStream_t stream);

@@ -6,6 +6,7 @@
 //   DyadicMultiply   hexl/experimental/seal/dyadic-multiply-internal.cpp:17-73
 //   KeySwitch        hexl/experimental/seal/key-switch-internal.cpp:25-201
 //   rescale          SEAL's RNSTool::divide_and_round_q_last(_ntt)_inplace
+#include "galois.cuh"
 #include "internal.h"
 
 namespace hexl_b200 {
@@ -130,10 +131,14 @@ __global__ void __launch_bounds__(kThreads)
 
 // :93-130: lazy 128-bit multiply-accumulate of the digits with the switching keys, one
 // Shoup(hi, 2^64 mod q) + Barrett(lo) at the end, two conditional subtractions.
+// PERMUTE (the hoisted rotations): output slot l reads digit slot pi_g(l), the NTT-form automorphism applied to the
+// transformed digits on load.  An aligned block of 2^t output slots reads one aligned block of 2^t digit slots, so the
+// reads stay as coalesced as the plain ones.
+template <bool PERMUTE>
 __global__ void __launch_bounds__(kThreads)
     ks_mac_kernel(u64* prod, const u64* ops, u64 ops_stride, const __grid_constant__ KeyPointers keys, u64 n,
                   u64 jcount, u64 kcc, u64 key_modulus_size, u64 count, const __grid_constant__ KsModuli mods,
-                  int accumulate) {
+                  int accumulate, unsigned galois_elt) {
   const u64 per_mod = kcc * n;
   const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
   if (g >= per_mod * count) return;
@@ -141,7 +146,9 @@ __global__ void __launch_bounds__(kThreads)
   const u64 k = r / n, l = r - k * n;
   const KsModulus& md = mods.m[e];
   const u64 key_off = n * md.c + k * key_modulus_size * n + l;
-  const u64* op = ops + e * ops_stride + l;
+  u64 src = l;
+  if constexpr (PERMUTE) src = ntt_source((unsigned)l, galois_elt, (unsigned)(2 * n - 1), __ffsll((long long)n) - 1);
+  const u64* op = ops + e * ops_stride + src;
   u64 lo = 0, hi = 0;
   for (u64 j = 0; j < jcount; ++j) {
     const u64 a = op[j * n];
@@ -267,9 +274,11 @@ cudaError_t launch_rns_eltwise(int op, u64* result, const u64* a, const u64* b, 
 
 cudaError_t launch_ks_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPointers& keys, u64 n, u64 jcount,
                           u64 kcc, u64 key_modulus_size, u64 count, const KsModuli& mods, int accumulate,
-                          cudaStream_t stream) {
-  ks_mac_kernel<<<blocks_for(kcc * n * count), kThreads, 0, stream>>>(prod, ops, ops_stride, keys, n, jcount, kcc,
-                                                                     key_modulus_size, count, mods, accumulate);
+                          cudaStream_t stream, u64 galois_elt) {
+  auto kernel = galois_elt ? ks_mac_kernel<true> : ks_mac_kernel<false>;
+  kernel<<<blocks_for(kcc * n * count), kThreads, 0, stream>>>(prod, ops, ops_stride, keys, n, jcount, kcc,
+                                                              key_modulus_size, count, mods, accumulate,
+                                                              (unsigned)galois_elt);
   count_launch();
   return cudaGetLastError();
 }

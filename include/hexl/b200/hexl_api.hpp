@@ -657,5 +657,26 @@ inline void ApplyGaloisKeySwitch(uint64_t* ciphertexts, uint64_t n, uint64_t dec
                                                        stream));
 }
 
+namespace b200 {
+// extension: hoisted rotations -- each of `batch` ciphertexts rotated by every galois_elts[r] with *galois_keys[r],
+// its digits decomposed once for all elements; rotation r of ciphertext c goes to
+// results + (c * num_elts + r) * 2 * decomp_modulus_size * n (hexl_b200_apply_galois_key_switch_hoisted has the
+// formula).  Not bit-identical to ApplyGaloisKeySwitch: the digits are lifted to signed integers under sigma_g (equal
+// for g = 1; the same noise bound).  key_component_count must be 2; sharded key handles are refused.
+inline void ApplyGaloisKeySwitchHoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                        uint64_t decomp_modulus_size, uint64_t key_modulus_size,
+                                        uint64_t rns_modulus_size, uint64_t key_component_count,
+                                        const uint64_t* moduli, const KeySwitchKeys* const* galois_keys,
+                                        const uint64_t* galois_elts, uint64_t num_elts,
+                                        const uint64_t* modswitch_factors, uint64_t batch = 1,
+                                        void* stream = nullptr) {
+  std::vector<const hexl_b200_keys*> handles(num_elts);
+  for (uint64_t r = 0; r < num_elts; ++r) handles[r] = galois_keys[r] ? galois_keys[r]->Handle() : nullptr;
+  b200_detail::Throw(hexl_b200_apply_galois_key_switch_hoisted(
+      results, ciphertexts, n, decomp_modulus_size, key_modulus_size, rns_modulus_size, key_component_count, moduli,
+      handles.data(), galois_elts, num_elts, modswitch_factors, batch, stream));
+}
+}  // namespace b200
+
 }  // namespace hexl
 }  // namespace intel

@@ -332,6 +332,37 @@ int hexl_b200_apply_galois_key_switch(uint64_t* ciphertexts, uint64_t n, uint64_
                                       const hexl_b200_keys* galois_keys, const uint64_t* modswitch_factors,
                                       uint64_t galois_elt, uint64_t batch, void* stream);
 
+/* Hoisted rotations (extension; OpenFHE's EvalFastRotationPrecompute + EvalFastRotation): each of `batch` ciphertexts
+ * rotated by each of num_elts Galois elements in one call, its digits decomposed and transformed ONCE for every
+ * element.  Input ciphertext c is at ciphertexts + c * 2 * decomp * n, laid out as for
+ * hexl_b200_apply_galois_key_switch; its rotation by galois_elts[r] with galois_keys[r] is written to
+ * results + (c * num_elts + r) * 2 * decomp * n.  Out of place: ciphertexts is not modified.  For c = (c0, c1):
+ *   a_j        = INTT_{q_j}(c1_j)                          digit j < decomp, in [0, q_j)
+ *   D_{j,i}    = NTT_{q_i}(a_j mod q_i)                    every modulus i of the switch
+ *   prod_{i,k} = sum_j pi_g(D_{j,i}) (.) K[j][k][i]  mod q_i
+ *   out        = [sigma_g(c0), 0] + ModDown(prod)           (the mod-down of hexl_b200_key_switch)
+ * with pi_g / sigma_g the NTT-form automorphism of hexl_b200_apply_galois.  This is the key switch of sigma_g(c1)
+ * with digit j's coefficients lifted to the signed integers sigma_g(a_j) (entries +-a_j[t], below q_j in magnitude)
+ * instead of to [0, q_j), so it is NOT bit-identical to hexl_b200_apply_galois_key_switch: the two differ where
+ * sigma_g negates a nonzero coefficient, by q_j mod q_i in digit j's extended limbs; for g = 1 they are equal bit for
+ * bit.  The decryption noise bound is the same.  HEXL_B200_ERR_INVALID_ARG on the shape rules of
+ * hexl_b200_apply_galois_key_switch applied to every key handle (null, another shape, or sharded by modulus), for any
+ * element outside the rules of hexl_b200_apply_galois, and when results overlaps ciphertexts.  Elements may repeat.
+ * num_elts = 0 or batch = 0 does nothing.  Inputs are checked below their modulus under hexl_b200_set_debug(1).
+ * On the device, per ciphertext: one inverse transform of the digits and one gathered forward transform per round of
+ * moduli, shared by every element; per element, its multiply-accumulates, one automorphism launch of c0 straight into
+ * the output, a memset of the output's c1 and its mod-down.  For one element these are the launches of
+ * hexl_b200_apply_galois_key_switch.  Library scratch is one round of transformed digits, as for the key switch, plus
+ * num_elts x rns x 2 x n words of products: about the size of one ciphertext's results.  Host buffers: each ciphertext
+ * crosses PCIe in once and its num_elts rotations come back on the same staging stream, pipelined and split by
+ * ciphertext over the devices of hexl_b200_set_host_devices where every key handle holds a copy. */
+int hexl_b200_apply_galois_key_switch_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                              uint64_t decomp_modulus_size, uint64_t key_modulus_size,
+                                              uint64_t rns_modulus_size, uint64_t key_component_count,
+                                              const uint64_t* moduli, const hexl_b200_keys* const* galois_keys,
+                                              const uint64_t* galois_elts, uint64_t num_elts,
+                                              const uint64_t* modswitch_factors, uint64_t batch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
