@@ -6,11 +6,15 @@ Layout everywhere: `count` polynomials back to back, each of rns limbs of n word
     NTT form          result[j] = operand[pi_g(j)], pi_g(j) = rev(((g (2 rev(j) + 1)) mod 2n - 1) / 2)
 The NTT form is the forward-transform order of ntt_exact.forward (slot j holds a(psi^(2 rev(j) + 1))), so
 forward(sigma_coef(a)) == sigma_ntt(forward(a)); tests/test_galois_exact.py pins that.
+
+rotation_exact() is ApplyGaloisKeySwitch exactly: the exact key switch (tests/ks_exact.py) of [sigma(c0), 0] with the
+digits sigma(c1).
 """
 from __future__ import annotations
 
 import numpy as np
 
+import ks_exact
 from ntt_exact import _brv
 from util import uniform_below
 
@@ -55,6 +59,20 @@ def sigma_int(coeffs, n, g):
         else:
             out[k - n] = -c
     return out
+
+
+def rotation_exact(port, case, ct, g, batch):
+    """ks_exact of r = [sigma(c0), 0] with t = sigma(c1), per ciphertext: `batch` ciphertexts of the ks_exact.Case
+    `case` (two components of decomp limbs each, NTT form) back to back"""
+    comp = case.decomp * case.n
+    out = []
+    for c in range(batch):
+        c0 = ct[2 * c * comp:(2 * c + 1) * comp]
+        c1 = ct[(2 * c + 1) * comp:(2 * c + 2) * comp]
+        r = np.concatenate([sigma_ntt(c0, case.n, g), np.zeros(comp, dtype=U64)])
+        out.append(ks_exact.key_switch_exact(port, r, sigma_ntt(c1, case.n, g), *case.shape, case.keys,
+                                             case.modswitch))
+    return np.concatenate(out)
 
 
 def galois_keys(port, s, g, n, mods, decomp, error_seed, bound_e):

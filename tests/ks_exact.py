@@ -98,10 +98,12 @@ def make_case(port, name, n=None):
     one_digit     1 digit (SEAL's level above the bottom) of a 50-bit prime, so rns_modulus_size = 2
     slots         kcc3 with 3 unused key slots between the digits and the special prime
                   (key_modulus_size = rns_modulus_size + 3)
+    slots2        slots with key_component_count 2, the only count the rotations take
     small_special 3 digits of 50-bit primes and a 29-bit special prime, smaller than every digit: its inverse transform
                   runs the 32-bit-word kernels, and the mod-down moves values into larger moduli
     kcc3_wrap     17 digits just below 2^61 with key_component_count 3: one multiply-accumulate launch holds 16 digits
                   there, so every modulus takes two launches
+    wrap17        kcc3_wrap with key_component_count 2: the rotations' two launches (16 + 1 digits) per element
     seal_chain    a SEAL-style chain: first digit just below 2^61, larger than the special prime (just above 2^60),
                   then 40-bit digits, so the multi-modulus transforms run in WIDE mode; digits in [0, 2q); one unused
                   key slot between the digits and the special prime (key_modulus_size = rns_modulus_size + 1)
@@ -117,10 +119,10 @@ def make_case(port, name, n=None):
         n = n or 1 << 12
         mods = primes(5, 50, True, n)
         decomp = 4
-    elif name in ("kcc1", "kcc3", "slots"):
+    elif name in ("kcc1", "kcc3", "slots", "slots2"):
         n = n or 1 << 12
-        decomp, kcc = 3, 1 if name == "kcc1" else 3
-        mods = primes(7 if name == "slots" else 4, 50, True, n)
+        decomp, kcc = 3, {"kcc1": 1, "slots2": 2}.get(name, 3)
+        mods = primes(7 if name in ("slots", "slots2") else 4, 50, True, n)
     elif name == "one_digit":
         n = n or 1 << 12
         decomp = 1
@@ -130,9 +132,9 @@ def make_case(port, name, n=None):
         decomp = 3
         mods = primes(3, 50, True, n) + primes(1, 29, True, n)
         assert mods[-1] < 1 << 30 and mods[-1] < min(mods[:decomp])
-    elif name == "kcc3_wrap":
+    elif name in ("kcc3_wrap", "wrap17"):
         n = n or 1 << 12
-        decomp, kcc = 17, 3
+        decomp, kcc = 17, 3 if name == "kcc3_wrap" else 2
         mods = primes(18, 60, False, n)
     elif name == "seal_chain":
         n = n or 1 << 12

@@ -298,25 +298,12 @@ def _ciphertexts(case, batch, seed):
                            for c in range(2 * batch) for i in range(d)])
 
 
-def _rotation_exact(port, case, ct, g, batch):
-    """ks_exact of r = [sigma(c0), 0] with t = sigma(c1), per ciphertext"""
-    comp = case.decomp * case.n
-    out = []
-    for c in range(batch):
-        c0 = ct[2 * c * comp:(2 * c + 1) * comp]
-        c1 = ct[(2 * c + 1) * comp:(2 * c + 2) * comp]
-        r = np.concatenate([gx.sigma_ntt(c0, case.n, g), np.zeros(comp, dtype=U64)])
-        out.append(ks_exact.key_switch_exact(port, r, gx.sigma_ntt(c1, case.n, g), *case.shape, case.keys,
-                                             case.modswitch))
-    return np.concatenate(out)
-
-
 def _ks_prepared(port, name, g, n=None):
     if (name, g, n) not in _ks_cache:
         case = ks_exact.make_case(port, name, n)
         gg = 2 * case.n - 1 if g == "2n-1" else g
         ct = _ciphertexts(case, 3, 11)
-        _ks_cache[name, g, n] = case, gg, ct, _rotation_exact(port, case, ct, gg, 3)
+        _ks_cache[name, g, n] = case, gg, ct, gx.rotation_exact(port, case, ct, gg, 3)
     return _ks_cache[name, g, n]
 
 
@@ -393,7 +380,7 @@ def test_apply_galois_key_switch_graph_replay(hb, port):
     d.copy_(dev(ct2))
     graph.replay()
     torch.cuda.synchronize()
-    _check(host(d), _rotation_exact(port, case, ct2, g, 3), "graph replay, new data")
+    _check(host(d), gx.rotation_exact(port, case, ct2, g, 3), "graph replay, new data")
 
 
 def test_apply_galois_key_switch_refuses_sharded_keys(hb, port):

@@ -338,8 +338,10 @@ def test_concurrent_host_threads(hb, checker):
     """The reference is "single-threaded and thread-safe" (README.md:264-265): many host
     threads may call it at once.  Eight threads share one NTT object and the NTT cache and
     mix device-pointer calls (each on its own stream), host-pointer calls (which share the
-    per-device staging buffers) and KeySwitch-style scratch use; ctypes drops the GIL for
-    the duration of every call, so the calls really overlap."""
+    per-device staging buffers) and lookups in the NTT cache that race with its first
+    creation of a handle; ctypes drops the GIL for the duration of every call, so the calls
+    really overlap.  No composite runs here: the rotations from several threads, sharing
+    the scratch pool and the staging slots, are in test_gpu_rotation_shapes.py."""
     import threading
     n = 1 << 12
     q = hb.GeneratePrimes(1, 55, True, n)[0]

@@ -13,10 +13,11 @@ import pytest
 
 import ks_exact
 
-NON_WRAPPING = ("uniform", "seal_chain", "word_classes", "kcc1", "kcc3", "one_digit", "slots", "small_special")
+NON_WRAPPING = ("uniform", "seal_chain", "word_classes", "kcc1", "kcc3", "one_digit", "slots", "slots2",
+                "small_special")
 # the older cases run at two row-kernel degrees; the shape variants also at the tiny-kernel degrees 2, 4 and 8
 DEGREES = {name: (1 << 8, 1 << 11) for name in ("uniform", "seal_chain", "word_classes")}
-WRAPPING = ("wrap_keys", "wrap_blocks", "kcc3_wrap")
+WRAPPING = ("wrap_keys", "wrap_blocks", "kcc3_wrap", "wrap17")
 
 
 def test_exact_model_gives_the_reference_kat(port):
@@ -36,7 +37,7 @@ def test_exact_model_gives_the_reference_kat(port):
 def test_exact_model_equals_checkers_where_they_do_not_wrap(request, port, checker_kind, name):
     """uniform moduli; a SEAL-style chain with a digit prime larger than the special prime, digits in [0, 2q) and
     key_modulus_size > rns_modulus_size; moduli of all three word classes in one switch; key_component_count 1 and 3;
-    one digit; three unused key slots; a special prime smaller than every digit"""
+    one digit; three unused key slots, with three components and with two; a special prime smaller than every digit"""
     chk = port if checker_kind == "port" else request.getfixturevalue("ref")
     if checker_kind == "ref" and not chk.has_seal:
         pytest.skip("oracle/_ref was built without the experimental/seal sources")
@@ -54,16 +55,16 @@ def test_exact_model_equals_checkers_where_they_do_not_wrap(request, port, check
 @pytest.mark.parametrize("name", NON_WRAPPING + WRAPPING)
 def test_cases_have_the_shapes_their_names_say(port, name):
     """wraps is set exactly on the cases whose 128-bit sum can wrap, so the GPU tests compare the checkers with the
-    model on every other case; kcc3_wrap needs two multiply-accumulate launches of 16 digits and 1 digit"""
+    model on every other case; kcc3_wrap and wrap17 need two multiply-accumulate launches of 16 digits and 1 digit"""
     case = ks_exact.make_case(port, name)
     assert case.wraps == (name in WRAPPING)
-    shape = {"kcc1": (3, 4, 1), "kcc3": (3, 4, 3), "one_digit": (1, 2, 2), "slots": (3, 7, 3),
-             "small_special": (3, 4, 2), "kcc3_wrap": (17, 18, 3)}
+    shape = {"kcc1": (3, 4, 1), "kcc3": (3, 4, 3), "one_digit": (1, 2, 2), "slots": (3, 7, 3), "slots2": (3, 7, 2),
+             "small_special": (3, 4, 2), "kcc3_wrap": (17, 18, 3), "wrap17": (17, 18, 2)}
     if name in shape:
         assert (case.decomp, case.kms, case.kcc) == shape[name]
     if name == "small_special":
         assert case.mods[-1] < 1 << 30 < min(case.mods[:case.decomp])
-    if name == "kcc3_wrap":
+    if name in ("kcc3_wrap", "wrap17"):
         q = max(case.mods)
         assert (1 << 60) < min(case.mods) and q < (1 << 61)
         per_launch = ((1 << 128) - 1) // ((4 * q - 1) * (q - 1))
