@@ -1,4 +1,4 @@
-// Internal interfaces between the C ABI (capi.cu) and the kernel launchers.
+// Internal interfaces between the C ABI (capi*.cu) and the kernel launchers.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

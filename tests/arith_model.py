@@ -74,7 +74,7 @@ def csub(x, b):
 
 
 def prod_constants(q):
-    """capi.cu:dyadic_modulus -- shift = bits(q) - 2, mu = floor(2^(shift + 64) / q)"""
+    """capi.h:dyadic_modulus -- shift = bits(q) - 2, mu = floor(2^(shift + 64) / q)"""
     shift = q.bit_length() - 2
     return (1 << (shift + 64)) // q, shift
 
@@ -183,7 +183,7 @@ def shoup_lazy(x, w, q):
 
 
 def ks_mac_digits_per_launch(q):
-    """capi.cu:ks_mac_digits_per_launch -- digits one ks_mac_kernel launch adds up for moduli up to q: each product is
+    """capi_keyswitch.cu:ks_mac_digits_per_launch -- digits one ks_mac_kernel launch adds up for moduli up to q: each product is
     a lazy transform output (< 4q) times a key word (< q), and their sum must stay below 2^128"""
     return min(64, ((1 << 128) - 1) // ((4 * q - 1) * (q - 1)))
 

@@ -1,4 +1,4 @@
-"""The scratch rounds of the RNS composites (hexl_b200/csrc/capi.cu) restated in Python, and the shapes of
+"""The scratch rounds of the RNS composites (hexl_b200/csrc/capi_keyswitch.cu, capi_galois.cu) restated in Python, and the shapes of
 tests/test_gpu_composite_rounds.py.
 
 Each composite splits one device call into rounds that fit about 256 MiB of pool scratch:
@@ -8,7 +8,8 @@ Each composite splits one device call into rounds that fit about 256 MiB of pool
     key_switch_rounds       key_switch_on_device, step 2: RNS moduli per round
     ks_mac_launches         the digits of each ks_mac_kernel launch within one round (ks_mac_digits_per_launch)
 
-Every function returns the list of round (or launch) sizes.  SOURCE holds the capi.cu lines each formula restates;
+Every function returns the list of round (or launch) sizes.  SOURCE holds the source file under hexl_b200/csrc and the
+lines of it each formula restates;
 tests/test_composite_plan.py asserts they are still there, so a change of the budget or of a formula fails on the CPU
 before the GPU test silently runs a single round.
 """
@@ -18,14 +19,18 @@ PARAM_BLOCK = 64          # internal.h: kParamBlock, moduli per kernel parameter
 SCRATCH_BYTES = 256 << 20
 
 SOURCE = {
-    "rescale": ["const uint64_t block = std::min<uint64_t>(L, kParamBlock);",
-                "uint64_t chunk = std::max<uint64_t>(1, (256ull << 20) / ((block + 1) * n * 8));",
-                "chunk = std::min(chunk, count);"],
-    "galois": ["const uint64_t chunk = std::min<uint64_t>(count, std::max<uint64_t>(1, (256ull << 20) / (unit * 8)));"],
-    "key_switch": ["uint64_t ichunk = std::max<uint64_t>(1, (256ull << 20) / (per_mod * 8));",
-                   "ichunk = std::min<uint64_t>({ichunk, rns, (uint64_t)kParamBlock});"],
-    "ks_mac": ["const unsigned __int128 largest_product = (unsigned __int128)(4 * q - 1) * (q - 1);",
-               "return (uint64_t)std::min<unsigned __int128>(kParamBlock, ~(unsigned __int128)0 / largest_product);"],
+    "rescale": ("capi_keyswitch.cu",
+                ["const uint64_t block = std::min<uint64_t>(L, kParamBlock);",
+                 "uint64_t chunk = std::max<uint64_t>(1, (256ull << 20) / ((block + 1) * n * 8));",
+                 "chunk = std::min(chunk, count);"]),
+    "galois": ("capi_galois.cu",
+               ["const uint64_t chunk = std::min<uint64_t>(count, std::max<uint64_t>(1, (256ull << 20) / (unit * 8)));"]),
+    "key_switch": ("capi_keyswitch.cu",
+                   ["uint64_t ichunk = std::max<uint64_t>(1, (256ull << 20) / (per_mod * 8));",
+                    "ichunk = std::min<uint64_t>({ichunk, rns, (uint64_t)kParamBlock});"]),
+    "ks_mac": ("capi_keyswitch.cu",
+               ["const unsigned __int128 largest_product = (unsigned __int128)(4 * q - 1) * (q - 1);",
+                "return (uint64_t)std::min<unsigned __int128>(kParamBlock, ~(unsigned __int128)0 / largest_product);"]),
 }
 
 

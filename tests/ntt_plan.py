@@ -15,7 +15,7 @@ import ntt_exact as nx
 # ntt_kernels.cuh: enum { kGeneric = 0, kFast = 1, kSmall = 2, kWide = 3 }
 GENERIC, FAST, SMALL, WIDE = 0, 1, 2, 3
 DEEP = 64                           # plan_single_pass: the pipelined forward takes 64 <= batch < 2^31 polynomials
-CHUNK_WORDS = (32 << 20) // 8       # capi.cu: kChunkBytes of host-pointer staging, in 64-bit words
+CHUNK_WORDS = (32 << 20) // 8       # capi.h: kChunkBytes of host-pointer staging, in 64-bit words
 
 # ------------------------------------------------------------------------------------------------ the parameter set
 LOGNS = list(range(1, nx.MAX_LOGN + 1))
@@ -41,7 +41,7 @@ def batches(log_n):
 
 
 def chunk_polys(log_n):
-    """polynomials per staging chunk of a host-pointer call (capi.cu:run_host_on_device): whole polynomials up to
+    """polynomials per staging chunk of a host-pointer call (capi.h:run_host_on_device): whole polynomials up to
     kChunkBytes"""
     return max(1, CHUNK_WORDS >> log_n)
 

@@ -1,9 +1,9 @@
-"""The scratch rounds of the RNS composites, restated in tests/composite_plan.py, against capi.cu and against the shapes
-of tests/test_gpu_composite_rounds.py (CPU only).
+"""The scratch rounds of the RNS composites, restated in tests/composite_plan.py, against the host sources that run them
+and against the shapes of tests/test_gpu_composite_rounds.py (CPU only).
 
 The GPU test is only worth its time if every one of its calls runs more than one round and the last round is shorter
 than the others, so that a round that reads or writes the first round's polynomials (or moduli) again gives a wrong
-answer somewhere.  This file asserts that of every shape, and that the formulas are still the ones capi.cu runs."""
+answer somewhere.  This file asserts that of every shape, and that the formulas are still the ones the host sources run."""
 import os
 
 import pytest
@@ -18,14 +18,15 @@ def _several_uneven(rounds):
     return len(rounds) >= 2 and rounds[-1] < rounds[0] and all(r == rounds[0] for r in rounds[:-1])
 
 
-def test_formulas_are_the_ones_capi_cu_runs():
-    with open(os.path.join(ROOT, "hexl_b200", "csrc", "capi.cu")) as f:
-        src = f.read()
-    with open(os.path.join(ROOT, "hexl_b200", "csrc", "internal.h")) as f:
+def test_formulas_are_the_ones_the_host_sources_run():
+    csrc = os.path.join(ROOT, "hexl_b200", "csrc")
+    with open(os.path.join(csrc, "internal.h")) as f:
         assert f"constexpr int kParamBlock = {plan.PARAM_BLOCK};" in f.read()
-    for what, lines in plan.SOURCE.items():
+    for what, (name, lines) in plan.SOURCE.items():
+        with open(os.path.join(csrc, name)) as f:
+            src = f.read()
         for line in lines:
-            assert line in src, f"{what}: capi.cu no longer has `{line}`; restate the change in composite_plan.py"
+            assert line in src, f"{what}: {name} no longer has `{line}`; restate the change in composite_plan.py"
 
 
 def test_spot_values():

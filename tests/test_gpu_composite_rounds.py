@@ -1,5 +1,5 @@
 """The RNS composites at production sizes, where one device call runs its scratch rounds more than once
-(the rounds are restated in tests/composite_plan.py, which tests/test_composite_plan.py checks against capi.cu):
+(the rounds are restated in tests/composite_plan.py, which tests/test_composite_plan.py checks against the host sources):
 
     DivideAndRoundQLast, NTT form    polynomials per round: seal chain at N = 2^16, 31 limbs, 35 polynomials in rounds
                                      of 16, 16 and 3; 70 limbs at 2^14, 33 polynomials in rounds of 31 and 2, each round

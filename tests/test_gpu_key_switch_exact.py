@@ -3,7 +3,9 @@
     device      hexl_b200_key_switch with device pointers
     host        hexl_b200_key_switch with host pointers (keys uploaded per call, staging streams)
     resident    hexl_b200_key_switch_resident, batch 2, host and device buffers
-    sharded     a handle sharded by modulus over three shards on device 0 (its own multiply-accumulate loop)
+    sharded     a handle sharded by modulus over three shards on device 0
+    sharded_one the same over a single shard: with wrap_blocks' 71 moduli, the shard's multiply-accumulate rounds and
+                mod-down blocks each run two parameter blocks
     sharded_rns+2  the same with rns_modulus_size + 2 devices listed, at N = 2 and 4; the upload cuts the list to
                    rns_modulus_size shards of one modulus each
 
@@ -44,7 +46,7 @@ def _entries(logn):
     return ENTRY_POINTS if logn == 17 or logn in SMALL_LOGNS else ("device", "host")
 
 
-CASES = ([(name, None, entry) for name in GPU_CASES for entry in ENTRY_POINTS]
+CASES = ([(name, None, entry) for name in GPU_CASES for entry in ENTRY_POINTS + ("sharded_one",)]
          + [(name, logn, entry) for name, logn in DEGREES for entry in _entries(logn)])
 
 
@@ -113,7 +115,7 @@ def test_key_switch_equals_exact_model(hb, port, checker, name, logn, entry):
         hb.KeySwitchResident(d, dev(both_t), *case.shape, handle, case.modswitch, 2)
         _check(host(d), np.concatenate(exp), f"{name} resident device batch 2")
     else:
-        shards = 3 if entry == "sharded" else case.rns + 2
+        shards = {"sharded": 3, "sharded_one": 1}.get(entry, case.rns + 2)
         try:
             hb.set_host_devices([0] * shards)
             handle = hb.KeySwitchKeys(case.keys, case.n, case.decomp, case.kms, case.kcc, sharded_by_modulus=True)
