@@ -127,6 +127,8 @@ _sig("hexl_b200_key_switch_resident", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _
 _sig("hexl_b200_apply_galois_key_switch", _int, [_vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _u64, _vp])
 _sig("hexl_b200_apply_galois_key_switch_hoisted", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp])
+_sig("hexl_b200_fast_base_convert", _int, [_vp, _vp, _u64, _vp, _u64, _vp, _u64, _u64, _vp])
+_sig("hexl_b200_key_switch_hybrid", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -607,3 +609,32 @@ def ApplyGaloisKeySwitchHoisted(results, ciphertexts, n, decomp_modulus_size, ke
                                                           keys, elts.ctypes.data, elts.size, ms.ctypes.data, batch,
                                                           _stream(stream, rc or cc)))
     return results
+
+
+def FastBaseConvert(result, operand, n, from_moduli, to_moduli, count=1, stream=None):
+    """Fast base conversion (hexl_b200_fast_base_convert) of `count` polynomials, coefficient form: polynomial p of
+    operand holds len(from_moduli) limbs of n words, its result len(to_moduli) limbs,
+    result_e = [sum_i [x_i (Q/q_i)^-1]_{q_i} [Q/q_i]_{t_e}]_{t_e}."""
+    src = np.ascontiguousarray(from_moduli, dtype=np.uint64)
+    dst = np.ascontiguousarray(to_moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); op, on, oc = _buf(operand)
+    _need("result", rn, count * dst.size * n); _need("operand", on, count * src.size * n)
+    _check(_lib.hexl_b200_fast_base_convert(rp, op, n, src.ctypes.data, src.size, dst.ctypes.data, dst.size, count,
+                                            _stream(stream, rc or oc)))
+    return result
+
+
+def KeySwitchHybrid(result, target, n, level_size, q_size, p_size, digit_size, key_component_count, moduli,
+                    keys: KeySwitchKeys, batch=1, stream=None):
+    """Hybrid key switch (hexl_b200_key_switch_hybrid) of `batch` ciphertexts at level level_size: moduli holds the
+    q_size data moduli, then the p_size special primes; keys were uploaded with decomp = ceil(q_size / digit_size) and
+    key_modulus_size = q_size + p_size.  Ciphertext c reads target[c * level_size*n:] and accumulates into
+    result[c * key_component_count*level_size*n:]."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); tp, tn, tc = _buf(target)
+    _need("moduli", mods.size, q_size + p_size)
+    _need("result", rn, batch * key_component_count * level_size * n); _need("target", tn, batch * level_size * n)
+    _check(_lib.hexl_b200_key_switch_hybrid(rp, tp, n, level_size, q_size, p_size, digit_size, key_component_count,
+                                            mods.ctypes.data, keys._h if keys is not None else None, batch,
+                                            _stream(stream, rc or tc)))
+    return result

@@ -1,5 +1,6 @@
 // What the host sources of the C ABI (include/hexl_b200.h) share: capi.cu (library state, staging, scratch pool),
-// capi_ntt.cu, capi_eltwise.cu, capi_keyswitch.cu (key switch, key handles, rescale) and capi_galois.cu.
+// capi_ntt.cu, capi_eltwise.cu, capi_keyswitch.cu (key switch, key handles, rescale), capi_galois.cu and
+// capi_hybrid.cu (hybrid key switch, fast base conversion).
 // Host-side responsibilities, all one-off or O(1) per call:
 //   * argument validation mirroring the reference's HEXL_CHECKs,
 //   * NTT handle = (N, q, root) -> twiddle tables, built on the host exactly as
@@ -373,6 +374,13 @@ uint64_t keys_on_device(const hexl_b200_keys* const* keys, uint64_t count, int d
 int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, uint64_t n, uint64_t decomp,
                          uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
                          const uint64_t* const* d_key_ptrs_host, const uint64_t* modswitch, cudaStream_t s);
+// The multiply-accumulate of one step-2 round: ops ([e][j][n], lazily transformed digits under the round's cnt moduli,
+// hs[e] their transforms and slots[e] their slots in keys of kms slots) times the keys of each of `elts` switches,
+// into prod + r * prod_stride ([e][k][n]); chunked by ks_mac_digits_per_launch.  keys[r][j]: digit j's key of switch
+// r; galois_elts[r] (nullptr: none) makes switch r read the digits permuted by pi_g.
+int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cnt, uint64_t kms, const uint64_t* ops,
+                    uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod, uint64_t prod_stride,
+                    const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s);
 int key_switch_elts_on_device(int dev, uint64_t* const* results, const uint64_t* t_target, uint64_t n, uint64_t decomp,
                               uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
                               const uint64_t* const* const* d_key_ptrs, const uint64_t* galois_elts, uint64_t elts,

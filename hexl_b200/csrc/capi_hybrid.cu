@@ -1,0 +1,267 @@
+// Hybrid key switching (OpenFHE's KeySwitchHYBRID): digits of up to 64 data moduli and up to 64 special primes, the
+// mod-up and the mod-down by fast base conversion (rns.cu); and the base conversion on its own.
+#include <numeric>
+
+#include "capi.h"
+
+using namespace hexl_b200;
+
+namespace hexl_b200 {
+
+static uint64_t mul_mod128(uint64_t a, uint64_t b, uint64_t m) { return (uint64_t)((unsigned __int128)a * b % m); }
+
+// floor(M/2) mod m for M the product of `count` odd moduli (M odd, so floor(M/2) = (M - 1) / 2) and m odd
+static uint64_t half_product_mod(const uint64_t* moduli, uint64_t count, uint64_t m) {
+  uint64_t r = 1 % m;
+  for (uint64_t i = 0; i < count; ++i) r = mul_mod128(r, moduli[i] % m, m);
+  return mul_mod128((r + m - 1) % m, (m + 1) / 2, m);  // (m + 1) / 2 = 2^-1 mod m
+}
+
+// Base conversion of `polys` polynomials from the moduli `from` (pairwise coprime, Q their product) into the moduli
+// `to`, device pointers on the current device, asynchronous on s; strides as launch_base_conv.  One launch per block of
+// base_conv_targets(from_count) targets; the constants are computed here, per call.  round (the mod-down by
+// P = Q): x_i + [floor(P/2)]_{q_i} on input and - [floor(P/2)]_t on output, so that an input X in [0, P) comes out as
+// the centred lift of X + floor(P/2) minus floor(P/2), plus e P with 0 <= e < from_count.
+static int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t res_poly, const uint64_t* operand,
+                                  uint64_t op_limb, uint64_t op_poly, uint64_t n, uint64_t polys,
+                                  const uint64_t* from, uint64_t from_count, const uint64_t* to, uint64_t to_count,
+                                  bool round, cudaStream_t s) {
+  const uint64_t F = from_count, block = base_conv_targets(F);
+  BaseConvTable tab;
+  // (Q/q_i)^-1 mod q_i from prefix and suffix products under q_i
+  for (uint64_t i = 0; i < F; ++i) {
+    const uint64_t q = from[i];
+    uint64_t rest = 1 % q;
+    for (uint64_t j = 0; j < F; ++j)
+      if (j != i) rest = mul_mod128(rest, from[j] % q, q);
+    const Twiddle inv = make_twiddle(nt::inverse_mod(rest, q), q);
+    tab.w[4 * i] = q;
+    tab.w[4 * i + 1] = inv.w;
+    tab.w[4 * i + 2] = inv.wp;
+    tab.w[4 * i + 3] = round ? half_product_mod(from, F, q) : 0;
+  }
+  std::vector<uint64_t> prefix(F + 1), suffix(F + 1);
+  for (uint64_t e0 = 0; e0 < to_count; e0 += block) {
+    const uint64_t cnt = std::min(block, to_count - e0);
+    uint64_t* targets = tab.w + 4 * F;
+    uint64_t* matrix = targets + 5 * cnt;
+    for (uint64_t e = 0; e < cnt; ++e) {
+      const uint64_t t = to[e0 + e], mu = nt::multiply_factor(1, 64, t);
+      const Twiddle R = make_twiddle(mu * (0 - t) % t, t);  // 2^64 mod t
+      targets[5 * e] = t;
+      targets[5 * e + 1] = mu;
+      targets[5 * e + 2] = R.w;
+      targets[5 * e + 3] = R.wp;
+      targets[5 * e + 4] = round ? half_product_mod(from, F, t) : 0;
+      prefix[0] = suffix[F] = 1 % t;
+      for (uint64_t i = 0; i < F; ++i) prefix[i + 1] = mul_mod128(prefix[i], from[i] % t, t);
+      for (uint64_t i = F; i-- > 0;) suffix[i] = mul_mod128(suffix[i + 1], from[i] % t, t);
+      for (uint64_t i = 0; i < F; ++i) matrix[e * F + i] = mul_mod128(prefix[i], suffix[i + 1], t);  // [Q/q_i]_t
+    }
+    const cudaError_t e = launch_base_conv(result + e0 * res_limb, res_limb, res_poly, operand, op_limb, op_poly, n,
+                                           polys, F, cnt, tab, s);
+    if (e != cudaSuccess) return cuda_fail(e, "base conversion launch");
+  }
+  return 0;
+}
+
+// One hybrid key switch (include/hexl_b200.h has the definitions), every pointer a device pointer on the current
+// device, asynchronous on s.  h holds the transforms of the extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}} in that
+// order and bmods their moduli; keys[d] is digit d's key buffer, kcc x (q_size + K) x n words.  Scratch layouts are
+// [modulus][digit or component][n], as in key_switch_elts_on_device.
+static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level,
+                                       uint64_t q_size, uint64_t p_size, uint64_t alpha, uint64_t kcc,
+                                       const CachedNtts& h, const uint64_t* bmods, const uint64_t* const* keys,
+                                       cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size;
+  // moduli handled per round of the mod-up: bounded by the parameter block and by ~256 MiB of scratch
+  const uint64_t per_mod = D * n;
+  uint64_t ichunk = std::max<uint64_t>(1, (256ull << 20) / (per_mod * 8));
+  ichunk = std::min<uint64_t>({ichunk, nb, (uint64_t)kParamBlock});
+  Scratch ws(s);
+  uint64_t *t_coef = nullptr, *ops = nullptr, *prod = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&t_coef, level * n)) return rc;
+  if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;                                  // [e][d][n]
+  if (int rc = ws.get(&prod, nb * kcc * n)) return rc;                                      // [b][k][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * kcc * n)) return rc;  // [i][k][n], one block
+  // 1. the target's limbs back to coefficients, canonical
+  if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s)) return rc;
+  // 2. mod-up: every digit converted into each modulus of the round, lazily transformed, multiplied with the keys.
+  //    (A digit's own limbs are converted and transformed again like the others: NTT(INTT(t)) = t.)
+  const uint64_t* const* key_sets = keys;
+  for (uint64_t b0 = 0; b0 < nb; b0 += ichunk) {
+    const uint64_t cnt = std::min(ichunk, nb - b0);
+    for (uint64_t d = 0; d < D; ++d) {
+      const uint64_t lo = d * alpha, width = std::min(alpha, level - lo);
+      if (int rc = base_convert_on_device(ops + d * n, per_mod, 0, t_coef + lo * n, n, 0, n, 1, bmods + lo, width,
+                                          bmods + b0, cnt, false, s))
+        return rc;
+    }
+    if (int rc = ntt_multi_on_device(true, dev, h.data() + b0, cnt, ops, ops, 4, D, s)) return rc;
+    uint64_t slots[kParamBlock];
+    for (uint64_t e = 0; e < cnt; ++e) slots[e] = b0 + e < level ? b0 + e : q_size + (b0 + e - level);
+    if (int rc = ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, kcc, prod + b0 * kcc * n, 0, &key_sets,
+                                 nullptr, 1, s))
+      return rc;
+  }
+  // 3. mod-down by P: the special limbs back to coefficients, rounded and converted into each data modulus,
+  //    transformed, and (prod - that) * P^-1 accumulated into result
+  uint64_t* special = prod + level * kcc * n;  // [j][k][n]
+  if (int rc = ntt_multi_on_device(false, dev, h.data() + level, p_size, special, special, 1, kcc, s)) return rc;
+  for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
+    const uint64_t cnt = std::min<uint64_t>(kParamBlock, level - i0);
+    if (int rc = base_convert_on_device(tmp, kcc * n, n, special, kcc * n, n, n, kcc, bmods + level, p_size,
+                                        bmods + i0, cnt, true, s))
+      return rc;
+    if (int rc = ntt_multi_on_device(true, dev, h.data() + i0, cnt, tmp, tmp, 4, kcc, s)) return rc;
+    KsModuli fin;
+    for (uint64_t e = 0; e < cnt; ++e) {
+      const uint64_t q = bmods[i0 + e];
+      uint64_t P = 1 % q;
+      for (uint64_t j = 0; j < p_size; ++j) P = mul_mod128(P, bmods[level + j] % q, q);
+      const Twiddle f = make_twiddle(nt::inverse_mod(P, q), q);
+      fin.m[e] = KsModulus{q, nt::multiply_factor(1, 64, q), f.w, f.wp, 0};
+    }
+    const cudaError_t e = launch_ks_finish(result, prod + i0 * kcc * n, tmp, n, kcc, level, i0, cnt, fin, false, true, s);
+    if (e != cudaSuccess) return cuda_fail(e, "hybrid mod-down: finish launch");
+  }
+  return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
+}
+
+// Host buffers of the base conversion: whole polynomials through the staging slots, split by polynomial over the host
+// devices; a slot holds one chunk of input polynomials and one of results.
+static int base_convert_host(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* from,
+                             uint64_t from_count, const uint64_t* to, uint64_t to_count, uint64_t count) {
+  std::vector<int> devs;
+  if (int rc = host_devices(&devs)) return rc;
+  const uint64_t in_words = from_count * n, out_words = to_count * n;
+  const uint64_t chunk = std::max<uint64_t>(1, (kChunkBytes / 8) / std::max(in_words, out_words));
+  const uint64_t ndev = std::min<uint64_t>(devs.size(), count);
+  int rc = 0;
+  for (uint64_t di = 0; di < ndev && !rc; ++di) {
+    const uint64_t lo = count * di / ndev, hi = count * (di + 1) / ndev;
+    DeviceGuard g;
+    if ((rc = g.enter(devs[di]))) break;
+    StageCtx* st = stage_for(devs[di]);
+    std::lock_guard<std::mutex> lk(st->mu);
+    if ((rc = st->init())) break;
+    int slot = 0;
+    for (uint64_t p0 = lo; p0 < hi && !rc; p0 += chunk, slot = (slot + 1) % kSlots) {
+      const uint64_t cnt = std::min(chunk, hi - p0);
+      if ((rc = st->reserve(slot, 0, cnt * out_words * 8)) || (rc = st->reserve(slot, 1, cnt * in_words * 8))) break;
+      const cudaStream_t sx = st->stream[slot];
+      cudaError_t e = cudaMemcpyAsync(st->buf[slot][1], operand + p0 * in_words, cnt * in_words * 8,
+                                      cudaMemcpyHostToDevice, sx);
+      if (e != cudaSuccess) {
+        rc = cuda_fail(e, "FastBaseConvert H2D");
+        break;
+      }
+      if ((rc = base_convert_on_device(st->buf[slot][0], n, out_words, st->buf[slot][1], n, in_words, n, cnt, from,
+                                       from_count, to, to_count, false, sx)))
+        break;
+      e = cudaMemcpyAsync(result + p0 * out_words, st->buf[slot][0], cnt * out_words * 8, cudaMemcpyDeviceToHost, sx);
+      if (e != cudaSuccess) rc = cuda_fail(e, "FastBaseConvert D2H");
+    }
+  }
+  for (uint64_t di = 0; di < ndev; ++di) {  // always drain: host buffers are in flight
+    const int rc2 = sync_stage(devs[di]);
+    if (!rc) rc = rc2;
+  }
+  return rc;
+}
+
+}  // namespace hexl_b200
+
+// =============================================================== extern "C"
+extern "C" {
+
+int hexl_b200_fast_base_convert(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* from_moduli,
+                                uint64_t from_count, const uint64_t* to_moduli, uint64_t to_count, uint64_t count,
+                                void* stream) {
+  REQUIRE(result && operand && from_moduli && to_moduli, "Require non-null arguments");
+  REQUIRE(n >= 1, "Require n >= 1");
+  REQUIRE(from_count >= 1 && from_count <= (uint64_t)kParamBlock, "Require 1 <= from_count <= %d", kParamBlock);
+  REQUIRE(to_count >= 1, "Require to_count >= 1");
+  for (uint64_t i = 0; i < from_count; ++i)
+    REQUIRE(from_moduli[i] > 1 && from_moduli[i] < (1ull << 61), "Require 1 < from_moduli[%llu] < 2^61",
+            (unsigned long long)i);
+  for (uint64_t e = 0; e < to_count; ++e)
+    REQUIRE(to_moduli[e] > 1 && to_moduli[e] < (1ull << 61), "Require 1 < to_moduli[%llu] < 2^61",
+            (unsigned long long)e);
+  for (uint64_t i = 0; i < from_count; ++i)
+    for (uint64_t j = 0; j < i; ++j)
+      REQUIRE(std::gcd(from_moduli[i], from_moduli[j]) == 1, "Require from_moduli pairwise coprime (%llu and %llu)",
+              (unsigned long long)j, (unsigned long long)i);
+  if (count == 0) return 0;
+  const uint64_t in_total = count * from_count * n, out_total = count * to_count * n;
+  REQUIRE(result + out_total <= operand || operand + in_total <= result, "result and operand must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, operand}, &pi)) return rc;
+  if (int rc = check_limb_bounds(operand, count, from_count, n, [&](u64 i) { return from_moduli[i]; }, pi, "operand"))
+    return rc;
+  if (pi.where == Where::Device)
+    return run_on_device(pi, stream, [&] {
+      return base_convert_on_device(result, n, to_count * n, operand, n, from_count * n, n, count, from_moduli,
+                                    from_count, to_moduli, to_count, false, (cudaStream_t)stream);
+    });
+  return base_convert_host(result, operand, n, from_moduli, from_count, to_moduli, to_count, count);
+}
+
+int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
+                                uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
+                                const uint64_t* moduli, const hexl_b200_keys* keys, uint64_t batch, void* stream) {
+  const uint64_t level = level_size, alpha = digit_size, kcc = key_component_count, kms = q_size + p_size;
+  REQUIRE(result && target && moduli && keys, "Require non-null arguments");
+  REQUIRE(n >= 2 && n <= (1ull << 20) && !(n & (n - 1)), "Require n a power of two in [2, 2^20]");
+  REQUIRE(level >= 1 && level <= q_size, "Require 1 <= level_size <= q_size");
+  REQUIRE(alpha >= 1 && alpha <= (uint64_t)kParamBlock, "Require 1 <= digit_size <= %d", kParamBlock);
+  REQUIRE(p_size >= 1 && p_size <= (uint64_t)kParamBlock, "Require 1 <= p_size <= %d", kParamBlock);
+  REQUIRE(kcc >= 1, "Require key_component_count >= 1");
+  for (uint64_t i = 0; i < kms; ++i) {
+    const char* why = "";
+    // the lazy sums of the multiply-accumulate and of the finish step (< 8q) need q < 2^61
+    REQUIRE(moduli[i] < (1ull << 61), "Require moduli < 2^61 (moduli[%llu])", (unsigned long long)i);
+    REQUIRE(check_ntt_arguments(n, moduli[i], &why), "moduli[%llu]: %s", (unsigned long long)i, why);
+  }
+  std::vector<uint64_t> sorted(moduli, moduli + kms);
+  std::sort(sorted.begin(), sorted.end());
+  REQUIRE(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end(), "Require distinct moduli");
+  REQUIRE(keys_fit(keys, n, (q_size + alpha - 1) / alpha, kcc, kms),
+          "the key handle was uploaded for another shape (decomp = ceil(q_size / digit_size), "
+          "key_modulus_size = q_size + p_size)");
+  REQUIRE(keys->shards.empty(), "KeySwitchHybrid does not take keys sharded by modulus: upload them with "
+                                "hexl_b200_keys_upload");
+  if (batch == 0) return 0;
+  const uint64_t in_words = level * n, out_words = kcc * level * n;
+  REQUIRE(result + batch * out_words <= target || target + batch * in_words <= result,
+          "result and target must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, target}, &pi)) return rc;
+  if (int rc = check_limb_bounds(target, batch, level, n, [&](u64 i) { return moduli[i]; }, pi, "target")) return rc;
+  // the extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}} and its transforms
+  std::vector<uint64_t> bmods(moduli, moduli + level);
+  bmods.insert(bmods.end(), moduli + q_size, moduli + kms);
+  CachedNtts h(bmods.size());
+  for (uint64_t b = 0; b < bmods.size(); ++b)
+    if (int rc = h.load(b, n, bmods[b])) return rc;
+  if (pi.where == Where::Host)
+    return key_switch_host_batch(result, out_words, true, target, in_words, in_words, &keys, 1, batch,
+                                 [&](int dev, uint64_t* d_res, uint64_t* d_t, const uint64_t* const* const* dk,
+                                     cudaStream_t s) {
+                                   return key_switch_hybrid_on_device(dev, d_res, d_t, n, level, q_size, p_size,
+                                                                      alpha, kcc, h, bmods.data(), dk[0], s);
+                                 });
+  std::vector<const uint64_t* const*> dk;
+  if (keys_on_device(&keys, 1, pi.device, &dk) < 1)
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "the key handle holds no copy on the device of result");
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = key_switch_hybrid_on_device(pi.device, result + c * out_words, target + c * in_words, n, level,
+                                               q_size, p_size, alpha, kcc, h, bmods.data(), dk[0],
+                                               (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+}  // extern "C"

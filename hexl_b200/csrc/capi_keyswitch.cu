@@ -48,6 +48,15 @@ static int ks_mac_round(int dev, hexl_b200_ntt* const* hs, const uint64_t* slots
                         uint64_t* ops, const uint64_t* t_coef, uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod,
                         uint64_t prod_stride, const uint64_t* const* const* keys, const uint64_t* galois_elts,
                         uint64_t elts, cudaStream_t s) {
+  // every digit into every modulus of the round (:77-85) happens inside the transform: it reads the digits from
+  // t_coef (L2-resident) and reduces on load, instead of a reduce kernel writing decomp x cnt x n words for it
+  if (int rc = ntt_multi_on_device(true, dev, hs, cnt, ops, t_coef, 4, decomp, s, nullptr, true)) return rc;
+  return ks_mac_products(hs, slots, cnt, kms, ops, decomp, n, kcc, prod, prod_stride, keys, galois_elts, elts, s);
+}
+
+int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cnt, uint64_t kms, const uint64_t* ops,
+                    uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod, uint64_t prod_stride,
+                    const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s) {
   KsModuli mods;
   for (uint64_t e = 0; e < cnt; ++e) {
     const uint64_t q = hs[e]->q, mu = nt::multiply_factor(1, 64, q);
@@ -55,9 +64,6 @@ static int ks_mac_round(int dev, hexl_b200_ntt* const* hs, const uint64_t* slots
     const Twiddle R = make_twiddle(r64 % q, q);
     mods.m[e] = KsModulus{q, mu, R.w, R.wp, slots[e]};
   }
-  // every digit into every modulus of the round (:77-85) happens inside the transform: it reads the digits from
-  // t_coef (L2-resident) and reduces on load, instead of a reduce kernel writing decomp x cnt x n words for it
-  if (int rc = ntt_multi_on_device(true, dev, hs, cnt, ops, t_coef, 4, decomp, s, nullptr, true)) return rc;
   const uint64_t per_mod = decomp * n, jmax = ks_mac_digits_per_launch(mods, cnt);
   for (uint64_t r = 0; r < elts; ++r)
     for (uint64_t j0 = 0; j0 < decomp; j0 += jmax) {  // key pointers ride in the kernel parameters

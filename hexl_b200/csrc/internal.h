@@ -154,6 +154,23 @@ cudaError_t launch_ks_finish(u64* result, const u64* in, const u64* tmp, u64 n, 
 cudaError_t launch_rescale_coef(u64* result, const u64* operand, u64 n, u64 rns, u64 i0, u64 count, u64 polys,
                                 u64 q_last, u64 mu_last, const KsModuli& mods, cudaStream_t stream);
 
+// Fast base conversion (rns.cu) of `polys` polynomials from `from` <= kParamBlock source moduli q_i (Q = their product)
+// into `to` target moduli t_e, coefficient form; limb i of polynomial p is operand[p op_poly + i op_limb + l], limb e
+// of its result is result[p res_poly + e res_limb + l]:
+//   result_e = [ sum_i [(x_i + add_i) (Q/q_i)^-1]_{q_i} [Q/q_i]_{t_e} - sub_e ]_{t_e},  every modulus below 2^61.
+// The constants travel in the kernel parameters (capturable, no upload); the table holds, in this order:
+//   per source i (4 words):  q_i, (Q/q_i)^-1 mod q_i, its Shoup factor, add_i < q_i
+//   per target e (5 words):  t_e, floor(2^64 / t_e), 2^64 mod t_e, its Shoup factor, sub_e < t_e
+//   per target e (from words): [Q/q_i]_{t_e} for every source i
+// so one launch takes at most base_conv_targets(from) targets; the mod-down's rounding sets add and sub (capi_hybrid.cu).
+constexpr int kBaseConvWords = 480;  // 3840 bytes: with the other arguments inside the 4 KiB of kernel parameters
+struct BaseConvTable {
+  u64 w[kBaseConvWords];
+};
+inline u64 base_conv_targets(u64 from) { return (kBaseConvWords - 4 * from) / (5 + from); }
+cudaError_t launch_base_conv(u64* result, u64 res_limb, u64 res_poly, const u64* operand, u64 op_limb, u64 op_poly,
+                             u64 n, u64 polys, u64 from, u64 to, const BaseConvTable& tab, cudaStream_t stream);
+
 // Galois automorphism sigma_g (galois.cu).  NTT form: `polys` polynomials of 2^log_n words, one launch, words move
 // unchanged (result[j] = operand[pi_g(j)]).  Coefficient form: limbs [i0, i0 + cnt) of `polys` polynomials of rns
 // limbs each, limb i0 + e under mods.q[e]; galois_inv = g^-1 mod 2n.  result and operand must not overlap.

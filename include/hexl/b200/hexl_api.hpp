@@ -676,6 +676,26 @@ inline void ApplyGaloisKeySwitchHoisted(uint64_t* results, const uint64_t* ciphe
       results, ciphertexts, n, decomp_modulus_size, key_modulus_size, rns_modulus_size, key_component_count, moduli,
       handles.data(), galois_elts, num_elts, modswitch_factors, batch, stream));
 }
+
+// extension: fast base conversion of `count` polynomials from from_count moduli into to_count moduli, coefficient form
+// (hexl_b200_fast_base_convert has the layout and the formula).  result and operand must not overlap.
+inline void FastBaseConvert(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* from_moduli,
+                            uint64_t from_count, const uint64_t* to_moduli, uint64_t to_count, uint64_t count = 1,
+                            void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_fast_base_convert(result, operand, n, from_moduli, from_count, to_moduli, to_count,
+                                                 count, stream));
+}
+
+// extension: hybrid key switch of `batch` ciphertexts at level level_size -- digits of digit_size data moduli and
+// p_size special primes, moduli = data moduli then special primes; keys uploaded with decomp = ceil(q_size /
+// digit_size) and key_modulus_size = q_size + p_size (hexl_b200_key_switch_hybrid has the definitions).  result
+// (key_component_count x level_size limbs per ciphertext) is accumulated into.
+inline void KeySwitchHybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size, uint64_t q_size,
+                            uint64_t p_size, uint64_t digit_size, uint64_t key_component_count, const uint64_t* moduli,
+                            const KeySwitchKeys& keys, uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_key_switch_hybrid(result, target, n, level_size, q_size, p_size, digit_size,
+                                                 key_component_count, moduli, keys.Handle(), batch, stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

@@ -363,6 +363,50 @@ int hexl_b200_apply_galois_key_switch_hoisted(uint64_t* results, const uint64_t*
                                               const uint64_t* galois_elts, uint64_t num_elts,
                                               const uint64_t* modswitch_factors, uint64_t batch, void* stream);
 
+/* Fast base conversion (extension; OpenFHE's ApproxSwitchCRTBasis, SEAL's BaseConverter::fast_convert_array),
+ * coefficient form: `count` polynomials; polynomial p reads from_count limbs of n words at operand + p*from_count*n
+ * (limb i under from_moduli[i]) and writes to_count limbs at result + p*to_count*n (limb e under to_moduli[e]):
+ *   result_e = [ sum_i [x_i (Q/q_i)^-1]_{q_i} [Q/q_i]_{t_e} ]_{t_e},  Q = prod from_moduli,
+ * canonical.  That is X + u Q mod t_e, X the CRT lift of the x_i in [0, Q) and 0 <= u < from_count.  A target equal to
+ * a source modulus q_i gets x_i back.  HEXL_B200_ERR_INVALID_ARG unless every pointer is non-null, n >= 1,
+ * 1 <= from_count <= 64, to_count >= 1, every modulus is in (1, 2^61), the from_moduli are pairwise coprime, and result
+ * and operand do not overlap.  Inputs must be below their modulus (checked under hexl_b200_set_debug(1)).  count = 0
+ * does nothing.  One launch per block of targets (up to 79 for from_count = 1, 3 for from_count = 64: the constants
+ * travel in the kernel parameters, so a device call can be captured into a CUDA graph).  Host buffers are staged by
+ * whole polynomials and split by polynomial over the devices of hexl_b200_set_host_devices. */
+int hexl_b200_fast_base_convert(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* from_moduli,
+                                uint64_t from_count, const uint64_t* to_moduli, uint64_t to_count, uint64_t count,
+                                void* stream);
+
+/* Hybrid key switch (extension; OpenFHE's KeySwitchHYBRID) of `batch` ciphertexts at level level_size = l.  moduli
+ * holds q_size data moduli q_0..q_{L-1} and then p_size special primes p_0..p_{K-1} (P = prod p_k), all distinct,
+ * NTT-friendly for n and below 2^61.  Digit d covers the data moduli [d a, min((d+1) a, L)), a = digit_size; the key
+ * handle holds dnum = ceil(L / a) buffers of key_component_count x (L + K) x n words in NTT form, limb i < L under q_i
+ * and limb L + k under p_k (hexl_b200_keys_upload with decomp = dnum, key_modulus_size = L + K).  Ciphertext c reads
+ * its target, l limbs in NTT form, canonical, at target + c*l*n, and accumulates into key_component_count x l limbs at
+ * result + c*key_component_count*l*n.  With S_d = [d a, min((d+1) a, l)) for d < D = ceil(l / a), Q_d = prod_{S_d} q_i
+ * and B = {q_0..q_{l-1}, p_0..p_{K-1}}:
+ *   a_i        = INTT_{q_i}(t_i)
+ *   D_{d,m}    = NTT_m([ sum_{i in S_d} [a_i (Q_d/q_i)^-1]_{q_i} [Q_d/q_i]_m ]_m)     mod-up, every m in B
+ *   prod_{m,k} = sum_{d<D} D_{d,m} keys[d][k][slot(m)] mod m,  slot(q_i) = i, slot(p_j) = L + j
+ *   x_j        = INTT_{p_j}(prod_{p_j,k}),  z_j = [(x_j + floor(P/2)) (P/p_j)^-1]_{p_j}
+ *   c_i        = [ sum_j z_j [P/p_j]_{q_i} - floor(P/2) ]_{q_i}                       mod-down, rounded
+ *   result_{k,i} += (prod_{q_i,k} - NTT_{q_i}(c_i)) P^-1 mod q_i, canonical.
+ * With digit_size = 1 and p_size = 1 this is bit for bit hexl_b200_key_switch_resident with decomp = l,
+ * key_modulus_size = L + 1 and modswitch factors p^-1 mod q_i.  The library computes every constant itself.
+ * HEXL_B200_ERR_INVALID_ARG for a null pointer, n not a power of two in [2, 2^20], level_size outside [1, q_size],
+ * digit_size or p_size outside [1, 64], key_component_count = 0, a modulus that is not NTT-friendly, is >= 2^61 or
+ * repeats, a handle of another shape or sharded by modulus, and result overlapping target.  batch = 0 does nothing.
+ * Inputs are checked below their modulus under hexl_b200_set_debug(1).  On the device, per ciphertext: one inverse
+ * transform of the target; per round of at most 64 moduli of B (and ~256 MiB of scratch), one base-conversion launch
+ * per digit and block of targets, one forward transform and the multiply-accumulates; then one inverse transform of
+ * the special limbs and, per block of 64 data moduli, the rounding base conversion, one forward transform and the
+ * finish step.  Device calls capture into a CUDA graph once the transforms are warm.  Host buffers are pipelined and
+ * split by ciphertext over the devices holding the keys, as for hexl_b200_key_switch_resident. */
+int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
+                                uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
+                                const uint64_t* moduli, const hexl_b200_keys* keys, uint64_t batch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
