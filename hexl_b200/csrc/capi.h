@@ -183,7 +183,7 @@ int run_on_device(const PtrInfo& pi, void* stream, Run&& run) {
 int host_devices(std::vector<int>* out);
 
 // ----------------------------------------------------------- host-pointer staging
-// One staging context per device: kSlots rotating {stream, device buffers}.
+// One staging context per device: kSlots rotating {stream, device buffers}, used only through stage_items.
 constexpr int kSlots = 3;
 constexpr size_t kChunkBytes = 32u << 20;  // per buffer per slot
 
@@ -211,78 +211,87 @@ struct StageCtx {
 };
 
 StageCtx* stage_for(int dev);
-int sync_stage(int dev);
+int sync_stage(int dev);  // waits for every slot stream of dev
 
-// A host-pointer job: `total` elements, processed in chunks that are multiples
-// of `unit` elements.  a is always present; b optional; result may alias a or b.
-// launch(dev_result, dev_a, dev_b, off, elems, stream) enqueues the kernel(s) for the
-// elements [off, off + elems) of the whole job (`base` = offset of this device's block);
-// it returns a cudaError_t, or an int error code whose message it has already set.
-// unit_out (non-zero): only the first unit_out elements of every unit are copied back.
-template <class Launch>
-int run_host_on_device(int dev, u64* result, const u64* a, const u64* b, u64 total, u64 unit,
-                       Launch&& launch, bool wait, u64 base = 0, u64 unit_out = 0) {
-  DeviceGuard g;
-  if (int rc = g.enter(dev)) return rc;
-  StageCtx* st = stage_for(dev);
-  std::lock_guard<std::mutex> lk(st->mu);
-  if (int rc = st->init()) return rc;
-  u64 chunk = (kChunkBytes / sizeof(u64)) / unit * unit;
-  if (chunk == 0) chunk = unit;
-  int slot = 0;
-  for (u64 off = 0; off < total; off += chunk, slot = (slot + 1) % kSlots) {
-    const u64 elems = (total - off < chunk) ? total - off : chunk;
-    const size_t bytes = elems * sizeof(u64);
-    if (int rc = st->reserve(slot, 0, bytes)) return rc;
-    if (b)
-      if (int rc = st->reserve(slot, 1, bytes)) return rc;
-    cudaStream_t s = st->stream[slot];
-    CU(cudaMemcpyAsync(st->buf[slot][0], a + off, bytes, cudaMemcpyHostToDevice, s));
-    if (b) CU(cudaMemcpyAsync(st->buf[slot][1], b + off, bytes, cudaMemcpyHostToDevice, s));
-    const auto e = launch(st->buf[slot][0], st->buf[slot][0], b ? st->buf[slot][1] : nullptr, base + off, elems, s);
-    if constexpr (std::is_same_v<std::decay_t<decltype(e)>, int>) {
-      if (e) return e;
-    } else if (e != cudaSuccess) {
-      return cuda_fail(e, "kernel launch");
-    }
-    if (unit_out && unit_out < unit)
-      CU(cudaMemcpy2DAsync(result + off, unit * sizeof(u64), st->buf[slot][0], unit * sizeof(u64),
-                           unit_out * sizeof(u64), elems / unit, cudaMemcpyDeviceToHost, s));
-    else
-      CU(cudaMemcpyAsync(result + off, st->buf[slot][0], bytes, cudaMemcpyDeviceToHost, s));
+// Slot i of a device's staging context, as a step of stage_items sees it
+struct StageSlot {
+  StageCtx* st;
+  int i;
+  cudaStream_t stream() const { return st->stream[i]; }
+  u64* buf(int which) const { return st->buf[i][which]; }
+  int reserve(int which, size_t bytes) const { return st->reserve(i, which, bytes); }
+};
+
+// The one staging loop of the host-pointer calls.  Items [0, items) are split over devs by contiguous blocks (no
+// inter-GPU traffic): device d of nd = min(|devs|, items) takes [items d / nd, items (d + 1) / nd), the rule
+// hexl_b200/sharding.py states.  On each device, with it current and its staging lock held, prepare(dev, lo, hi, stage)
+// readies what its block needs and returns an error code or stage(step), which runs step(slot, first, count) for
+// chunks of at most per_chunk items on the rotating slots, so the copies of one chunk overlap the kernels of its
+// neighbours.  Returns the first error, always after waiting for every slot stream of every device of the split:
+// copies into the caller's buffers may still be queued when a step fails.
+template <class Prepare>
+int stage_items(const std::vector<int>& devs, u64 items, u64 per_chunk, Prepare&& prepare) {
+  const u64 nd = std::min<u64>(devs.size(), items);
+  int rc = 0;
+  for (u64 d = 0; d < nd && !rc; ++d) {
+    const u64 lo = items * d / nd, hi = items * (d + 1) / nd;
+    DeviceGuard g;
+    if ((rc = g.enter(devs[d]))) break;
+    StageCtx* st = stage_for(devs[d]);
+    std::lock_guard<std::mutex> lk(st->mu);
+    if ((rc = st->init())) break;
+    rc = prepare(devs[d], lo, hi, [&](auto&& step) {
+      int slot = 0;
+      for (u64 first = lo; first < hi; first += per_chunk, slot = (slot + 1) % kSlots)
+        if (int e = step(StageSlot{st, slot}, first, std::min(per_chunk, hi - first))) return e;
+      return 0;
+    });
   }
-  if (wait)
-    for (int s = 0; s < kSlots; ++s) CU(cudaStreamSynchronize(st->stream[s]));
-  return 0;
+  for (u64 d = 0; d < nd; ++d) {
+    const int rc2 = sync_stage(devs[d]);
+    if (!rc) rc = rc2;
+  }
+  return rc;
 }
 
-// Split a host-pointer job over the host devices by contiguous blocks of whole units (no inter-GPU traffic), enqueue
-// everything, then wait.  make(dev, lo, hi, run) prepares device dev for the elements [lo, hi) of the job and returns
-// either an error code or run(launch), which stages the block through `launch` (see run_host_on_device).
+// A host-pointer job of `total` elements in whole units of `unit` elements, through stage_items: split over the host
+// devices by unit, in chunks of whole units up to kChunkBytes (or of one unit).  a is always present; b optional;
+// result may alias a or b.  make(dev, lo, hi, run) prepares device dev for the elements [lo, hi) of the job and
+// returns either an error code or run(launch).  launch(dev_result, dev_a, dev_b, off, elems, stream) enqueues the
+// kernel(s) for the elements [off, off + elems) of the whole job, staged in the slot's buffer 0 (b in buffer 1); it
+// returns a cudaError_t, or an int error code whose message it has already set.
+// unit_out (non-zero): only the first unit_out elements of every unit are copied back.
 template <class MakeLaunch>
 int run_host(u64* result, const u64* a, const u64* b, u64 total, u64 unit, MakeLaunch&& make, u64 unit_out = 0) {
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
-  if (devs.size() == 1 || total / unit < 2)
-    return make(devs[0], (u64)0, total, [&](auto&& launch) {
-      return run_host_on_device(devs[0], result, a, b, total, unit, launch, true, 0, unit_out);
+  const u64 per_chunk = std::max<u64>(1, (kChunkBytes / sizeof(u64)) / unit);
+  return stage_items(devs, total / unit, per_chunk, [&](int dev, u64 lo, u64 hi, auto&& stage) {
+    return make(dev, lo * unit, hi * unit, [&](auto&& launch) {
+      return stage([&](const StageSlot& sl, u64 first, u64 count) -> int {
+        const u64 off = first * unit, elems = count * unit;
+        const size_t bytes = elems * sizeof(u64);
+        if (int rc = sl.reserve(0, bytes)) return rc;
+        if (b)
+          if (int rc = sl.reserve(1, bytes)) return rc;
+        cudaStream_t s = sl.stream();
+        CU(cudaMemcpyAsync(sl.buf(0), a + off, bytes, cudaMemcpyHostToDevice, s));
+        if (b) CU(cudaMemcpyAsync(sl.buf(1), b + off, bytes, cudaMemcpyHostToDevice, s));
+        const auto e = launch(sl.buf(0), sl.buf(0), b ? sl.buf(1) : nullptr, off, elems, s);
+        if constexpr (std::is_same_v<std::decay_t<decltype(e)>, int>) {
+          if (e) return e;
+        } else if (e != cudaSuccess) {
+          return cuda_fail(e, "kernel launch");
+        }
+        if (unit_out && unit_out < unit)
+          CU(cudaMemcpy2DAsync(result + off, unit * sizeof(u64), sl.buf(0), unit * sizeof(u64),
+                               unit_out * sizeof(u64), count, cudaMemcpyDeviceToHost, s));
+        else
+          CU(cudaMemcpyAsync(result + off, sl.buf(0), bytes, cudaMemcpyDeviceToHost, s));
+        return 0;
+      });
     });
-  const u64 units = total / unit;
-  const u64 ndev = devs.size() < units ? devs.size() : units;
-  int rc = 0;
-  for (u64 d = 0; d < ndev && !rc; ++d) {
-    // on failure, fall through: copies already enqueued on other devices still target `result`
-    const u64 lo = units * d / ndev * unit, hi = units * (d + 1) / ndev * unit;
-    rc = make(devs[d], lo, hi, [&](auto&& launch) {
-      return run_host_on_device(devs[d], result + lo, a + lo, b ? b + lo : nullptr, hi - lo, unit, launch, false, lo,
-                                unit_out);
-    });
-  }
-  for (u64 d = 0; d < ndev; ++d) {
-    int rc2 = sync_stage(devs[d]);
-    if (!rc) rc = rc2;
-  }
-  return rc;
+  });
 }
 
 // ---------------------------------------------------------------- debug checks

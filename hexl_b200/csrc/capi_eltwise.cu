@@ -429,35 +429,28 @@ int hexl_b200_dyadic_multiply(uint64_t* result, const uint64_t* operand1, const 
     return run_on_device(pi, stream, [&] {
       return dyadic_on_device(result, operand1, operand2, n, moduli, num_moduli, (cudaStream_t)stream);
     });
-  // Host pointers: blocks of moduli travel through the rotating staging slots (the layout is
-  // [polynomial][modulus][n], so a block of moduli is a 2-D copy: 2 rows in, 3 rows out).
+  // Host pointers: blocks of moduli travel through the staging slots (stage_items) of the first host device (the
+  // layout is [polynomial][modulus][n], so a block of moduli is a 2-D copy: 2 rows in, 3 rows out).
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
-  const int cur = devs[0];
-  DeviceGuard g;
-  if (int rc = g.enter(cur)) return rc;
-  StageCtx* st = stage_for(cur);
-  std::lock_guard<std::mutex> lk(st->mu);
-  if (int rc = st->init()) return rc;
   u64 mb = std::max<u64>(1, (kChunkBytes / sizeof(u64)) / (3 * n));
   mb = std::min<u64>({mb, (u64)kParamBlock, num_moduli});
   const size_t row = (size_t)num_moduli * n * sizeof(u64);  // host pitch: one polynomial over all moduli
-  int slot = 0;
-  for (u64 m0 = 0; m0 < num_moduli; m0 += mb, slot = (slot + 1) % kSlots) {
-    const u64 cnt = std::min(mb, num_moduli - m0);
-    const size_t w = (size_t)cnt * n * sizeof(u64);
-    if (int rc = st->reserve(slot, 0, 3 * w)) return rc;
-    if (int rc = st->reserve(slot, 1, 2 * w)) return rc;
-    if (int rc = st->reserve(slot, 2, 2 * w)) return rc;
-    cudaStream_t sx = st->stream[slot];
-    u64 *dr = st->buf[slot][0], *d1 = st->buf[slot][1], *d2 = st->buf[slot][2];
-    CU(cudaMemcpy2DAsync(d1, w, operand1 + m0 * n, row, w, 2, cudaMemcpyHostToDevice, sx));
-    CU(cudaMemcpy2DAsync(d2, w, operand2 + m0 * n, row, w, 2, cudaMemcpyHostToDevice, sx));
-    if (int rc = dyadic_on_device(dr, d1, d2, n, moduli + m0, cnt, sx)) return rc;
-    CU(cudaMemcpy2DAsync(result + m0 * n, row, dr, w, w, 3, cudaMemcpyDeviceToHost, sx));
-  }
-  for (int k = 0; k < kSlots; ++k) CU(cudaStreamSynchronize(st->stream[k]));
-  return 0;
+  return stage_items({devs[0]}, num_moduli, mb, [&](int, u64, u64, auto&& stage) {
+    return stage([&](const StageSlot& sl, u64 m0, u64 cnt) -> int {
+      const size_t w = (size_t)cnt * n * sizeof(u64);
+      if (int rc = sl.reserve(0, 3 * w)) return rc;
+      if (int rc = sl.reserve(1, 2 * w)) return rc;
+      if (int rc = sl.reserve(2, 2 * w)) return rc;
+      cudaStream_t sx = sl.stream();
+      u64 *dr = sl.buf(0), *d1 = sl.buf(1), *d2 = sl.buf(2);
+      CU(cudaMemcpy2DAsync(d1, w, operand1 + m0 * n, row, w, 2, cudaMemcpyHostToDevice, sx));
+      CU(cudaMemcpy2DAsync(d2, w, operand2 + m0 * n, row, w, 2, cudaMemcpyHostToDevice, sx));
+      if (int rc = dyadic_on_device(dr, d1, d2, n, moduli + m0, cnt, sx)) return rc;
+      CU(cudaMemcpy2DAsync(result + m0 * n, row, dr, w, w, 3, cudaMemcpyDeviceToHost, sx));
+      return 0;
+    });
+  });
 }
 
 }  // extern "C"

@@ -128,46 +128,29 @@ static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t
   return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
 }
 
-// Host buffers of the base conversion: whole polynomials through the staging slots, split by polynomial over the host
-// devices; a slot holds one chunk of input polynomials and one of results.
+// Host buffers of the base conversion: chunks of whole polynomials through stage_items, split by polynomial over the
+// host devices; a slot holds a chunk of input polynomials in buffer 1 and their results in buffer 0.
 static int base_convert_host(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* from,
                              uint64_t from_count, const uint64_t* to, uint64_t to_count, uint64_t count) {
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
   const uint64_t in_words = from_count * n, out_words = to_count * n;
   const uint64_t chunk = std::max<uint64_t>(1, (kChunkBytes / 8) / std::max(in_words, out_words));
-  const uint64_t ndev = std::min<uint64_t>(devs.size(), count);
-  int rc = 0;
-  for (uint64_t di = 0; di < ndev && !rc; ++di) {
-    const uint64_t lo = count * di / ndev, hi = count * (di + 1) / ndev;
-    DeviceGuard g;
-    if ((rc = g.enter(devs[di]))) break;
-    StageCtx* st = stage_for(devs[di]);
-    std::lock_guard<std::mutex> lk(st->mu);
-    if ((rc = st->init())) break;
-    int slot = 0;
-    for (uint64_t p0 = lo; p0 < hi && !rc; p0 += chunk, slot = (slot + 1) % kSlots) {
-      const uint64_t cnt = std::min(chunk, hi - p0);
-      if ((rc = st->reserve(slot, 0, cnt * out_words * 8)) || (rc = st->reserve(slot, 1, cnt * in_words * 8))) break;
-      const cudaStream_t sx = st->stream[slot];
-      cudaError_t e = cudaMemcpyAsync(st->buf[slot][1], operand + p0 * in_words, cnt * in_words * 8,
-                                      cudaMemcpyHostToDevice, sx);
-      if (e != cudaSuccess) {
-        rc = cuda_fail(e, "FastBaseConvert H2D");
-        break;
-      }
-      if ((rc = base_convert_on_device(st->buf[slot][0], n, out_words, st->buf[slot][1], n, in_words, n, cnt, from,
-                                       from_count, to, to_count, false, sx)))
-        break;
-      e = cudaMemcpyAsync(result + p0 * out_words, st->buf[slot][0], cnt * out_words * 8, cudaMemcpyDeviceToHost, sx);
-      if (e != cudaSuccess) rc = cuda_fail(e, "FastBaseConvert D2H");
-    }
-  }
-  for (uint64_t di = 0; di < ndev; ++di) {  // always drain: host buffers are in flight
-    const int rc2 = sync_stage(devs[di]);
-    if (!rc) rc = rc2;
-  }
-  return rc;
+  return stage_items(devs, count, chunk, [&](int, u64, u64, auto&& stage) {
+    return stage([&](const StageSlot& sl, u64 p0, u64 cnt) -> int {
+      if (int rc = sl.reserve(0, cnt * out_words * 8)) return rc;
+      if (int rc = sl.reserve(1, cnt * in_words * 8)) return rc;
+      const cudaStream_t sx = sl.stream();
+      cudaError_t e =
+          cudaMemcpyAsync(sl.buf(1), operand + p0 * in_words, cnt * in_words * 8, cudaMemcpyHostToDevice, sx);
+      if (e != cudaSuccess) return cuda_fail(e, "FastBaseConvert H2D");
+      if (int rc = base_convert_on_device(sl.buf(0), n, out_words, sl.buf(1), n, in_words, n, cnt, from, from_count,
+                                          to, to_count, false, sx))
+        return rc;
+      e = cudaMemcpyAsync(result + p0 * out_words, sl.buf(0), cnt * out_words * 8, cudaMemcpyDeviceToHost, sx);
+      return e == cudaSuccess ? 0 : cuda_fail(e, "FastBaseConvert D2H");
+    });
+  });
 }
 
 }  // namespace hexl_b200

@@ -191,11 +191,11 @@ uint64_t keys_on_device(const hexl_b200_keys* const* keys, uint64_t count, int d
   return count;
 }
 
-// One or more key switches on HOST buffers against keys already on the devices.  Ciphertext c's result block
-// (res_words words at result + c * res_words) crosses PCIe out, and in as well when result_in; in_words words of `in`
-// (in + c * in_words; nothing when in is null) go into the slot's second buffer, which holds buf_words words.  Each
-// ciphertext runs on one of the rotating staging streams, so the copies of one ciphertext overlap the kernels of its
-// neighbours; with host devices set the batch is split into contiguous blocks over the devices holding every key.
+// One or more key switches on HOST buffers against keys already on the devices, one ciphertext per staging chunk
+// (stage_items), split by ciphertext over the host devices holding every key.  Ciphertext c's result block
+// (res_words words at result + c * res_words, in the slot's buffer 0) crosses PCIe out, and in as well when
+// result_in; in_words words of `in` (in + c * in_words; nothing when in is null) go into the slot's buffer 1, which
+// holds buf_words words.
 int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, const uint64_t* in,
                           uint64_t in_words, uint64_t buf_words, const hexl_b200_keys* const* keys,
                           uint64_t num_keys, uint64_t batch, const HostSwitch& run) {
@@ -206,41 +206,23 @@ int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, 
   for (int d : devs)
     if (keys_on_device(keys, num_keys, d, &dk) == num_keys) use.push_back(d);
   if (use.empty()) return fail(HEXL_B200_ERR_INVALID_ARG, "the key handle holds no copy on the device(s) used for host calls");
-  if (use.size() > batch) use.resize(batch);
-  int rc = 0;
-  for (size_t di = 0; di < use.size() && !rc; ++di) {
-    const int dev = use[di];
-    const u64 c_lo = batch * di / use.size(), c_hi = batch * (di + 1) / use.size();
-    DeviceGuard g;
-    if ((rc = g.enter(dev))) break;
-    StageCtx* st = stage_for(dev);
-    std::lock_guard<std::mutex> lk(st->mu);
-    if ((rc = st->init())) break;
+  return stage_items(use, batch, 1, [&](int dev, u64, u64, auto&& stage) {
     keys_on_device(keys, num_keys, dev, &dk);
-    int slot = 0;
-    for (u64 c = c_lo; c < c_hi && !rc; ++c, slot = (slot + 1) % kSlots) {
-      if ((rc = st->reserve(slot, 0, res_words * 8))) break;
-      if ((rc = st->reserve(slot, 1, buf_words * 8))) break;
-      cudaStream_t sx = st->stream[slot];
-      u64 *d_res = st->buf[slot][0], *d_in = st->buf[slot][1];
+    return stage([&](const StageSlot& sl, u64 c, u64) -> int {
+      if (int rc = sl.reserve(0, res_words * 8)) return rc;
+      if (int rc = sl.reserve(1, buf_words * 8)) return rc;
+      cudaStream_t sx = sl.stream();
+      u64 *d_res = sl.buf(0), *d_in = sl.buf(1);
       cudaError_t e = cudaSuccess;
       if (in) e = cudaMemcpyAsync(d_in, in + c * in_words, in_words * 8, cudaMemcpyHostToDevice, sx);
       if (e == cudaSuccess && result_in)
         e = cudaMemcpyAsync(d_res, result + c * res_words, res_words * 8, cudaMemcpyHostToDevice, sx);
-      if (e != cudaSuccess) {
-        rc = cuda_fail(e, "KeySwitch H2D");
-        break;
-      }
-      if ((rc = run(dev, d_res, d_in, dk.data(), sx))) break;
+      if (e != cudaSuccess) return cuda_fail(e, "KeySwitch H2D");
+      if (int rc = run(dev, d_res, d_in, dk.data(), sx)) return rc;
       e = cudaMemcpyAsync(result + c * res_words, d_res, res_words * 8, cudaMemcpyDeviceToHost, sx);
-      if (e != cudaSuccess) rc = cuda_fail(e, "KeySwitch D2H");
-    }
-  }
-  for (int dev : use) {
-    int rc2 = sync_stage(dev);
-    if (!rc) rc = rc2;
-  }
-  return rc;
+      return e == cudaSuccess ? 0 : cuda_fail(e, "KeySwitch D2H");
+    });
+  });
 }
 
 int key_switch_check(const void* result, const void* t_target, uint64_t n, uint64_t decomp,

@@ -3,7 +3,7 @@
 The hot path has no data dependence between units (SURVEY.md 8(e)), so scaling
 is a contiguous block split with no data-path collective.  The same rule is
 used by the C ABI for host-pointer calls over several devices
-(hexl_b200_set_host_devices, csrc/capi.h run_host) and by bench.py's ranks.
+(hexl_b200_set_host_devices, csrc/capi.h stage_items) and by bench.py's ranks.
 """
 from __future__ import annotations
 

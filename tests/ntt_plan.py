@@ -41,8 +41,8 @@ def batches(log_n):
 
 
 def chunk_polys(log_n):
-    """polynomials per staging chunk of a host-pointer call (capi.h:run_host_on_device): whole polynomials up to
-    kChunkBytes"""
+    """polynomials per staging chunk of a host-pointer call (capi.h:run_host, staged by stage_items): whole
+    polynomials up to kChunkBytes"""
     return max(1, CHUNK_WORDS >> log_n)
 
 

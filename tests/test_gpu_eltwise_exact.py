@@ -201,7 +201,9 @@ def test_add_sub_mod_multi(hb, op, per_mod):
 
 # ------------------------------------------------------------------------------------------------ DyadicMultiply
 DYADIC_LISTS = {"witnesses": [*W, ee.prime_below(1 << 62), ee.prime_below(1 << 60), ee.prime_below(1 << 29)],
-                "below_2_61": [(1 << 61) - 1, ee.prime_above(1 << 60), ee.prime_below(1 << 30), ee.COMPOSITE_MODULI[1]]}
+                "below_2_61": [(1 << 61) - 1, ee.prime_above(1 << 60), ee.prime_below(1 << 30), ee.COMPOSITE_MODULI[1]],
+                # more moduli than one parameter block: kernel launches and host staging chunks of 64 and 6 moduli
+                "seventy": [ee.prime_below((1 << 62) - (i << 55)) for i in range(70)]}
 
 
 @pytest.mark.parametrize("n", [4096, 4099])

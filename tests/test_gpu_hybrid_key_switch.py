@@ -184,27 +184,31 @@ def _convert_model(port, x, n, src, dst, count):
     return np.concatenate([hx.fast_base_convert(port, x[p * per:(p + 1) * per], n, src, dst) for p in range(count)])
 
 
-@pytest.mark.parametrize("n", [1, 3, 1 << 10])
-@pytest.mark.parametrize("shape", ["from64_worst", "to70", "small"])
+@pytest.mark.parametrize("shape, n", [(shape, n) for shape in ("from64_worst", "to70", "small")
+                                      for n in (1, 3, 1 << 10)] + [("one_per_slot", 1 << 16)])
 def test_fast_base_convert(hb, port, shape, n):
+    """one_per_slot: a polynomial's result (33 x 2^16 words) is more than half of a 32 MiB staging chunk, so each
+    host chunk is one polynomial, and 4 of them wrap around the 3 staging slots"""
+    count = 4 if shape == "one_per_slot" else 3
     if shape == "from64_worst":
         mods = [int(q) for q in port.generate_primes(67, 60, False, 2)]
         src, dst = mods[:64], mods[64:]
-        x = np.concatenate([np.full(n, q - 1, dtype=U64) for _ in range(3) for q in src])
+        x = np.concatenate([np.full(n, q - 1, dtype=U64) for _ in range(count) for q in src])
     else:
-        mods = [int(q) for q in port.generate_primes(73 if shape == "to70" else 5, 50, True, 2)]
-        src, dst = (mods[:3], mods[3:]) if shape == "to70" else (mods[:2], mods[2:])
-        x = np.concatenate([uniform_below(11 * p + i, n, q) for p in range(3) for i, q in enumerate(src)])
-    exp = _convert_model(port, x, n, src, dst, 3)
+        sizes = {"to70": (3, 70), "small": (2, 3), "one_per_slot": (2, 33)}[shape]
+        mods = [int(q) for q in port.generate_primes(sum(sizes), 50, True, 2)]
+        src, dst = mods[:sizes[0]], mods[sizes[0]:]
+        x = np.concatenate([uniform_below(11 * p + i, n, q) for p in range(count) for i, q in enumerate(src)])
+    exp = _convert_model(port, x, n, src, dst, count)
     out = torch.full((exp.size,), -1, dtype=torch.int64, device="cuda")
-    hb.FastBaseConvert(out, dev(x), n, src, dst, 3)
+    hb.FastBaseConvert(out, dev(x), n, src, dst, count)
     torch.cuda.synchronize()
     _check(host(out), exp, f"{shape} n={n} device")
     # an unaligned view (8-byte offset) runs the word-at-a-time kernel
     buf = torch.full((exp.size + 2,), -1, dtype=torch.int64, device="cuda")
     xin = torch.zeros(x.size + 1, dtype=torch.int64, device="cuda")
     xin[1:] = dev(x)
-    hb.FastBaseConvert(buf[1:1 + exp.size], xin[1:], n, src, dst, 3)
+    hb.FastBaseConvert(buf[1:1 + exp.size], xin[1:], n, src, dst, count)
     torch.cuda.synchronize()
     _check(host(buf[1:1 + exp.size]), exp, f"{shape} n={n} offset view")
     assert int(buf[0]) == -1 and int(buf[-1]) == -1, "a word next to the result was written"
@@ -212,7 +216,7 @@ def test_fast_base_convert(hb, port, shape, n):
         try:
             hb.set_host_devices(devices)
             got = np.full(exp.size, SENTINEL, dtype=U64)
-            hb.FastBaseConvert(got, x.copy(), n, src, dst, 3)
+            hb.FastBaseConvert(got, x.copy(), n, src, dst, count)
         finally:
             hb.set_host_devices([])
         _check(got, exp, f"{shape} n={n} host {devices}")

@@ -277,7 +277,8 @@ def test_composite_host_paths_span_many_staging_chunks(hb, checker):
 
 def test_key_switch_resident_keys_and_batches(hb, checker):
     """hexl_b200_keys_upload + hexl_b200_key_switch_resident: several ciphertexts per call against keys uploaded
-    once, host buffers (pipelined over the staging streams) and device buffers, against the reference per ciphertext."""
+    once, host buffers (pipelined over the staging streams) and device buffers, against the reference per ciphertext;
+    and refusals, one of them part-way through a host batch."""
     n, decomp, batch = 1 << 13, 7, 5
     kms, rns, kcc, mods, _, keys, _, modswitch = _c5_case(hb, n, decomp, 50)
     t_all = np.concatenate([np.concatenate([uniform_below(900 * c + j, n, mods[j]) for j in range(decomp)])
@@ -300,6 +301,21 @@ def test_key_switch_resident_keys_and_batches(hb, checker):
     assert (got == exp[:res_sz]).all()
     with pytest.raises(hb.HexlB200Error):                                     # shape mismatch is refused
         hb.KeySwitchResident(got, t_all[:t_sz], n // 2, decomp, kms, rns, kcc, mods, handle2, modswitch)
+    # a digit modulus >= 2^61 is refused inside the switch of the first ciphertext, after its copies are queued, on a
+    # batch split over two blocks: result stays as it was, and the next call is right
+    try:
+        hb.set_host_devices([0, 0])
+        h_split = hb.KeySwitchKeys(keys, n, decomp, kms, kcc)
+        got = r_all.copy()
+        with pytest.raises(hb.HexlB200Error) as e:
+            hb.KeySwitchResident(got, t_all, n, decomp, kms, rns, kcc, [(1 << 61) + 1] + list(mods[1:]), h_split,
+                                 modswitch, batch)
+        assert e.value.code == -1 and "KeySwitch: Require moduli < 2^61 (slot 0)" in str(e.value), e.value
+        assert (got == r_all).all(), "a refused call wrote"
+        hb.KeySwitchResident(got, t_all, n, decomp, kms, rns, kcc, mods, h_split, modswitch, batch)
+        assert (got == exp).all()
+    finally:
+        hb.set_host_devices([])
     ndev = hb.device_count()
     if ndev >= 2:                                                             # keys on every device, batch split
         try:

@@ -52,7 +52,7 @@ def test_two_ranks_share_units_and_agree_on_time(tmp_path, total_units):
 
 def test_split_units_matches_c_abi_rule():
     from hexl_b200.sharding import split_units
-    # same arithmetic as csrc/capi.h run_host: units*d/ndev
+    # same arithmetic as csrc/capi.h stage_items: items*d/ndev
     assert split_units(30, 8) == [(0, 3), (3, 7), (7, 11), (11, 15), (15, 18), (18, 22), (22, 26), (26, 30)]
     assert sorted(hi - lo for lo, hi in split_units(30, 8)) == [3, 3, 4, 4, 4, 4, 4, 4]
     for total in (1, 5, 8192):
