@@ -113,6 +113,7 @@ constexpr int kFastBound = 8;  // FAST inverse: every value is < 8q at a pass bo
 struct Mod {
   u64 q, two_q, four_q, mu;  // mu = floor(2^64 / q)
   unsigned n0, n1;           // low / high word of 2^64 - q
+  unsigned zero;             // 0, unknown to the compiler (add_alu)
 };
 
 __device__ __forceinline__ unsigned lo32(u64 x) { return (unsigned)x; }
@@ -145,6 +146,13 @@ __device__ __forceinline__ unsigned mad_lo(unsigned a, unsigned b, unsigned c) {
   asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c));
   return r;
 }
+
+// a + b with the carry into the high word on the ALU pipe.  ptxas puts the high half of a two-operand 64-bit add on
+// the multiplier pipe (IMAD.X) whenever it judges the ALU busier, which in these kernels it always is by that
+// measure although the multiplier is the bound.  With a third operand -- m.zero, 0 at run time but a kernel parameter
+// the compiler cannot see through -- the low word produces two carries and the high word becomes a three-input
+// IADD3.X, which has no IMAD form.  (Checked in SASS: tests/test_pipe_budget.py.)
+__device__ __forceinline__ u64 add_alu(u64 a, u64 b, const Mod& m) { return a + b + m.zero; }
 
 __device__ __forceinline__ Twiddle ld_tw(const Twiddle* p) {
   const ulonglong2 v = __ldg(reinterpret_cast<const ulonglong2*>(p));
@@ -222,12 +230,17 @@ __device__ __forceinline__ u64 barrett_lazy_bigq(u64 x, const Mod& m) {
 }
 // any 64-bit value -> [0,3q) for q >= 2^32 with one wide product less: Q = hi32(x1*mu) is floor(x*mu/2^64) or
 // up to two less.  Enough wherever the result only has to drop below a lazy bound (FAST inverse fix-ups).
+// x is added with a three-input IADD3.X rather than as the accumulator of the wide product: the coefficient arrays
+// do not keep a value's two words in an aligned register pair, and ptxas then splits the wide mad into a product
+// plus a 64-bit add whose high half lands on IMAD.X.
 __device__ __forceinline__ u64 barrett_lazy3_bigq(u64 x, const Mod& m) {
-  unsigned x0, x1, t0, t1;
+  unsigned x0, x1, p0, p1;
   split(x, x0, x1);
   const unsigned Q = hi32(mul_wide(x1, lo32(m.mu)));
-  split(mad_wide(Q, m.n0, x), t0, t1);
-  return join(t0, mad_lo(Q, m.n1, t1));
+  split(mul_wide(Q, m.n0), p0, p1);
+  const unsigned qn1 = Q * m.n1;
+  const u64 s = x + join(p0, p1);
+  return join(lo32(s), hi32(s) + qn1);
 }
 
 // any 64-bit value -> [0, q) (Barrett with floor(2^64/q), then one conditional subtraction; q < 2^63)
@@ -270,13 +283,13 @@ __device__ __forceinline__ void fwd_bfly(u64& X, u64& Y, const TW& w, const Mod&
   if (MODE == kFast) {
     const u64 T = mul_tw<kFast>(Y, w, m);  // [0,4q)
     Y = X + m.four_q - T;
-    X = X + T;
+    X = add_alu(X, T, m);
   } else if (MODE == kWide) {
     // (the 64-bit compare form here: with csub_s ptxas moves the high-word adds from IMAD.X to the ALU pipe, which
     // this mode loads as much as the multiplier)
     const u64 tx = csub(X, m.four_q);      // [0,8q) -> [0,4q)
     const u64 T = mul_tw<kWide>(Y, w, m);  // [0,4q)
-    X = tx + T;
+    X = add_alu(tx, T, m);
     Y = tx + m.four_q - T;
   } else {
     const u64 tx = csub_s(X, m.two_q);
@@ -291,10 +304,10 @@ template <int MODE, typename TW>
 __device__ __forceinline__ void inv_bfly(u64& X, u64& Y, const TW& w, const Mod& m, u64 cq) {
   if (MODE == kFast) {
     const u64 d = X + cq - Y;
-    X = X + Y;
+    X = add_alu(X, Y, m);
     Y = mul_tw<kFast>(d, w, m);  // [0,4q)
   } else if (MODE == kWide) {
-    const u64 s = X + Y;  // inputs in [0,4q)
+    const u64 s = add_alu(X, Y, m);  // inputs in [0,4q)
     const u64 d = X + m.four_q - Y;
     X = csub_s(s, m.four_q);
     Y = mul_tw<kWide>(d, w, m);  // [0,4q)
@@ -308,26 +321,34 @@ __device__ __forceinline__ void inv_bfly(u64& X, u64& Y, const TW& w, const Mod&
 
 // Root stage of the inverse with N^-1 folded in (ntt-radix-2.cpp:484-509).  The
 // Shoup multiply accepts any 64-bit input, so the sum needs no reduction first.
+// FAST / WIDE: the three-product quotient, products in [0,4q) (4q < 2^63 there);
+// GENERIC keeps the exact quotient, [0,2q), since 4q may not fit 64 bits.
+template <int MODE>
 __device__ __forceinline__ void inv_bfly_last(u64& X, u64& Y, const Twiddle inv_n, const Twiddle inv_n_w,
                                               const Mod& m, u64 cq) {
-  const u64 s = X + Y;
+  const u64 s = add_alu(X, Y, m);
   const u64 d = X + cq - Y;
-  X = mul_tw_exact(s, inv_n, m);    // [0,2q)
-  Y = mul_tw_exact(d, inv_n_w, m);  // [0,2q)
+  if (MODE == kFast || MODE == kWide) {
+    X = mul_tw<MODE>(s, inv_n, m);    // [0,4q)
+    Y = mul_tw<MODE>(d, inv_n_w, m);  // [0,4q)
+  } else {
+    X = mul_tw_exact(s, inv_n, m);    // [0,2q)
+    Y = mul_tw_exact(d, inv_n_w, m);  // [0,2q)
+  }
 }
 
-// forward output: GENERIC [0,4q) / FAST anything  ->  [0,q) (out_mf 1) or < 4q (out_mf 4)
+// forward output: GENERIC [0,4q) / WIDE [0,8q) / FAST anything  ->  [0,q) (out_mf 1) or < 4q (out_mf 4)
 template <int MODE>
 __device__ __forceinline__ u64 fwd_out(u64 v, const Mod& m, int out_mf) {
-  if (MODE == kFast) {
-    v = barrett_lazy_bigq(v, m);  // [0,2q), fine for out_mf == 4 as well
-    return out_mf == 1 ? csub_s(v, m.q) : v;
-  }
-  if (MODE == kWide) v = csub_s(v, m.four_q);  // [0,8q) -> [0,4q)
+  if (MODE == kFast) v = barrett_lazy3_bigq(v, m);  // [0,3q)
+  if (MODE == kWide) v = csub_s(v, m.four_q);       // [0,8q) -> [0,4q)
   return out_mf == 1 ? csub_s(csub_s(v, m.two_q), m.q) : v;
 }
-// inverse output after the folded root stage: [0,2q) -> [0,q) when out_mf == 1
+// inverse output after the folded root stage: FAST / WIDE [0,4q), GENERIC [0,2q)  ->  [0,2q) (out_mf 2) or
+// [0,q) (out_mf 1)
+template <int MODE>
 __device__ __forceinline__ u64 inv_out(u64 v, const Mod& m, int out_mf) {
+  if (MODE == kFast || MODE == kWide) v = csub_s(v, m.two_q);
   return out_mf == 1 ? csub_s(v, m.q) : v;
 }
 
@@ -354,6 +375,7 @@ __device__ __forceinline__ void inv_bfly(unsigned& X, unsigned& Y, const TW& w, 
   X = csub32(s, two_q);
   Y = mul_tw32(d, w, m);
 }
+template <int MODE>
 __device__ __forceinline__ void inv_bfly_last(unsigned& X, unsigned& Y, const Twiddle32 inv_n,
                                               const Twiddle32 inv_n_w, const Mod& m, unsigned) {
   const unsigned s = X + Y;
@@ -365,6 +387,7 @@ template <int MODE>
 __device__ __forceinline__ unsigned fwd_out(unsigned v, const Mod& m, int out_mf) {
   return out_mf == 1 ? csub32(csub32(v, lo32(m.two_q)), lo32(m.q)) : v;
 }
+template <int MODE>
 __device__ __forceinline__ unsigned inv_out(unsigned v, const Mod& m, int out_mf) {
   return out_mf == 1 ? csub32(v, lo32(m.q)) : v;
 }
@@ -389,10 +412,19 @@ __device__ __forceinline__ typename Ar<MODE>::E stage_cq(int step, const Mod& m)
   return (typename Ar<MODE>::E)m.two_q;
 }
 
+// Brings every slot of such a pass back below kFastBound*q: a Barrett reduction (< 3q) where the bound exceeds
+// kFastFixupCsub*q, else one conditional subtraction per halving (16q -> 8q, 32q -> 16q -> 8q).
+constexpr int kFastFixupCsub = 32;
 template <int K, int NSLOTS, int E = 0>
 __device__ __forceinline__ void inv_pass_fixup(u64* v, const Mod& m) {
   if constexpr (E < NSLOTS) {
-    if constexpr (inv_slot_bound(K, E & ((1 << K) - 1)) > kFastBound) v[E] = barrett_lazy3_bigq(v[E], m);  // < 3q <= 8q
+    constexpr int bound = inv_slot_bound(K, E & ((1 << K) - 1));
+    if constexpr (bound > kFastFixupCsub) {
+      v[E] = barrett_lazy3_bigq(v[E], m);
+    } else {
+      if constexpr (bound > 2 * kFastBound) v[E] = csub_s(v[E], m.four_q << 2);
+      if constexpr (bound > kFastBound) v[E] = csub_s(v[E], m.four_q << 1);
+    }
     inv_pass_fixup<K, NSLOTS, E + 1>(v, m);
   }
 }
@@ -506,7 +538,7 @@ __device__ __forceinline__ void reg_stages(typename Ar<MODE>::E (&v)[16], unsign
         // root stage of the whole transform: one group, N^-1 folded in
         static_for<0, (1 << eb)>([&](auto L) {
           constexpr int l = L;
-          inv_bfly_last(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
+          inv_bfly_last<MODE>(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
         });
       } else {
         groups();
@@ -621,24 +653,29 @@ __device__ __forceinline__ void st_coef(u64* p, u64 v) {
     __stcs(p, v);
 }
 
-// coefficient idx of a row whose storage is global u64 (kStream / kViaL2) or a shared-memory row of E
+// coefficient u0 + off of a row whose storage is global u64 (kStream / kViaL2) or a shared-memory row of E.  The
+// register slots of a thread are one index u0 = reg_index(u, 0) plus a compile-time offset (slot << LB): in global
+// memory the offset is added to the pointer, so the 16 accesses share one 64-bit address and take the offsets as
+// immediates instead of widening each 32-bit index (an IADD3 + IMAD.X + LEA pair per access).
 template <int POLICY, typename E>
-__device__ __forceinline__ E ld_row(const void* base, unsigned idx) {
+__device__ __forceinline__ E ld_row(const void* base, unsigned u0, unsigned off) {
+  const unsigned idx = u0 + off;
   if constexpr (POLICY == kSmemRow)
     return static_cast<const E*>(base)[idx];
   else if constexpr (POLICY == kSmemRowPad)
     return static_cast<const E*>(base)[idx + (idx >> 4)];
   else
-    return (E)ld_coef<POLICY>(static_cast<const u64*>(base) + idx);
+    return (E)ld_coef<POLICY>(static_cast<const u64*>(base) + u0 + off);
 }
 template <int POLICY, typename E>
-__device__ __forceinline__ void st_row(void* base, unsigned idx, E v) {
+__device__ __forceinline__ void st_row(void* base, unsigned u0, unsigned off, E v) {
+  const unsigned idx = u0 + off;
   if constexpr (POLICY == kSmemRow)
     static_cast<E*>(base)[idx] = v;
   else if constexpr (POLICY == kSmemRowPad)
     static_cast<E*>(base)[idx + (idx >> 4)] = v;
   else
-    st_coef<POLICY>(static_cast<u64*>(base) + idx, v);
+    st_coef<POLICY>(static_cast<u64*>(base) + u0 + off, v);
 }
 
 // Extra destinations of a transform's final stores (see NttMulti::mirror): buffer p receives value v at p[i] + off + idx
@@ -662,7 +699,8 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
   // cta_stab: every row of this CTA has the same root (whole polynomials, N == C): one table
   // filled by all threads of the CTA instead of one per row
   Tw* stab = cta_stab ? cta_stab : reinterpret_cast<Tw*>(srow + row_elems<E>(LOGC));
-  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, reg_index<LB0>(u, e)); });
+  const unsigned u_in = reg_index<LB0>(u, 0);
+  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, u_in, e << LB0); });
   if constexpr (LD < kSmemRow && sizeof(E) == 8) {
     if (reduce_in) {  // NttMulti::gather: the input is a value of ANOTHER modulus
       static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = reduce_any(v[e], m); });
@@ -684,7 +722,8 @@ __device__ __forceinline__ void row_fwd_body(void* out, const void* in, typename
   constexpr int LB_OUT = LB0 < 4 ? LB0 : 4;
   if constexpr (LOGC > 4) smem_exchange<0, LB_OUT>(v, srow, u);
   if (active) {
-    static_for<0, 16>([&](auto I) { constexpr int e = I; st_row<ST, E>(out, reg_index<LB_OUT>(u, e), v[e]); });
+    const unsigned u_out = reg_index<LB_OUT>(u, 0);
+    static_for<0, 16>([&](auto I) { constexpr int e = I; st_row<ST, E>(out, u_out, e << LB_OUT, v[e]); });
   }
 }
 
@@ -703,7 +742,8 @@ __device__ __forceinline__ void row_inv_body(void* out, const void* in, typename
   constexpr int LB0 = LOGC - 4;
   constexpr int LB_IN = LB0 < 4 ? LB0 : 4;  // 16 lanes read one 128-byte line per instruction
   Tw* stab = cta_stab ? cta_stab : reinterpret_cast<Tw*>(srow + row_elems<E>(LOGC));
-  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, reg_index<LB_IN>(u, e)); });
+  const unsigned u_in = reg_index<LB_IN>(u, 0);
+  static_for<0, 16>([&](auto I) { constexpr int e = I; v[e] = ld_row<LD, E>(in, u_in, e << LB_IN); });
   if constexpr (LD < kSmemRow && sizeof(E) == 8) {
     if (prod) {  // NttMulti::mul: the transform of a point-wise product, multiplied on load
       static_for<0, 16>([&](auto I) {
@@ -727,13 +767,13 @@ __device__ __forceinline__ void row_inv_body(void* out, const void* in, typename
   if (active) {
     static_for<0, 16>([&](auto I) {
       constexpr int e = I;
-      st_row<ST, E>(out, reg_index<LB0>(u, e), fold ? inv_out(v[e], m, out_mf) : v[e]);
+      st_row<ST, E>(out, reg_index<LB0>(u, 0), e << LB0, fold ? inv_out<MODE>(v[e], m, out_mf) : v[e]);
     });
     if (mir && fold) {
       for (unsigned p = 0; p < mir->count; ++p) {
         static_for<0, 16>([&](auto I) {
           constexpr int e = I;
-          mir->p[p][mir->off + reg_index<LB0>(u, e)] = (u64)inv_out(v[e], m, out_mf);
+          mir->p[p][mir->off + reg_index<LB0>(u, e)] = (u64)inv_out<MODE>(v[e], m, out_mf);
         });
       }
     }
@@ -818,7 +858,7 @@ __device__ __forceinline__ void col_stages(typename Ar<MODE>::E (&v)[1 << LOGR],
       if (root_fold) {
         static_for<0, (1 << eb)>([&](auto L) {
           constexpr int l = L;
-          inv_bfly_last(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
+          inv_bfly_last<MODE>(v[l], v[l | (1 << eb)], inv_n, inv_n_w, m, cq);
         });
       } else {
         groups();
@@ -853,13 +893,13 @@ __device__ __forceinline__ void col_body(u64* result, const u64* operand, u64 of
   const bool final_out = !FWD && root_fold;
   static_for<0, R>([&](auto I) {
     constexpr int e = I;
-    st_coef<ST>(result + off + ((u64)e << log_stride), final_out ? inv_out(v[e], m, out_mf) : v[e]);
+    st_coef<ST>(result + off + ((u64)e << log_stride), final_out ? inv_out<MODE>(v[e], m, out_mf) : v[e]);
   });
   if (mir && final_out) {
     for (unsigned p = 0; p < mir->count; ++p) {
       static_for<0, R>([&](auto I) {
         constexpr int e = I;
-        mir->p[p][mir->off + off + ((u64)e << log_stride)] = (u64)inv_out(v[e], m, out_mf);
+        mir->p[p][mir->off + off + ((u64)e << log_stride)] = (u64)inv_out<MODE>(v[e], m, out_mf);
       });
     }
   }
@@ -1209,7 +1249,7 @@ __global__ void __launch_bounds__(DsmemCfg<LOGR, MODE>::THREADS, DsmemCfg<LOGR, 
     col_stages<MODE, LOGR, false>(v, stw, m, true, inv_n, inv_n_w);
     static_for<0, Cfg::R>([&](auto I) {
       constexpr int e = I;
-      st_coef<kStream>(result + poly_off + ((u64)e << Cfg::LOGC) + col, inv_out(v[e], m, out_mf));
+      st_coef<kStream>(result + poly_off + ((u64)e << Cfg::LOGC) + col, inv_out<MODE>(v[e], m, out_mf));
     });
   }
   cluster_barrier();  // nobody leaves while a peer may still read its rows
@@ -1237,9 +1277,9 @@ __global__ void ntt_stage_simple(u64* result, const u64* src, const Twiddle* __r
       Y = fwd_out<kGeneric>(Y, m, out_mf);
     }
   } else if (last) {
-    inv_bfly_last(X, Y, inv_n, inv_n_w, m, m.two_q);
-    X = inv_out(X, m, out_mf);
-    Y = inv_out(Y, m, out_mf);
+    inv_bfly_last<kGeneric>(X, Y, inv_n, inv_n_w, m, m.two_q);
+    X = inv_out<kGeneric>(X, m, out_mf);
+    Y = inv_out<kGeneric>(Y, m, out_mf);
   } else {
     inv_bfly<kGeneric>(X, Y, ld_tw(tw + (1ull << s) + i), m, m.two_q);
   }
@@ -1330,6 +1370,7 @@ __host__ __device__ inline Mod make_mod(u64 q, u64 mu) {
   const u64 negq = 0 - q;
   m.n0 = (unsigned)negq;
   m.n1 = (unsigned)(negq >> 32);
+  m.zero = 0;
   return m;
 }
 inline Mod make_mod(const NttDeviceTables& t) { return make_mod(t.q, t.mu); }

@@ -168,7 +168,7 @@ __global__ void ntt_tiny_multi(u64* result, const u64* operand, const __grid_con
         if constexpr (FWD)
           fwd_bfly<kGeneric>(X, Y, P.fwd[(1 << s) + i], m);
         else if constexpr (s == 0)
-          inv_bfly_last(X, Y, P.inv_n, P.inv_n_w, m, m.two_q);
+          inv_bfly_last<kGeneric>(X, Y, P.inv_n, P.inv_n_w, m, m.two_q);
         else
           inv_bfly<kGeneric>(X, Y, P.inv[(1 << s) + i], m, m.two_q);
       });
@@ -176,13 +176,13 @@ __global__ void ntt_tiny_multi(u64* result, const u64* operand, const __grid_con
   });
   static_for<0, n>([&](auto I) {
     constexpr int e = I;
-    result[unit * n + e] = FWD ? fwd_out<kGeneric>(v[e], m, out_mf) : inv_out(v[e], m, out_mf);
+    result[unit * n + e] = FWD ? fwd_out<kGeneric>(v[e], m, out_mf) : inv_out<kGeneric>(v[e], m, out_mf);
   });
   if (!FWD)
     for (unsigned p = 0; p < multi.mirrors; ++p)
       static_for<0, n>([&](auto I) {
         constexpr int e = I;
-        multi.mirror[p][unit * n + e] = inv_out(v[e], m, out_mf);
+        multi.mirror[p][unit * n + e] = inv_out<kGeneric>(v[e], m, out_mf);
       });
 }
 
