@@ -129,6 +129,10 @@ _sig("hexl_b200_apply_galois_key_switch_hoisted", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp])
 _sig("hexl_b200_fast_base_convert", _int, [_vp, _vp, _u64, _vp, _u64, _vp, _u64, _u64, _vp])
 _sig("hexl_b200_key_switch_hybrid", _int, [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _u64, _vp])
+_sig("hexl_b200_apply_galois_key_switch_hybrid_hoisted", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _u64, _vp])
+_sig("hexl_b200_linear_transform_hybrid", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -637,4 +641,43 @@ def KeySwitchHybrid(result, target, n, level_size, q_size, p_size, digit_size, k
     _check(_lib.hexl_b200_key_switch_hybrid(rp, tp, n, level_size, q_size, p_size, digit_size, key_component_count,
                                             mods.ctypes.data, keys._h if keys is not None else None, batch,
                                             _stream(stream, rc or tc)))
+    return result
+
+
+def ApplyGaloisKeySwitchHybridHoisted(results, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli,
+                                      galois_keys, galois_elts, batch=1, stream=None):
+    """Hoisted rotations with hybrid keys (hexl_b200_apply_galois_key_switch_hybrid_hoisted): ciphertext c of
+    `ciphertexts` (2*level_size*n words each) rotated by every galois_elts[r] with galois_keys[r] (a list of hybrid
+    KeySwitchKeys, key_component_count 2), into results[(c * len(galois_elts) + r) * 2*level_size*n:], its mod-up done
+    once for all elements.  Not bit-identical to ApplyGalois + KeySwitchHybrid for g != 1 (signed digit lift)."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    elts = np.ascontiguousarray(galois_elts, dtype=np.uint64)
+    rp, rn, rc = _buf(results); cp, cn, cc = _buf(ciphertexts)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size); _need("galois_keys", len(galois_keys), elts.size)
+    _need("results", rn, batch * elts.size * per); _need("ciphertexts", cn, batch * per)
+    keys = (_vp * max(1, len(galois_keys)))(*[k._h if k is not None else None for k in galois_keys])
+    _check(_lib.hexl_b200_apply_galois_key_switch_hybrid_hoisted(rp, cp, n, level_size, q_size, p_size, digit_size,
+                                                                 mods.ctypes.data, keys, elts.ctypes.data, elts.size,
+                                                                 batch, _stream(stream, rc or cc)))
+    return results
+
+
+def LinearTransformHybrid(result, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, galois_keys,
+                          galois_elts, diagonals, batch=1, stream=None):
+    """sum_r w_r (.) Rot_{g_r}(ct) with hybrid keys and one mod-down (hexl_b200_linear_transform_hybrid): ciphertext c
+    of `ciphertexts` (2*level_size*n words each) goes to result[c * 2*level_size*n:].  diagonals holds
+    len(galois_elts) x (level_size + p_size) x n words in NTT form (limb i < level_size under q_i, then the special
+    primes).  galois_keys[r] is None for an identity term (galois_elts[r] = 1, adds w_r (.) ct without a key switch)."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    elts = np.ascontiguousarray(galois_elts, dtype=np.uint64)
+    rp, rn, rc = _buf(result); cp, cn, cc = _buf(ciphertexts); dp, dn, dc = _buf(diagonals)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size); _need("galois_keys", len(galois_keys), elts.size)
+    _need("result", rn, batch * per); _need("ciphertexts", cn, batch * per)
+    _need("diagonals", dn, elts.size * (level_size + p_size) * n)
+    keys = (_vp * max(1, len(galois_keys)))(*[k._h if k is not None else None for k in galois_keys])
+    _check(_lib.hexl_b200_linear_transform_hybrid(rp, cp, n, level_size, q_size, p_size, digit_size, mods.ctypes.data,
+                                                  keys, elts.ctypes.data, elts.size, dp, batch,
+                                                  _stream(stream, rc or cc or dc)))
     return result

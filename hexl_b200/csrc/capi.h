@@ -1,6 +1,6 @@
 // What the host sources of the C ABI (include/hexl_b200.h) share: capi.cu (library state, staging, scratch pool),
 // capi_ntt.cu, capi_eltwise.cu, capi_keyswitch.cu (key switch, key handles, rescale), capi_galois.cu and
-// capi_hybrid.cu (hybrid key switch, fast base conversion).
+// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations with hybrid keys).
 // Host-side responsibilities, all one-off or O(1) per call:
 //   * argument validation mirroring the reference's HEXL_CHECKs,
 //   * NTT handle = (N, q, root) -> twiddle tables, built on the host exactly as
@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "../../include/hexl_b200.h"
+#include "hybrid_rotation.h"
 #include "internal.h"
 #include "numtheory.h"
 
@@ -387,6 +388,12 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
 // hs[e] their transforms and slots[e] their slots in keys of kms slots) times the keys of each of `elts` switches,
 // into prod + r * prod_stride ([e][k][n]); chunked by ks_mac_digits_per_launch.  keys[r][j]: digit j's key of switch
 // r; galois_elts[r] (nullptr: none) makes switch r read the digits permuted by pi_g.
+// The multiply-accumulate's constants of cnt <= kParamBlock moduli: q, floor(2^64 / q), 2^64 mod q and its Shoup
+// factor, and c = slots[e] (0 when slots is null)
+KsModuli ks_mac_moduli(const uint64_t* moduli, const uint64_t* slots, uint64_t cnt);
+// Digits one multiply-accumulate launch may sum unreduced in 128 bits for the moduli of mods: 64 below 2^60, down to
+// 16 just below 2^61
+uint64_t ks_mac_digits_per_launch(const KsModuli& mods, uint64_t count);
 int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cnt, uint64_t kms, const uint64_t* ops,
                     uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod, uint64_t prod_stride,
                     const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s);
@@ -394,10 +401,11 @@ int key_switch_elts_on_device(int dev, uint64_t* const* results, const uint64_t*
                               uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
                               const uint64_t* const* const* d_key_ptrs, const uint64_t* galois_elts, uint64_t elts,
                               const uint64_t* modswitch, cudaStream_t s);
-// run(dev, device result block, device input block, the key handles' copies on dev, stream): one ciphertext's switch
+// run(dev, device result block, device input block, the key handles' copies on dev, stream): one ciphertext's switch.
+// prepare(dev) (optional) runs once on each device of the split, with it current, before its first ciphertext.
 using HostSwitch = std::function<int(int, uint64_t*, uint64_t*, const uint64_t* const* const*, cudaStream_t)>;
 int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, const uint64_t* in, uint64_t in_words,
                           uint64_t buf_words, const hexl_b200_keys* const* keys, uint64_t num_keys, uint64_t batch,
-                          const HostSwitch& run);
+                          const HostSwitch& run, const std::function<int(int)>& prepare = nullptr);
 
 }  // namespace hexl_b200

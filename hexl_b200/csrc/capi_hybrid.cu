@@ -1,5 +1,7 @@
 // Hybrid key switching (OpenFHE's KeySwitchHYBRID): digits of up to 64 data moduli and up to 64 special primes, the
-// mod-up and the mod-down by fast base conversion (rns.cu); and the base conversion on its own.
+// mod-up and the mod-down by fast base conversion (rns.cu); the base conversion on its own; and the rotations with
+// hybrid keys: hoisted, and the diagonal-weighted sum of rotations under one mod-down (the linear transform).
+#include <cstdio>
 #include <numeric>
 
 #include "capi.h"
@@ -65,30 +67,28 @@ static int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t 
   return 0;
 }
 
-// One hybrid key switch (include/hexl_b200.h has the definitions), every pointer a device pointer on the current
-// device, asynchronous on s.  h holds the transforms of the extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}} in that
-// order and bmods their moduli; keys[d] is digit d's key buffer, kcc x (q_size + K) x n words.  Scratch layouts are
-// [modulus][digit or component][n], as in key_switch_elts_on_device.
-static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level,
-                                       uint64_t q_size, uint64_t p_size, uint64_t alpha, uint64_t kcc,
-                                       const CachedNtts& h, const uint64_t* bmods, const uint64_t* const* keys,
-                                       cudaStream_t s) {
-  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size;
+// The mod-up of one target (level limbs in NTT form, device memory), steps 1 and 2 of the hybrid switch
+// (include/hexl_b200.h has the definitions).  h holds the transforms of the extended basis
+// B = {q_0..q_{l-1}, p_0..p_{K-1}} in that order and bmods their moduli.  The target's limbs go back to coefficients
+// once; then, per round of moduli of B, every digit is converted into each modulus of the round and lazily
+// transformed into ops ([e][d][n], D x n words between moduli), and mac(b0, cnt, ops, slots) multiplies them with the
+// keys: moduli [b0, b0 + cnt) of B, slots[e] the key slot of modulus b0 + e.  Scratch comes from ws.
+template <class Mac>
+static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t level, uint64_t q_size,
+                         uint64_t p_size, uint64_t alpha, const CachedNtts& h, const uint64_t* bmods, Scratch& ws,
+                         Mac&& mac, cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size;
   // moduli handled per round of the mod-up: bounded by the parameter block and by ~256 MiB of scratch
   const uint64_t per_mod = D * n;
   uint64_t ichunk = std::max<uint64_t>(1, (256ull << 20) / (per_mod * 8));
   ichunk = std::min<uint64_t>({ichunk, nb, (uint64_t)kParamBlock});
-  Scratch ws(s);
-  uint64_t *t_coef = nullptr, *ops = nullptr, *prod = nullptr, *tmp = nullptr;
+  uint64_t *t_coef = nullptr, *ops = nullptr;
   if (int rc = ws.get(&t_coef, level * n)) return rc;
-  if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;                                  // [e][d][n]
-  if (int rc = ws.get(&prod, nb * kcc * n)) return rc;                                      // [b][k][n]
-  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * kcc * n)) return rc;  // [i][k][n], one block
+  if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;  // [e][d][n]
   // 1. the target's limbs back to coefficients, canonical
   if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s)) return rc;
   // 2. mod-up: every digit converted into each modulus of the round, lazily transformed, multiplied with the keys.
   //    (A digit's own limbs are converted and transformed again like the others: NTT(INTT(t)) = t.)
-  const uint64_t* const* key_sets = keys;
   for (uint64_t b0 = 0; b0 < nb; b0 += ichunk) {
     const uint64_t cnt = std::min(ichunk, nb - b0);
     for (uint64_t d = 0; d < D; ++d) {
@@ -100,12 +100,16 @@ static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t
     if (int rc = ntt_multi_on_device(true, dev, h.data() + b0, cnt, ops, ops, 4, D, s)) return rc;
     uint64_t slots[kParamBlock];
     for (uint64_t e = 0; e < cnt; ++e) slots[e] = b0 + e < level ? b0 + e : q_size + (b0 + e - level);
-    if (int rc = ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, kcc, prod + b0 * kcc * n, 0, &key_sets,
-                                 nullptr, 1, s))
-      return rc;
+    if (int rc = mac(b0, cnt, (const uint64_t*)ops, (const uint64_t*)slots)) return rc;
   }
-  // 3. mod-down by P: the special limbs back to coefficients, rounded and converted into each data modulus,
-  //    transformed, and (prod - that) * P^-1 accumulated into result
+  return 0;
+}
+
+// Step 3, the mod-down by P, of one switch's products prod ([b][k][n] over the moduli of B, kcc components): the
+// special limbs back to coefficients in place, rounded and converted into each data modulus, transformed, and
+// (prod - that) * P^-1 accumulated into result (kcc x level x n).  tmp holds min(level, 64) x kcc x n words.
+static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* tmp, uint64_t n, uint64_t level,
+                           uint64_t p_size, uint64_t kcc, const CachedNtts& h, const uint64_t* bmods, cudaStream_t s) {
   uint64_t* special = prod + level * kcc * n;  // [j][k][n]
   if (int rc = ntt_multi_on_device(false, dev, h.data() + level, p_size, special, special, 1, kcc, s)) return rc;
   for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
@@ -125,7 +129,168 @@ static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t
     const cudaError_t e = launch_ks_finish(result, prod + i0 * kcc * n, tmp, n, kcc, level, i0, cnt, fin, false, true, s);
     if (e != cudaSuccess) return cuda_fail(e, "hybrid mod-down: finish launch");
   }
+  return 0;
+}
+
+// `elts` hybrid key switches of one target, every pointer a device pointer on the current device, asynchronous on s:
+// the mod-up once, then for switch r the multiply-accumulate with keys[r] (keys[r][d]: digit d's key buffer,
+// kcc x (q_size + K) x n words) and one mod-down accumulated into results[r].  galois_elts[r] (nullptr: none) makes
+// switch r read the transformed digits permuted by pi_g, as key_switch_elts_on_device does for the hoisted
+// rotations.  Scratch: one round of transformed digits plus elts x (level + K) x kcc x n words of products.
+static int key_switch_hybrid_elts_on_device(int dev, uint64_t* const* results, const uint64_t* target, uint64_t n,
+                                            uint64_t level, uint64_t q_size, uint64_t p_size, uint64_t alpha,
+                                            uint64_t kcc, const CachedNtts& h, const uint64_t* bmods,
+                                            const uint64_t* const* const* keys, const uint64_t* galois_elts,
+                                            uint64_t elts, cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size;
+  Scratch ws(s);
+  uint64_t *prod = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&prod, elts * nb * kcc * n)) return rc;                               // [r][b][k][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * kcc * n)) return rc;  // [i][k][n], one block
+  if (int rc = hybrid_mod_up(dev, target, n, level, q_size, p_size, alpha, h, bmods, ws,
+                             [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) {
+                               return ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, kcc,
+                                                      prod + b0 * kcc * n, nb * kcc * n, keys, galois_elts, elts, s);
+                             },
+                             s))
+    return rc;
+  for (uint64_t r = 0; r < elts; ++r)
+    if (int rc = hybrid_mod_down(dev, results[r], prod + r * nb * kcc * n, tmp, n, level, p_size, kcc, h, bmods, s))
+      return rc;
   return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
+}
+
+static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level,
+                                       uint64_t q_size, uint64_t p_size, uint64_t alpha, uint64_t kcc,
+                                       const CachedNtts& h, const uint64_t* bmods, const uint64_t* const* keys,
+                                       cudaStream_t s) {
+  return key_switch_hybrid_elts_on_device(dev, &result, target, n, level, q_size, p_size, alpha, kcc, h, bmods, &keys,
+                                          nullptr, 1, s);
+}
+
+// The hoisted hybrid rotations of one ciphertext ct (two components of level limbs, NTT form, device memory) by
+// `elts` elements: per element one automorphism launch of c0 straight into its output and a memset of the output's
+// c1, then the shared switch of c1 with every element's keys, read through pi_g.
+static int hybrid_hoisted_on_device(int dev, uint64_t* out, const uint64_t* ct, uint64_t n, uint64_t level,
+                                    uint64_t q_size, uint64_t p_size, uint64_t alpha, const CachedNtts& h,
+                                    const uint64_t* bmods, const uint64_t* const* const* keys,
+                                    const uint64_t* galois_elts, uint64_t elts, cudaStream_t s) {
+  const uint64_t comp = level * n;
+  std::vector<uint64_t*> results(elts);
+  for (uint64_t r = 0; r < elts; ++r) {
+    results[r] = out + r * 2 * comp;
+    const cudaError_t e = launch_galois_ntt(results[r], ct, floor_log2(n), level, galois_elts[r], s);
+    if (e != cudaSuccess) return cuda_fail(e, "ApplyGaloisKeySwitchHybridHoisted: automorphism launch");
+    CU(cudaMemsetAsync(results[r] + comp, 0, comp * sizeof(uint64_t), s));
+  }
+  return key_switch_hybrid_elts_on_device(dev, results.data(), ct + comp, n, level, q_size, p_size, alpha, 2, h, bmods,
+                                          keys, galois_elts, elts, s);
+}
+
+// The hybrid linear transform of one ciphertext ct (as above) into result (2 x level x n words, device memory):
+// keys[r] is element r's key copy, or nullptr for an identity term; diag holds elts diagonals of (level + K) x n
+// words.  First the weighted permuted sum of ct's limbs is stored into result (one launch per chunk of 64 elements
+// and block of 64 data moduli); then, when any element has keys, the shared mod-up, the weighted multiply-accumulate
+// of every keyed element into one accumulator over B (one launch per round, chunk of (element, digit) pairs and
+// chunk of digits) and one mod-down of the accumulator into result.
+static int linear_transform_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct, const uint64_t* diag,
+                                             uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size,
+                                             uint64_t alpha, const CachedNtts& h, const uint64_t* bmods,
+                                             const uint64_t* const* const* keys, const uint64_t* galois_elts,
+                                             uint64_t elts, cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, dstride = nb * n;
+  for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
+    const uint64_t cnt = std::min<uint64_t>(kParamBlock, level - i0);
+    const KsModuli mods = ks_mac_moduli(bmods + i0, nullptr, cnt);
+    for (uint64_t r0 = 0; r0 < elts; r0 += kParamBlock) {
+      const uint64_t ecnt = std::min<uint64_t>(kParamBlock, elts - r0);
+      PermutedSumElts ps{};
+      for (uint64_t r = 0; r < ecnt; ++r) {
+        ps.diag[r] = diag + (r0 + r) * dstride + i0 * n;
+        ps.elt[r] = (unsigned)galois_elts[r0 + r];
+        if (!keys[r0 + r]) ps.identity |= 1ull << r;
+      }
+      const cudaError_t e = launch_ks_permuted_sum(result, ct, n, level, i0, cnt, ps, ecnt, mods, r0 != 0, s);
+      if (e != cudaSuccess) return cuda_fail(e, "LinearTransformHybrid: permuted sum launch");
+    }
+  }
+  std::vector<uint64_t> keyed;
+  for (uint64_t r = 0; r < elts; ++r)
+    if (keys[r]) keyed.push_back(r);
+  if (keyed.empty()) return 0;
+  Scratch ws(s);
+  uint64_t *acc = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&acc, nb * 2 * n)) return rc;                                       // [b][k][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * 2 * n)) return rc;  // [i][k][n], one block
+  auto mac = [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) -> int {
+    const KsModuli mods = ks_mac_moduli(bmods + b0, slots, cnt);
+    // (element, digit) pairs per launch: a digit chunk within the 128-bit bound, as many elements as fill the block
+    const uint64_t jc = std::min(ks_mac_digits_per_launch(mods, cnt), D);
+    const uint64_t per = std::max<uint64_t>(1, kParamBlock / jc);
+    bool accumulate = false;
+    for (uint64_t j0 = 0; j0 < D; j0 += jc) {
+      const uint64_t jcnt = std::min(jc, D - j0);
+      for (uint64_t k0 = 0; k0 < keyed.size(); k0 += per) {
+        const uint64_t ecnt = std::min<uint64_t>(per, keyed.size() - k0);
+        WeightedMacElts we{};
+        for (uint64_t e = 0; e < ecnt; ++e) {
+          const uint64_t r = keyed[k0 + e];
+          for (uint64_t j = 0; j < jcnt; ++j) we.key[e * jcnt + j] = keys[r][j0 + j];
+          we.diag[e] = diag + r * dstride + b0 * n;
+          we.elt[e] = (unsigned)galois_elts[r];
+        }
+        const cudaError_t e = launch_ks_weighted_mac(acc + b0 * 2 * n, ops + j0 * n, D * n, we, n, jcnt, ecnt, kms,
+                                                     cnt, mods, accumulate, s);
+        if (e != cudaSuccess) return cuda_fail(e, "LinearTransformHybrid: multiply-accumulate launch");
+        accumulate = true;
+      }
+    }
+    return 0;
+  };
+  if (int rc = hybrid_mod_up(dev, ct + level * n, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s)) return rc;
+  return hybrid_mod_down(dev, result, acc, tmp, n, level, p_size, 2, h, bmods, s);
+}
+
+// The shape rules of hexl_b200_key_switch_hybrid, without the key handle
+static int hybrid_shape_check(uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size, uint64_t alpha,
+                              uint64_t kcc, const uint64_t* moduli) {
+  const uint64_t kms = q_size + p_size;
+  REQUIRE(n >= 2 && n <= (1ull << 20) && !(n & (n - 1)), "Require n a power of two in [2, 2^20]");
+  REQUIRE(level >= 1 && level <= q_size, "Require 1 <= level_size <= q_size");
+  REQUIRE(alpha >= 1 && alpha <= (uint64_t)kParamBlock, "Require 1 <= digit_size <= %d", kParamBlock);
+  REQUIRE(p_size >= 1 && p_size <= (uint64_t)kParamBlock, "Require 1 <= p_size <= %d", kParamBlock);
+  REQUIRE(kcc >= 1, "Require key_component_count >= 1");
+  for (uint64_t i = 0; i < kms; ++i) {
+    const char* why = "";
+    // the lazy sums of the multiply-accumulate and of the finish step (< 8q) need q < 2^61
+    REQUIRE(moduli[i] < (1ull << 61), "Require moduli < 2^61 (moduli[%llu])", (unsigned long long)i);
+    REQUIRE(check_ntt_arguments(n, moduli[i], &why), "moduli[%llu]: %s", (unsigned long long)i, why);
+  }
+  std::vector<uint64_t> sorted(moduli, moduli + kms);
+  std::sort(sorted.begin(), sorted.end());
+  REQUIRE(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end(), "Require distinct moduli");
+  return 0;
+}
+
+// A hybrid key handle of the shape: ceil(q_size / digit_size) digits, kcc x (q_size + p_size) words, not sharded
+static int hybrid_handle_check(const hexl_b200_keys* keys, uint64_t n, uint64_t q_size, uint64_t p_size,
+                               uint64_t alpha, uint64_t kcc, const char* what) {
+  REQUIRE(keys_fit(keys, n, (q_size + alpha - 1) / alpha, kcc, q_size + p_size),
+          "%s was uploaded for another shape (decomp = ceil(q_size / digit_size), "
+          "key_modulus_size = q_size + p_size)", what);
+  REQUIRE(keys->shards.empty(), "%s: hybrid key switching does not take keys sharded by modulus: upload them with "
+                                "hexl_b200_keys_upload", what);
+  return 0;
+}
+
+// The extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}} and its transforms
+static int hybrid_basis(uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size, const uint64_t* moduli,
+                        std::vector<uint64_t>* bmods, CachedNtts* h) {
+  bmods->assign(moduli, moduli + level);
+  bmods->insert(bmods->end(), moduli + q_size, moduli + q_size + p_size);
+  for (uint64_t b = 0; b < bmods->size(); ++b)
+    if (int rc = h->load(b, n, (*bmods)[b])) return rc;
+  return 0;
 }
 
 // Host buffers of the base conversion: chunks of whole polynomials through stage_items, split by polynomial over the
@@ -193,27 +358,10 @@ int hexl_b200_fast_base_convert(uint64_t* result, const uint64_t* operand, uint6
 int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
                                 uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
                                 const uint64_t* moduli, const hexl_b200_keys* keys, uint64_t batch, void* stream) {
-  const uint64_t level = level_size, alpha = digit_size, kcc = key_component_count, kms = q_size + p_size;
+  const uint64_t level = level_size, alpha = digit_size, kcc = key_component_count;
   REQUIRE(result && target && moduli && keys, "Require non-null arguments");
-  REQUIRE(n >= 2 && n <= (1ull << 20) && !(n & (n - 1)), "Require n a power of two in [2, 2^20]");
-  REQUIRE(level >= 1 && level <= q_size, "Require 1 <= level_size <= q_size");
-  REQUIRE(alpha >= 1 && alpha <= (uint64_t)kParamBlock, "Require 1 <= digit_size <= %d", kParamBlock);
-  REQUIRE(p_size >= 1 && p_size <= (uint64_t)kParamBlock, "Require 1 <= p_size <= %d", kParamBlock);
-  REQUIRE(kcc >= 1, "Require key_component_count >= 1");
-  for (uint64_t i = 0; i < kms; ++i) {
-    const char* why = "";
-    // the lazy sums of the multiply-accumulate and of the finish step (< 8q) need q < 2^61
-    REQUIRE(moduli[i] < (1ull << 61), "Require moduli < 2^61 (moduli[%llu])", (unsigned long long)i);
-    REQUIRE(check_ntt_arguments(n, moduli[i], &why), "moduli[%llu]: %s", (unsigned long long)i, why);
-  }
-  std::vector<uint64_t> sorted(moduli, moduli + kms);
-  std::sort(sorted.begin(), sorted.end());
-  REQUIRE(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end(), "Require distinct moduli");
-  REQUIRE(keys_fit(keys, n, (q_size + alpha - 1) / alpha, kcc, kms),
-          "the key handle was uploaded for another shape (decomp = ceil(q_size / digit_size), "
-          "key_modulus_size = q_size + p_size)");
-  REQUIRE(keys->shards.empty(), "KeySwitchHybrid does not take keys sharded by modulus: upload them with "
-                                "hexl_b200_keys_upload");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, kcc, moduli)) return rc;
+  if (int rc = hybrid_handle_check(keys, n, q_size, p_size, alpha, kcc, "the key handle")) return rc;
   if (batch == 0) return 0;
   const uint64_t in_words = level * n, out_words = kcc * level * n;
   REQUIRE(result + batch * out_words <= target || target + batch * in_words <= result,
@@ -221,12 +369,9 @@ int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64
   PtrInfo pi;
   if (int rc = classify_all({result, target}, &pi)) return rc;
   if (int rc = check_limb_bounds(target, batch, level, n, [&](u64 i) { return moduli[i]; }, pi, "target")) return rc;
-  // the extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}} and its transforms
-  std::vector<uint64_t> bmods(moduli, moduli + level);
-  bmods.insert(bmods.end(), moduli + q_size, moduli + kms);
-  CachedNtts h(bmods.size());
-  for (uint64_t b = 0; b < bmods.size(); ++b)
-    if (int rc = h.load(b, n, bmods[b])) return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(level + p_size);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
   if (pi.where == Where::Host)
     return key_switch_host_batch(result, out_words, true, target, in_words, in_words, &keys, 1, batch,
                                  [&](int dev, uint64_t* d_res, uint64_t* d_t, const uint64_t* const* const* dk,
@@ -242,6 +387,161 @@ int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64
       if (int rc = key_switch_hybrid_on_device(pi.device, result + c * out_words, target + c * in_words, n, level,
                                                q_size, p_size, alpha, kcc, h, bmods.data(), dk[0],
                                                (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+}  // extern "C"
+
+namespace {
+
+// The element and key-handle rules of the two hybrid rotation calls.  identity_ok: a null handle is an identity term,
+// allowed for the element 1 only; otherwise every handle must be there.
+int hybrid_elts_check(uint64_t n, uint64_t q_size, uint64_t p_size, uint64_t alpha, const hexl_b200_keys* const* keys,
+                      const uint64_t* elts, uint64_t num_elts, bool identity_ok) {
+  for (uint64_t r = 0; r < num_elts; ++r) {
+    REQUIRE(elts[r] % 2 == 1 && elts[r] < 2 * n, "Require galois_elts[%llu] odd and in [1, 2n)", (unsigned long long)r);
+    if (!keys[r]) {
+      REQUIRE(identity_ok, "Require galois_keys[%llu] != nullptr", (unsigned long long)r);
+      REQUIRE(elts[r] == 1, "galois_keys[%llu] may be null only for galois_elts[%llu] = 1 (an identity term)",
+              (unsigned long long)r, (unsigned long long)r);
+      continue;
+    }
+    char what[40];
+    std::snprintf(what, sizeof what, "galois_keys[%llu]", (unsigned long long)r);
+    if (int rc = hybrid_handle_check(keys[r], n, q_size, p_size, alpha, 2, what)) return rc;
+  }
+  return 0;
+}
+
+// Per element, the copy of its handle among `dk` (the copies of the non-null handles, in element order), or nullptr
+// for an identity term
+std::vector<const uint64_t* const*> per_element(const hexl_b200_keys* const* keys, uint64_t num_elts,
+                                                const uint64_t* const* const* dk) {
+  std::vector<const uint64_t* const*> out(num_elts, nullptr);
+  for (uint64_t r = 0, k = 0; r < num_elts; ++r)
+    if (keys[r]) out[r] = dk[k++];
+  return out;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                                     uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                                     uint64_t digit_size, const uint64_t* moduli,
+                                                     const hexl_b200_keys* const* galois_keys,
+                                                     const uint64_t* galois_elts, uint64_t num_elts, uint64_t batch,
+                                                     void* stream) {
+  const uint64_t level = level_size, alpha = digit_size;
+  REQUIRE(results && ciphertexts && moduli, "Require non-null arguments");
+  REQUIRE(num_elts == 0 || (galois_keys && galois_elts), "Require galois_keys, galois_elts != nullptr");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (int rc = hybrid_elts_check(n, q_size, p_size, alpha, galois_keys, galois_elts, num_elts, false)) return rc;
+  if (num_elts == 0 || batch == 0) return 0;
+  const uint64_t comp = level * n, in_total = batch * 2 * comp, out_total = batch * num_elts * 2 * comp;
+  REQUIRE(results + out_total <= ciphertexts || ciphertexts + in_total <= results,
+          "results and ciphertexts must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({results, ciphertexts}, &pi)) return rc;
+  if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
+                                 "ciphertexts"))
+    return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(level + p_size);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  // host pointers: each ciphertext crosses PCIe in once and its num_elts rotations come back from the same slot
+  if (pi.where == Where::Host)
+    return key_switch_host_batch(results, num_elts * 2 * comp, false, ciphertexts, 2 * comp, 2 * comp, galois_keys,
+                                 num_elts, batch,
+                                 [&](int dev, uint64_t* d_res, uint64_t* d_ct, const uint64_t* const* const* dk,
+                                     cudaStream_t s) {
+                                   return hybrid_hoisted_on_device(dev, d_res, d_ct, n, level, q_size, p_size, alpha,
+                                                                   h, bmods.data(), dk, galois_elts, num_elts, s);
+                                 });
+  std::vector<const uint64_t* const*> dk;
+  const uint64_t missing = keys_on_device(galois_keys, num_elts, pi.device, &dk);
+  if (missing < num_elts)
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "galois_keys[%llu] holds no copy on the device of the ciphertexts",
+                (unsigned long long)missing);
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = hybrid_hoisted_on_device(pi.device, results + c * num_elts * 2 * comp, ciphertexts + c * 2 * comp, n,
+                                            level, q_size, p_size, alpha, h, bmods.data(), dk.data(), galois_elts,
+                                            num_elts, (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                                      uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                      const hexl_b200_keys* const* galois_keys, const uint64_t* galois_elts,
+                                      uint64_t num_elts, const uint64_t* diagonals, uint64_t batch, void* stream) {
+  const uint64_t level = level_size, alpha = digit_size;
+  REQUIRE(result && ciphertexts && moduli, "Require non-null arguments");
+  REQUIRE(num_elts == 0 || (galois_keys && galois_elts && diagonals),
+          "Require galois_keys, galois_elts, diagonals != nullptr");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (int rc = hybrid_elts_check(n, q_size, p_size, alpha, galois_keys, galois_elts, num_elts, true)) return rc;
+  if (num_elts == 0 || batch == 0) return 0;
+  const uint64_t comp = level * n, nb = level + p_size, ct_total = batch * 2 * comp, diag_total = num_elts * nb * n;
+  REQUIRE(result + ct_total <= ciphertexts || ciphertexts + ct_total <= result,
+          "result and ciphertexts must not overlap");
+  REQUIRE(result + ct_total <= diagonals || diagonals + diag_total <= result, "result and diagonals must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, ciphertexts, diagonals}, &pi)) return rc;
+  if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
+                                 "ciphertexts"))
+    return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(nb);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  if (int rc = check_limb_bounds(diagonals, num_elts, nb, n, [&](u64 i) { return bmods[i]; }, pi, "diagonals"))
+    return rc;
+  std::vector<const hexl_b200_keys*> keyed;  // the handles of the elements that switch keys
+  for (uint64_t r = 0; r < num_elts; ++r)
+    if (galois_keys[r]) keyed.push_back(galois_keys[r]);
+  if (pi.where == Where::Host) {
+    // host pointers: the diagonals go to each device of the split once, before its first ciphertext; each ciphertext
+    // crosses PCIe in once and its result comes back from the same slot
+    std::vector<std::pair<int, uint64_t*>> uploaded;
+    const int rc = key_switch_host_batch(
+        result, 2 * comp, false, ciphertexts, 2 * comp, 2 * comp, keyed.data(), keyed.size(), batch,
+        [&](int dev, uint64_t* d_res, uint64_t* d_ct, const uint64_t* const* const* dk, cudaStream_t s) {
+          const uint64_t* d_diag = nullptr;
+          for (auto& u : uploaded)
+            if (u.first == dev) d_diag = u.second;
+          const auto keys = per_element(galois_keys, num_elts, dk);
+          return linear_transform_hybrid_on_device(dev, d_res, d_ct, d_diag, n, level, q_size, p_size, alpha, h,
+                                                   bmods.data(), keys.data(), galois_elts, num_elts, s);
+        },
+        [&](int dev) -> int {
+          uint64_t* p = nullptr;
+          CU(cudaMalloc(&p, diag_total * sizeof(uint64_t)));
+          uploaded.emplace_back(dev, p);
+          CU(cudaMemcpy(p, diagonals, diag_total * sizeof(uint64_t), cudaMemcpyHostToDevice));
+          CU(cudaStreamSynchronize(nullptr));  // the staging streams do not wait for the legacy stream's copy
+          return 0;
+        });
+    for (auto& u : uploaded) {
+      DeviceGuard g;
+      if (g.enter(u.first) == 0) cudaFree(u.second);
+    }
+    return rc;
+  }
+  std::vector<const uint64_t* const*> dk;
+  const uint64_t found = keys_on_device(keyed.data(), keyed.size(), pi.device, &dk);
+  if (found < keyed.size())
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "a key handle holds no copy on the device of the ciphertexts");
+  const auto keys = per_element(galois_keys, num_elts, dk.data());
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = linear_transform_hybrid_on_device(pi.device, result + c * 2 * comp, ciphertexts + c * 2 * comp,
+                                                     diagonals, n, level, q_size, p_size, alpha, h, bmods.data(),
+                                                     keys.data(), galois_elts, num_elts, (cudaStream_t)stream))
         return rc;
     return 0;
   });

@@ -32,7 +32,7 @@ static int key_switch_ntts(CachedNtts& h, uint64_t n, const uint64_t* moduli, ui
 // output (< 4q) times a key word (< q) and the kernel sums them unreduced in 128 bits, so at most
 // (2^128 - 1) / ((4q - 1)(q - 1)) of them fit for the largest q: the whole 64-entry key block below 2^60, down to 16
 // just below 2^61.  Launches beyond the first add their reduced sums into prod (the `accumulate` flag).
-static uint64_t ks_mac_digits_per_launch(const KsModuli& mods, uint64_t count) {
+uint64_t ks_mac_digits_per_launch(const KsModuli& mods, uint64_t count) {
   uint64_t q = 0;
   for (uint64_t e = 0; e < count; ++e) q = std::max(q, mods.m[e].q);
   const unsigned __int128 largest_product = (unsigned __int128)(4 * q - 1) * (q - 1);
@@ -54,16 +54,23 @@ static int ks_mac_round(int dev, hexl_b200_ntt* const* hs, const uint64_t* slots
   return ks_mac_products(hs, slots, cnt, kms, ops, decomp, n, kcc, prod, prod_stride, keys, galois_elts, elts, s);
 }
 
+KsModuli ks_mac_moduli(const uint64_t* moduli, const uint64_t* slots, uint64_t cnt) {
+  KsModuli mods;
+  for (uint64_t e = 0; e < cnt; ++e) {
+    const uint64_t q = moduli[e], mu = nt::multiply_factor(1, 64, q);
+    const uint64_t r64 = mu * (0 - q);  // 2^64 - floor(2^64/q)*q = 2^64 mod q
+    const Twiddle R = make_twiddle(r64 % q, q);
+    mods.m[e] = KsModulus{q, mu, R.w, R.wp, slots ? slots[e] : 0};
+  }
+  return mods;
+}
+
 int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cnt, uint64_t kms, const uint64_t* ops,
                     uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod, uint64_t prod_stride,
                     const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s) {
-  KsModuli mods;
-  for (uint64_t e = 0; e < cnt; ++e) {
-    const uint64_t q = hs[e]->q, mu = nt::multiply_factor(1, 64, q);
-    const uint64_t r64 = mu * (0 - q);  // 2^64 - floor(2^64/q)*q = 2^64 mod q
-    const Twiddle R = make_twiddle(r64 % q, q);
-    mods.m[e] = KsModulus{q, mu, R.w, R.wp, slots[e]};
-  }
+  uint64_t q[kParamBlock];
+  for (uint64_t e = 0; e < cnt; ++e) q[e] = hs[e]->q;
+  const KsModuli mods = ks_mac_moduli(q, slots, cnt);
   const uint64_t per_mod = decomp * n, jmax = ks_mac_digits_per_launch(mods, cnt);
   for (uint64_t r = 0; r < elts; ++r)
     for (uint64_t j0 = 0; j0 < decomp; j0 += jmax) {  // key pointers ride in the kernel parameters
@@ -198,7 +205,8 @@ uint64_t keys_on_device(const hexl_b200_keys* const* keys, uint64_t count, int d
 // holds buf_words words.
 int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, const uint64_t* in,
                           uint64_t in_words, uint64_t buf_words, const hexl_b200_keys* const* keys,
-                          uint64_t num_keys, uint64_t batch, const HostSwitch& run) {
+                          uint64_t num_keys, uint64_t batch, const HostSwitch& run,
+                          const std::function<int(int)>& prepare) {
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
   std::vector<const uint64_t* const*> dk;
@@ -208,6 +216,8 @@ int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, 
   if (use.empty()) return fail(HEXL_B200_ERR_INVALID_ARG, "the key handle holds no copy on the device(s) used for host calls");
   return stage_items(use, batch, 1, [&](int dev, u64, u64, auto&& stage) {
     keys_on_device(keys, num_keys, dev, &dk);
+    if (prepare)
+      if (int rc = prepare(dev)) return rc;
     return stage([&](const StageSlot& sl, u64 c, u64) -> int {
       if (int rc = sl.reserve(0, res_words * 8)) return rc;
       if (int rc = sl.reserve(1, buf_words * 8)) return rc;

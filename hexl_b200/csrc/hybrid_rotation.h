@@ -1,0 +1,41 @@
+// Launchers of the two kernels of the hybrid linear transform (seal.cu): the weighted multi-element
+// multiply-accumulate and the weighted permuted sum of the ciphertext's limbs.  Both take two-component ciphertexts
+// (key component count 2) in NTT form, every word canonical, every modulus below 2^61.
+#pragma once
+#include "internal.h"
+
+namespace hexl_b200 {
+
+// One launch covers up to kParamBlock (element, digit) pairs: `elts` elements of a chunk times the digits
+// [j0, j0 + jcount) of a digit chunk.  key[r * jcount + j] is digit j0 + j's key of element r (2 x kms x n words),
+// diag[r] element r's diagonal at the limb of the round's first modulus, elt[r] its Galois element.
+struct WeightedMacElts {
+  const u64* key[kParamBlock];
+  const u64* diag[kParamBlock];
+  unsigned elt[kParamBlock];
+};
+// For the `count` moduli of a mod-up round (mods as for launch_ks_mac: a, b = 2^64 mod q and its Shoup factor, c =
+// the modulus's slot in the keys), every slot l and both key components k:
+//   acc[e][k][l] (+)= sum_r w_r[e][l] ( sum_{j < jcount} ops[e][j][pi_r(l)] key_{r,j}[k][c_e][l] mod q_e )  mod q_e
+// ops_stride = elements between e's.  The digit sum stays unreduced in 128 bits, so jcount must respect the bound of
+// ks_mac_digits_per_launch; the weighted sum of at most 64 canonical products cannot wrap below 2^61.
+cudaError_t launch_ks_weighted_mac(u64* acc, const u64* ops, u64 ops_stride, const WeightedMacElts& elts, u64 n,
+                                   u64 jcount, u64 num_elts, u64 key_modulus_size, u64 count, const KsModuli& mods,
+                                   bool accumulate, cudaStream_t stream);
+
+// Up to kParamBlock elements of one launch: diag[r] element r's diagonal at the limb of the block's first modulus,
+// elt[r] its Galois element; bit r of `identity` marks an identity term (g = 1 with no key), which adds w_r c1 too.
+struct PermutedSumElts {
+  const u64* diag[kParamBlock];
+  unsigned elt[kParamBlock];
+  u64 identity;
+};
+// For the data limbs [i0, i0 + count) of one ciphertext ct (two components of `level` limbs, mods.m[e] describing
+// limb i0 + e with a, b = 2^64 mod q and its Shoup factor), every slot l:
+//   result_0[i][l] (+)= sum_r w_r[i][l] c0_i[pi_r(l)],   result_1[i][l] (+)= sum_{r identity} w_r[i][l] c1_i[l]
+// canonical; accumulate adds into result (later chunks of elements), else stores.  result must not overlap ct.
+cudaError_t launch_ks_permuted_sum(u64* result, const u64* ct, u64 n, u64 level, u64 i0, u64 count,
+                                   const PermutedSumElts& elts, u64 num_elts, const KsModuli& mods, bool accumulate,
+                                   cudaStream_t stream);
+
+}  // namespace hexl_b200

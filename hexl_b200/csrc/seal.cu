@@ -7,6 +7,7 @@
 //   KeySwitch        hexl/experimental/seal/key-switch-internal.cpp:25-201
 //   rescale          SEAL's RNSTool::divide_and_round_q_last(_ntt)_inplace
 #include "galois.cuh"
+#include "hybrid_rotation.h"
 #include "internal.h"
 
 namespace hexl_b200 {
@@ -163,6 +164,88 @@ __global__ void __launch_bounds__(kThreads)
   prod[g] = v;
 }
 
+// ---- The hybrid linear transform: sum_r w_r (.) Rot_{g_r}(ct) with one mod-down for the whole sum.
+// (hi, lo) += a b, unreduced
+__device__ __forceinline__ void mac128(u64 a, u64 b, u64& lo, u64& hi) {
+  const u64 plo = a * b;
+  lo += plo;
+  hi += mulhi(a, b) + (lo < plo);
+}
+// (hi 2^64 + lo) mod q, canonical: Shoup(hi, 2^64 mod q) + Barrett(lo) < 4q, then two conditional subtractions
+__device__ __forceinline__ u64 reduce128(u64 hi, u64 lo, const KsModulus& md) {
+  const u64 v = shoup_lazy(hi, md.a, md.b, md.q) + barrett64_lazy(lo, md.q, md.mu);
+  return csub(csub(v, md.q << 1), md.q);
+}
+
+// A thread owns one slot l of one modulus e and both key components: per element it reads the permuted digits and the
+// diagonal word once, sums the digit products unreduced (the bound of ks_mac_digits_per_launch), reduces, and adds
+// w times that into a second 128-bit sum, which at most 64 canonical products cannot wrap for q < 2^61.  The
+// per-element products are never written.
+__global__ void __launch_bounds__(kThreads)
+    ks_weighted_mac_kernel(u64* acc, const u64* ops, u64 ops_stride, const __grid_constant__ WeightedMacElts elts,
+                           u64 n, u64 jcount, u64 num_elts, u64 key_modulus_size, u64 count,
+                           const __grid_constant__ KsModuli mods, int accumulate) {
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= n * count) return;
+  const u64 e = g / n, l = g - e * n;
+  const KsModulus& md = mods.m[e];
+  const u64 key_off = n * md.c + l, comp = key_modulus_size * n;
+  const int log_n = __ffsll((long long)n) - 1;
+  const u64* op = ops + e * ops_stride;
+  u64 lo0 = 0, hi0 = 0, lo1 = 0, hi1 = 0;
+  // (element, digit) pairs and digits fit 32 bits: at most kParamBlock of each
+  for (unsigned r = 0, kp = 0; r < (unsigned)num_elts; ++r) {
+    const u64* d = op + ntt_source((unsigned)l, elts.elt[r], (unsigned)(2 * n - 1), log_n);
+    u64 a0 = 0, b0 = 0, a1 = 0, b1 = 0;
+    for (unsigned j = 0; j < (unsigned)jcount; ++j, ++kp) {
+      const u64 x = d[j * n];
+      const u64* key = elts.key[kp] + key_off;
+      mac128(x, __ldcs(key), a0, b0);
+      mac128(x, __ldcs(key + comp), a1, b1);
+    }
+    const u64 w = elts.diag[r][e * n + l];
+    mac128(w, reduce128(b0, a0, md), lo0, hi0);
+    mac128(w, reduce128(b1, a1, md), lo1, hi1);
+  }
+  u64 v0 = reduce128(hi0, lo0, md), v1 = reduce128(hi1, lo1, md);
+  u64* out = acc + e * 2 * n + l;
+  if (accumulate) {
+    v0 = csub(v0 + out[0], md.q);
+    v1 = csub(v1 + out[n], md.q);
+  }
+  out[0] = v0;
+  out[n] = v1;
+}
+
+// A thread owns one slot l of one data limb: w_r times c0 at pi_r(l) for every element, and times c1 at l for the
+// identity terms, each sum in 128 bits (at most 64 canonical products) and reduced once.
+__global__ void __launch_bounds__(kThreads)
+    ks_permuted_sum_kernel(u64* result, const u64* ct, u64 n, u64 level, u64 i0, u64 count,
+                           const __grid_constant__ PermutedSumElts elts, u64 num_elts,
+                           const __grid_constant__ KsModuli mods, int accumulate) {
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= n * count) return;
+  const u64 e = g / n, l = g - e * n;
+  const KsModulus& md = mods.m[e];
+  const int log_n = __ffsll((long long)n) - 1;
+  const u64* c0 = ct + (i0 + e) * n;
+  const u64 c1 = elts.identity ? ct[(level + i0 + e) * n + l] : 0;
+  u64 lo0 = 0, hi0 = 0, lo1 = 0, hi1 = 0;
+  for (u64 r = 0; r < num_elts; ++r) {
+    const u64 w = elts.diag[r][e * n + l];
+    mac128(w, c0[ntt_source((unsigned)l, elts.elt[r], (unsigned)(2 * n - 1), log_n)], lo0, hi0);
+    if ((elts.identity >> r) & 1) mac128(w, c1, lo1, hi1);
+  }
+  u64 v0 = reduce128(hi0, lo0, md), v1 = reduce128(hi1, lo1, md);
+  u64* out = result + (i0 + e) * n + l;
+  if (accumulate) {
+    v0 = csub(v0 + out[0], md.q);
+    v1 = csub(v1 + out[level * n], md.q);
+  }
+  out[0] = v0;
+  out[level * n] = v1;
+}
+
 // The two halves of the mod-down by the last modulus, shared by the kernels below.
 // round: a coefficient of the last modulus's part (coefficient form, [0, 2 q_last)) rounded and moved into modulus q:
 //   t = (x + q_last/2) mod q_last;  out = (t mod q) + add,  add = q - (q_last/2 mod q);  out < 2q
@@ -279,6 +362,25 @@ cudaError_t launch_ks_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPo
   kernel<<<blocks_for(kcc * n * count), kThreads, 0, stream>>>(prod, ops, ops_stride, keys, n, jcount, kcc,
                                                               key_modulus_size, count, mods, accumulate,
                                                               (unsigned)galois_elt);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ks_weighted_mac(u64* acc, const u64* ops, u64 ops_stride, const WeightedMacElts& elts, u64 n,
+                                   u64 jcount, u64 num_elts, u64 key_modulus_size, u64 count, const KsModuli& mods,
+                                   bool accumulate, cudaStream_t stream) {
+  ks_weighted_mac_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(acc, ops, ops_stride, elts, n, jcount,
+                                                                        num_elts, key_modulus_size, count, mods,
+                                                                        accumulate);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ks_permuted_sum(u64* result, const u64* ct, u64 n, u64 level, u64 i0, u64 count,
+                                   const PermutedSumElts& elts, u64 num_elts, const KsModuli& mods, bool accumulate,
+                                   cudaStream_t stream) {
+  ks_permuted_sum_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(result, ct, n, level, i0, count, elts,
+                                                                        num_elts, mods, accumulate);
   count_launch();
   return cudaGetLastError();
 }

@@ -696,6 +696,38 @@ inline void KeySwitchHybrid(uint64_t* result, const uint64_t* target, uint64_t n
   b200_detail::Throw(hexl_b200_key_switch_hybrid(result, target, n, level_size, q_size, p_size, digit_size,
                                                  key_component_count, moduli, keys.Handle(), batch, stream));
 }
+
+// extension: hoisted rotations with hybrid keys -- each of `batch` ciphertexts (2 x level_size limbs) rotated by every
+// galois_elts[r] with *galois_keys[r] (hybrid keys, key_component_count 2), its mod-up done once for all elements;
+// rotation r of ciphertext c goes to results + (c * num_elts + r) * 2 * level_size * n
+// (hexl_b200_apply_galois_key_switch_hybrid_hoisted has the formula).  Not bit-identical to ApplyGalois followed by
+// KeySwitchHybrid for g != 1 (signed digit lift, the same noise bound).
+inline void ApplyGaloisKeySwitchHybridHoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                              uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                              uint64_t digit_size, const uint64_t* moduli,
+                                              const KeySwitchKeys* const* galois_keys, const uint64_t* galois_elts,
+                                              uint64_t num_elts, uint64_t batch = 1, void* stream = nullptr) {
+  std::vector<const hexl_b200_keys*> handles(num_elts);
+  for (uint64_t r = 0; r < num_elts; ++r) handles[r] = galois_keys[r] ? galois_keys[r]->Handle() : nullptr;
+  b200_detail::Throw(hexl_b200_apply_galois_key_switch_hybrid_hoisted(results, ciphertexts, n, level_size, q_size,
+                                                                      p_size, digit_size, moduli, handles.data(),
+                                                                      galois_elts, num_elts, batch, stream));
+}
+
+// extension: sum_r w_r (.) Rot_{g_r}(ct) with hybrid keys and one mod-down for the whole sum, for each of `batch`
+// ciphertexts; diagonals holds num_elts x (level_size + p_size) x n words in NTT form, and a null galois_keys[r] with
+// galois_elts[r] = 1 is an identity term (hexl_b200_linear_transform_hybrid has the formula).
+inline void LinearTransformHybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                                  uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                  const KeySwitchKeys* const* galois_keys, const uint64_t* galois_elts,
+                                  uint64_t num_elts, const uint64_t* diagonals, uint64_t batch = 1,
+                                  void* stream = nullptr) {
+  std::vector<const hexl_b200_keys*> handles(num_elts);
+  for (uint64_t r = 0; r < num_elts; ++r) handles[r] = galois_keys[r] ? galois_keys[r]->Handle() : nullptr;
+  b200_detail::Throw(hexl_b200_linear_transform_hybrid(result, ciphertexts, n, level_size, q_size, p_size, digit_size,
+                                                       moduli, handles.data(), galois_elts, num_elts, diagonals,
+                                                       batch, stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

@@ -407,6 +407,65 @@ int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64
                                 uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
                                 const uint64_t* moduli, const hexl_b200_keys* keys, uint64_t batch, void* stream);
 
+/* Hoisted rotations with hybrid keys (extension; OpenFHE's EvalFastRotation with KeySwitchHYBRID): each of `batch`
+ * ciphertexts rotated by each of num_elts Galois elements, its mod-up done ONCE for every element.  The moduli, digits
+ * and shape rules are those of hexl_b200_key_switch_hybrid with key_component_count = 2; galois_keys[r] is a hybrid key
+ * handle (dnum = ceil(q_size / digit_size) buffers of 2 x (q_size + p_size) x n words) that switches s(X^g) back to s
+ * for g = galois_elts[r].  Ciphertext c is two components of l = level_size limbs in NTT form, canonical, at
+ * ciphertexts + c * 2 * l * n; its rotation by galois_elts[r] is written to results + (c * num_elts + r) * 2 * l * n.
+ * Out of place: ciphertexts is not modified.  With the mod-up D_{d,m} and ModDown_P of hexl_b200_key_switch_hybrid
+ * applied to t = c1:
+ *   prod^r_{m,k} = sum_d pi_g(D_{d,m}) (.) K_r[d][k][slot(m)]  mod m,  every m in B
+ *   out_r        = [sigma_g(c0), 0] + ModDown_P(prod^r)
+ * with pi_g / sigma_g the NTT-form automorphism of hexl_b200_apply_galois.  Permuting the converted digits lifts digit
+ * d to the signed integers sigma_g(X + u Q_d) instead of sigma_g applied after an unsigned lift, so for g != 1 this is
+ * NOT bit-identical to the chain hexl_b200_apply_galois + hexl_b200_key_switch_hybrid; the lift is below alpha Q_d in
+ * magnitude either way, so the decryption noise bound is the same.  For g = 1 it is that chain bit for bit, and with
+ * digit_size = 1 and p_size = 1 it is hexl_b200_apply_galois_key_switch_hoisted bit for bit (decomp = l,
+ * key_modulus_size = q_size + 1, modswitch factors p^-1 mod q_i).  Elements may repeat.  num_elts = 0 or batch = 0
+ * does nothing.  HEXL_B200_ERR_INVALID_ARG on the shape rules of hexl_b200_key_switch_hybrid applied to every handle
+ * (null, another shape, or sharded by modulus), for an element outside the rules of hexl_b200_apply_galois, and when
+ * results overlaps ciphertexts.  Inputs are checked below their modulus under hexl_b200_set_debug(1).  On the device,
+ * per ciphertext: the mod-up of hexl_b200_key_switch_hybrid once; per element, one automorphism launch of c0 into the
+ * output, a memset of the output's c1, its multiply-accumulates and its mod-down.  Library scratch: one round of
+ * converted digits plus num_elts x (l + p_size) x 2 x n words of products.  Device calls capture into a CUDA graph
+ * once the transforms are warm.  Host buffers: each ciphertext crosses PCIe in once and its rotations come back on the
+ * same staging stream, split by ciphertext over the devices of hexl_b200_set_host_devices where every handle holds a
+ * copy. */
+int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                                     uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                                     uint64_t digit_size, const uint64_t* moduli,
+                                                     const hexl_b200_keys* const* galois_keys,
+                                                     const uint64_t* galois_elts, uint64_t num_elts, uint64_t batch,
+                                                     void* stream);
+
+/* Linear transform with hybrid keys (extension; Lattigo's MultiplyByDiagMatrix, OpenFHE's EvalLinearTransform): the
+ * plaintext-matrix x ciphertext product in diagonal form, sum_r w_r (.) Rot_{g_r}(ct), for each of `batch`
+ * ciphertexts, with ONE mod-down for the whole sum.  Arguments, layouts and rules as for
+ * hexl_b200_apply_galois_key_switch_hybrid_hoisted, plus diagonals: num_elts x (l + p_size) x n words in NTT form,
+ * canonical; limb i < l of diagonal r is under q_i and limb l + j under p_j.  Ciphertext c goes to
+ * result + c * 2 * l * n.  With prod^r of the hoisted call and I the identity terms (g_r = 1 with galois_keys[r] null,
+ * which add w_r (.) ct and switch no key):
+ *   acc_{m,k} = sum_{r not in I} w_{r,m} (.) prod^r_{m,k}  mod m,  every m in B
+ *   result    = [sum_r w_r (.) sigma_{g_r}(c0), sum_{r in I} w_r (.) c1] + ModDown_P(acc)
+ * canonical; when every term is an identity term there is no key switch and no ModDown term.  Weighting in the
+ * extended basis and rounding once is what makes the single mod-down possible, so the result is NOT the sum of
+ * weighted hoisted rotations bit for bit (that rounds once per element); with one element and every diagonal word 1 it
+ * equals hexl_b200_apply_galois_key_switch_hybrid_hoisted bit for bit.  A null handle for g != 1 is refused
+ * (HEXL_B200_ERR_INVALID_ARG), as are the refusals of the hoisted call and a result overlapping the ciphertexts or the
+ * diagonals.  Elements may repeat.  num_elts = 0 or batch = 0 does nothing.  Inputs, the diagonals included, are
+ * checked below their modulus under hexl_b200_set_debug(1).  On the device, per ciphertext: one weighted permuted-sum
+ * launch per chunk of 64 elements and block of 64 data moduli (stores [sum w sigma(c0), sum_I w c1]); then, when some
+ * element has keys, the mod-up once, per round of moduli one weighted multiply-accumulate launch per chunk of
+ * (element, digit) pairs (at most 64 pairs, each launch adding into one accumulator of (l + p_size) x 2 x n words
+ * without writing per-element products), and one mod-down.  Device calls capture into a CUDA graph once the transforms
+ * are warm.  Host buffers: the diagonals go to each device once per call, before its first ciphertext; the ciphertexts
+ * are pipelined and split over the devices as for the hoisted call. */
+int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                                      uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                      const hexl_b200_keys* const* galois_keys, const uint64_t* galois_elts,
+                                      uint64_t num_elts, const uint64_t* diagonals, uint64_t batch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
