@@ -54,6 +54,19 @@ static void build_tables(hexl_b200_ntt* h) {
   h->inv_n_w = make_twiddle(nt::mul_mod(inv_n, h->inv_tree[1].w, q), q);
 }
 
+// A tree in the order of its device copy (internal.h): the deepest four levels lane-major where the rows are 4096
+// points, node order elsewhere.
+static std::vector<Twiddle> device_order(const std::vector<Twiddle>& tree, int log_n) {
+  std::vector<Twiddle> out(tree);
+  if (!twiddle_lanes_major(log_n)) return out;
+  for (int j = 0; j < 4; ++j) {
+    const uint64_t level = 1ull << (log_n - 4 + j);
+    for (uint64_t i = 0; i < level; ++i)
+      out[level + lane_major((unsigned)(i >> j), (unsigned)(i & ((1u << j) - 1)), j)] = tree[level + i];
+  }
+  return out;
+}
+
 int device_tables(hexl_b200_ntt* h, int dev, NttDeviceTables* out, cudaStream_t user_stream) {
   std::lock_guard<std::mutex> lk(h->mu);
   auto it = h->dev.find(dev);
@@ -76,15 +89,16 @@ int device_tables(hexl_b200_ntt* h, int dev, NttDeviceTables* out, cudaStream_t 
     }                                                     \
   } while (0)
     const size_t bytes = h->n * sizeof(Twiddle);
+    const std::vector<Twiddle> fwd = device_order(h->fwd_tree, h->log_n), inv = device_order(h->inv_tree, h->log_n);
     CU_T(cudaMalloc(&d.fwd, bytes));
     CU_T(cudaMalloc(&d.inv, bytes));
-    CU_T(cudaMemcpy(d.fwd, h->fwd_tree.data(), bytes, cudaMemcpyHostToDevice));
-    CU_T(cudaMemcpy(d.inv, h->inv_tree.data(), bytes, cudaMemcpyHostToDevice));
+    CU_T(cudaMemcpy(d.fwd, fwd.data(), bytes, cudaMemcpyHostToDevice));
+    CU_T(cudaMemcpy(d.inv, inv.data(), bytes, cudaMemcpyHostToDevice));
     if (h->q < kSmallModulusLimit) {
       std::vector<Twiddle32> f32(h->n), i32(h->n);
       for (uint64_t k = 0; k < h->n; ++k) {
-        f32[k] = make_twiddle32(h->fwd_tree[k].w, h->q);
-        i32[k] = make_twiddle32(h->inv_tree[k].w, h->q);
+        f32[k] = make_twiddle32(fwd[k].w, h->q);
+        i32[k] = make_twiddle32(inv[k].w, h->q);
       }
       CU_T(cudaMalloc(&d.fwd32, h->n * sizeof(Twiddle32)));
       CU_T(cudaMalloc(&d.inv32, h->n * sizeof(Twiddle32)));

@@ -38,6 +38,12 @@ cudaError_t launch_eltwise(EltOp op, const EltParams& p, cudaStream_t stream);
 //           ntt-internal.cpp:144-154; here they keep the tree indexing)
 // The children of node k are 2k and 2k+1; a sub-transform rooted at node b uses
 // node b*2^s + i for its stage s, group i.
+// Device copies are in node order except where twiddle_lanes_major(log_n): there, entry i of each of the deepest
+// four tree levels (depth log_n - 4 + j, j = 0..3) is stored at lane_major(i >> j, i & (2^j - 1), j) of that level
+// instead of at i.  Those levels are read only by the last register pass of the 4096-point rows (reg_stages, LB = 0),
+// where global thread-row U = (row in polynomial) * 256 + u reads entry U * 2^j + g of level j for g < 2^j: in node
+// order adjacent lanes are 2^j entries apart, in this order they are adjacent for every g.  The host trees (and the
+// getters of the C ABI) keep node order.
 //
 // NttDeviceParams: what a kernel needs to know about one (N, q), resident in device
 // memory next to the tables, so that ONE launch can transform polynomials of several
@@ -68,6 +74,18 @@ struct NttDeviceTables {
   const NttDeviceParams* dparams;  // the same facts as a device-resident record
 };
 constexpr u64 kSmallModulusLimit = 1ull << 30;  // below: 4q < 2^32, the 32-bit kernels apply
+
+// log2 of the row length used for a transform of size 2^log_n: the whole polynomial up to 8192 coefficients, else
+// 4096-point rows after the column passes
+constexpr int pick_row_log(int log_n) { return log_n <= 13 ? log_n : 12; }
+// The transforms whose rows are 4096 points store their deepest four twiddle levels lane-major.
+constexpr bool twiddle_lanes_major(int log_n) { return pick_row_log(log_n) == 12; }
+// Position inside level j (of the deepest four) of the entry that thread-row U reads for group g < 2^j: warps of
+// 32 thread-rows own blocks of 32 * 2^j entries, g-major inside the block.  The three terms occupy disjoint bits, so
+// lane_major(U, g, j) = lane_major(U, 0, j) + (g << 5): the kernels add g << 5 to the address as an immediate offset.
+__host__ __device__ constexpr unsigned lane_major(unsigned U, unsigned g, int j) {
+  return ((U >> 5) << (j + 5)) + (g << 5) + (U & 31);
+}
 
 // result/operand: `batch` polynomials back to back on the current device.
 cudaError_t launch_ntt_forward(const NttDeviceTables& t, u64* result, const u64* operand,

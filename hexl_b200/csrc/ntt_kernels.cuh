@@ -508,6 +508,9 @@ __device__ __forceinline__ void reg_stages(typename Ar<MODE>::E (&v)[16], unsign
     auto fetch = [&](int g) {
       if constexpr (PT::kShared)
         return sroot[(8 >> eb) + g];                // local node 2^s' + g, s' = 3 - eb
+      else if constexpr (LOGC == 12 && LB == 0)
+        // last pass of a 4096-point row: level 3 - beta of the deepest four, stored lane-major (internal.h)
+        return ld_tw(tw + (base << (LOGC - 1 - beta)) + lane_major(u, 0, 3 - beta) + (g << 5));
       else
         return ld_tw(tw + (base << (LOGC - 1 - beta)) + ((u64)(u >> LB) << (LB + 3 - beta)) + g);
     };
@@ -1334,10 +1337,6 @@ cudaError_t launch_pipelined(u64 units, cudaStream_t stream, Args... args) {
   scratch_free_async(state, stream);
   return e;
 }
-
-// log2 of the row length used for a transform of size 2^log_n: the whole polynomial up to 8192 coefficients, else
-// 4096-point rows after the column passes
-inline int pick_row_log(int log_n) { return log_n <= 13 ? log_n : 12; }
 
 inline int pick_mode(u64 q) {
   if (q < kSmallModulusLimit) return kSmall;
