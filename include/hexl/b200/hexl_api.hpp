@@ -22,9 +22,11 @@
 
 #include <cmath>
 #include <cstdlib>
+#include <functional>
 #include <limits>
 #include <memory>
 #include <mutex>
+#include <shared_mutex>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -46,6 +48,11 @@
 #ifndef HEXL_VLOG
 #define HEXL_VLOG(N, rest) \
   {}
+#endif
+// hexl/include/hexl/util/gcc.hpp:55-56
+#ifndef HEXL_LOOP_UNROLL_4
+#define HEXL_LOOP_UNROLL_4 _Pragma("GCC unroll 4")
+#define HEXL_LOOP_UNROLL_8 _Pragma("GCC unroll 8")
 #endif
 
 namespace intel {
@@ -534,15 +541,21 @@ inline void EltwiseCmpSubMod(uint64_t* result, const uint64_t* operand1, uint64_
       hexl_b200_eltwise_cmp_sub_mod(result, operand1, n, modulus, static_cast<int>(cmp), bound, diff, stream));
 }
 
-// Montgomery-form helpers.  In the reference these are internal AVX-512 templates on <BitShift, r>
+// Montgomery-form helpers.  In the reference the element-wise ones are internal AVX-512 templates on <BitShift, r>
 // (hexl/eltwise/eltwise-reduce-mod-avx512.hpp:156-352); here r is a run-time argument and BitShift is 64.
 inline uint64_t HenselLemma2adicRoot(uint32_t r, uint64_t q) { return hexl_b200_hensel_lemma_2adic_root(r, q); }
+#if defined(__SIZEOF_INT128__)
+// number-theory.hpp:269-301, inline like the reference's, for every r with q < 2^r <= 2^63: T * 2^-r mod q for
+// T = T_hi * 2^64 + T_lo < q * 2^r, by REDC on the 128-bit sum T + m * q (below 2^128 because q * 2^r < 2^127).
 template <int BitShift>
-inline uint64_t MontgomeryReduce(uint64_t T_hi, uint64_t T_lo, uint64_t q, int r, uint64_t /*mod_R_msk*/,
+inline uint64_t MontgomeryReduce(uint64_t T_hi, uint64_t T_lo, uint64_t q, int r, uint64_t mod_R_msk,
                                  uint64_t inv_mod) {
   static_assert(BitShift == 64, "only the 64-bit form exists on the GPU path");
-  return hexl_b200_montgomery_reduce(T_hi, T_lo, q, r, inv_mod);
+  const uint64_t m = ((T_lo & mod_R_msk) * inv_mod) & mod_R_msk;
+  const uint64_t s = static_cast<uint64_t>((((uint128_t(T_hi) << 64) | T_lo) + uint128_t(m) * q) >> r);
+  return s >= q ? s - q : s;
 }
+#endif
 inline void EltwiseMontReduceMod(uint64_t* result, const uint64_t* a, const uint64_t* b, uint64_t n, uint64_t modulus,
                                  int r, uint64_t neg_inv_mod, void* stream = nullptr) {
   b200_detail::Throw(hexl_b200_eltwise_mont_reduce_mod(result, a, b, n, modulus, r, neg_inv_mod, stream));
@@ -561,6 +574,35 @@ inline void EltwiseMontgomeryFormOut(uint64_t* result, const uint64_t* a, uint64
 // NTT& into a process-wide map; here the cache lives behind the ABI and a cheap
 // handle copy is returned.
 inline NTT GetNTT(size_t N, uint64_t modulus) { return NTT::FromCache(N, modulus); }
+
+// hexl/include/hexl/experimental/seal/ntt-cache.hpp:13-25: the key hash of the reference's cache map
+struct HashPair {
+  template <class T1, class T2>
+  std::size_t operator()(const std::pair<T1, T2>& p) const {
+    return hash_combine(std::hash<T1>{}(p.first), std::hash<T2>{}(p.second));
+  }
+  static std::size_t hash_combine(std::size_t lhs, std::size_t rhs) {
+    return lhs ^ (rhs + 0x9e3779b9 + (lhs << 6) + (lhs >> 2));
+  }
+};
+
+// hexl/include/hexl/experimental/seal/locks.hpp: the reader-writer lock the reference's cache is guarded by
+using Lock = std::shared_mutex;
+using WriteLock = std::unique_lock<Lock>;
+using ReadLock = std::shared_lock<Lock>;
+class RWLock {
+ public:
+  RWLock() = default;
+  RWLock(const RWLock&) = delete;
+  RWLock& operator=(const RWLock&) = delete;
+  ReadLock AcquireRead() { return ReadLock(m_mutex); }
+  WriteLock AcquireWrite() { return WriteLock(m_mutex); }
+  ReadLock TryAcquireRead() noexcept { return ReadLock(m_mutex, std::try_to_lock); }
+  WriteLock TryAcquireWrite() noexcept { return WriteLock(m_mutex, std::try_to_lock); }
+
+ private:
+  Lock m_mutex{};
+};
 
 // hexl/include/hexl/experimental/seal/dyadic-multiply.hpp:26
 // Exact for every modulus below 2^62, like EltwiseMultMod: for 62-bit moduli the products take the second conditional
@@ -585,6 +627,22 @@ inline void KeySwitch(uint64_t* result, const uint64_t* t_target_iter_ptr, uint6
                                           rns_modulus_size, key_component_count, moduli, k_switch_keys,
                                           modswitch_factors, stream));
 }
+
+// hexl/include/hexl/experimental/seal/{dyadic-multiply,key-switch}-internal.hpp, which the reference's hexl.hpp
+// includes: the same operations under intel::hexl::internal
+namespace internal {
+inline void DyadicMultiply(uint64_t* result, const uint64_t* operand1, const uint64_t* operand2, uint64_t n,
+                           const uint64_t* moduli, uint64_t num_moduli) {
+  intel::hexl::DyadicMultiply(result, operand1, operand2, n, moduli, num_moduli);
+}
+inline void KeySwitch(uint64_t* result, const uint64_t* t_target_iter_ptr, uint64_t n, uint64_t decomp_modulus_size,
+                      uint64_t key_modulus_size, uint64_t rns_modulus_size, uint64_t key_component_count,
+                      const uint64_t* moduli, const uint64_t** k_switch_keys, const uint64_t* modswitch_factors,
+                      const uint64_t* root_of_unity_powers_ptr = nullptr) {
+  intel::hexl::KeySwitch(result, t_target_iter_ptr, n, decomp_modulus_size, key_modulus_size, rns_modulus_size,
+                         key_component_count, moduli, k_switch_keys, modswitch_factors, root_of_unity_powers_ptr);
+}
+}  // namespace internal
 
 // extension: rescale by the last RNS modulus, SEAL's RNSTool::divide_and_round_q_last(_ntt)_inplace batched over
 // `count` polynomials of rns_modulus_size limbs each (hexl_b200_divide_and_round_q_last in include/hexl_b200.h has the

@@ -1,0 +1,3 @@
+// Drop-in for the reference header of the same path; everything lives in hexl/b200/hexl_api.hpp.
+#pragma once
+#include "../../b200/hexl_api.hpp"
