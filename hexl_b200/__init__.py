@@ -133,6 +133,8 @@ _sig("hexl_b200_apply_galois_key_switch_hybrid_hoisted", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _u64, _vp])
 _sig("hexl_b200_linear_transform_hybrid", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp])
+_sig("hexl_b200_multiply_relinearize_hybrid", _int,
+     [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -680,4 +682,23 @@ def LinearTransformHybrid(result, ciphertexts, n, level_size, q_size, p_size, di
     _check(_lib.hexl_b200_linear_transform_hybrid(rp, cp, n, level_size, q_size, p_size, digit_size, mods.ctypes.data,
                                                   keys, elts.ctypes.data, elts.size, dp, batch,
                                                   _stream(stream, rc or cc or dc)))
+    return result
+
+
+def MultiplyRelinearizeHybrid(result, ct1, ct2, n, level_size, q_size, p_size, digit_size, moduli,
+                              relin_keys: KeySwitchKeys, rescale=False, batch=1, stream=None):
+    """ct1 x ct2 relinearized with hybrid keys (hexl_b200_multiply_relinearize_hybrid): pair c reads
+    ct1[c * 2*level_size*n:] and ct2[c * 2*level_size*n:] and its product is stored at result[c * 2*l'*n:],
+    l' = level_size - rescale.  relin_keys switches s^2 to s (key_component_count 2).  rescale=True divides by the last
+    limb in the same mod-down (one rounding, not bit-identical to a separate DivideAndRoundQLast).  ct1 may be ct2."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); ap, an, ac = _buf(ct1); bp, bn, bc = _buf(ct2)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size)
+    _need("result", rn, batch * 2 * (level_size - int(bool(rescale))) * n)
+    _need("ct1", an, batch * per); _need("ct2", bn, batch * per)
+    _check(_lib.hexl_b200_multiply_relinearize_hybrid(rp, ap, bp, n, level_size, q_size, p_size, digit_size,
+                                                      mods.ctypes.data,
+                                                      relin_keys._h if relin_keys is not None else None,
+                                                      int(bool(rescale)), batch, _stream(stream, rc or ac or bc)))
     return result

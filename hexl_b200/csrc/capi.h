@@ -1,6 +1,6 @@
 // What the host sources of the C ABI (include/hexl_b200.h) share: capi.cu (library state, staging, scratch pool),
 // capi_ntt.cu, capi_eltwise.cu, capi_keyswitch.cu (key switch, key handles, rescale), capi_galois.cu and
-// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations with hybrid keys).
+// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations and multiplication with hybrid keys).
 // Host-side responsibilities, all one-off or O(1) per call:
 //   * argument validation mirroring the reference's HEXL_CHECKs,
 //   * NTT handle = (N, q, root) -> twiddle tables, built on the host exactly as
@@ -403,9 +403,11 @@ int key_switch_elts_on_device(int dev, uint64_t* const* results, const uint64_t*
                               const uint64_t* modswitch, cudaStream_t s);
 // run(dev, device result block, device input block, the key handles' copies on dev, stream): one ciphertext's switch.
 // prepare(dev) (optional) runs once on each device of the split, with it current, before its first ciphertext.
+// in2 (optional): a second input of in_words words per ciphertext, copied into the input block after the first.
 using HostSwitch = std::function<int(int, uint64_t*, uint64_t*, const uint64_t* const* const*, cudaStream_t)>;
 int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, const uint64_t* in, uint64_t in_words,
                           uint64_t buf_words, const hexl_b200_keys* const* keys, uint64_t num_keys, uint64_t batch,
-                          const HostSwitch& run, const std::function<int(int)>& prepare = nullptr);
+                          const HostSwitch& run, const std::function<int(int)>& prepare = nullptr,
+                          const uint64_t* in2 = nullptr);
 
 }  // namespace hexl_b200

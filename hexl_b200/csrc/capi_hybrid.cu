@@ -1,6 +1,7 @@
 // Hybrid key switching (OpenFHE's KeySwitchHYBRID): digits of up to 64 data moduli and up to 64 special primes, the
 // mod-up and the mod-down by fast base conversion (rns.cu); the base conversion on its own; and the rotations with
-// hybrid keys: hoisted, and the diagonal-weighted sum of rotations under one mod-down (the linear transform).
+// hybrid keys: hoisted, and the diagonal-weighted sum of rotations under one mod-down (the linear transform); and the
+// ciphertext product relinearized with hybrid keys, its rescale optionally merged into the mod-down.
 #include <cstdio>
 #include <numeric>
 
@@ -72,11 +73,13 @@ static int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t 
 // B = {q_0..q_{l-1}, p_0..p_{K-1}} in that order and bmods their moduli.  The target's limbs go back to coefficients
 // once; then, per round of moduli of B, every digit is converted into each modulus of the round and lazily
 // transformed into ops ([e][d][n], D x n words between moduli), and mac(b0, cnt, ops, slots) multiplies them with the
-// keys: moduli [b0, b0 + cnt) of B, slots[e] the key slot of modulus b0 + e.  Scratch comes from ws.
+// keys: moduli [b0, b0 + cnt) of B, slots[e] the key slot of modulus b0 + e.  Scratch comes from ws.  mul (nullptr:
+// none; laid out like target) makes the target the point-wise product target (.) mul, multiplied in the first inverse
+// transform's load, so the product is never written.
 template <class Mac>
 static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t level, uint64_t q_size,
                          uint64_t p_size, uint64_t alpha, const CachedNtts& h, const uint64_t* bmods, Scratch& ws,
-                         Mac&& mac, cudaStream_t s) {
+                         Mac&& mac, cudaStream_t s, const uint64_t* mul = nullptr) {
   const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size;
   // moduli handled per round of the mod-up: bounded by the parameter block and by ~256 MiB of scratch
   const uint64_t per_mod = D * n;
@@ -86,7 +89,8 @@ static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t l
   if (int rc = ws.get(&t_coef, level * n)) return rc;
   if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;  // [e][d][n]
   // 1. the target's limbs back to coefficients, canonical
-  if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s)) return rc;
+  if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s, nullptr, false, mul))
+    return rc;
   // 2. mod-up: every digit converted into each modulus of the round, lazily transformed, multiplied with the keys.
   //    (A digit's own limbs are converted and transformed again like the others: NTT(INTT(t)) = t.)
   for (uint64_t b0 = 0; b0 < nb; b0 += ichunk) {
@@ -107,9 +111,12 @@ static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t l
 
 // Step 3, the mod-down by P, of one switch's products prod ([b][k][n] over the moduli of B, kcc components): the
 // special limbs back to coefficients in place, rounded and converted into each data modulus, transformed, and
-// (prod - that) * P^-1 accumulated into result (kcc x level x n).  tmp holds min(level, 64) x kcc x n words.
+// (prod - that) * P^-1 accumulated into result (kcc x level x n), or stored when !accumulate.  tmp holds
+// min(level, 64) x kcc x n words.  P is the product of the p_size moduli of B after the first `level`: called with
+// level - 1 and p_size + 1 it divides by q_{level-1} P as well, the mod-down merged with the rescale.
 static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* tmp, uint64_t n, uint64_t level,
-                           uint64_t p_size, uint64_t kcc, const CachedNtts& h, const uint64_t* bmods, cudaStream_t s) {
+                           uint64_t p_size, uint64_t kcc, const CachedNtts& h, const uint64_t* bmods, bool accumulate,
+                           cudaStream_t s) {
   uint64_t* special = prod + level * kcc * n;  // [j][k][n]
   if (int rc = ntt_multi_on_device(false, dev, h.data() + level, p_size, special, special, 1, kcc, s)) return rc;
   for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
@@ -126,7 +133,8 @@ static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* 
       const Twiddle f = make_twiddle(nt::inverse_mod(P, q), q);
       fin.m[e] = KsModulus{q, nt::multiply_factor(1, 64, q), f.w, f.wp, 0};
     }
-    const cudaError_t e = launch_ks_finish(result, prod + i0 * kcc * n, tmp, n, kcc, level, i0, cnt, fin, false, true, s);
+    const cudaError_t e =
+        launch_ks_finish(result, prod + i0 * kcc * n, tmp, n, kcc, level, i0, cnt, fin, false, accumulate, s);
     if (e != cudaSuccess) return cuda_fail(e, "hybrid mod-down: finish launch");
   }
   return 0;
@@ -155,7 +163,8 @@ static int key_switch_hybrid_elts_on_device(int dev, uint64_t* const* results, c
                              s))
     return rc;
   for (uint64_t r = 0; r < elts; ++r)
-    if (int rc = hybrid_mod_down(dev, results[r], prod + r * nb * kcc * n, tmp, n, level, p_size, kcc, h, bmods, s))
+    if (int rc =
+            hybrid_mod_down(dev, results[r], prod + r * nb * kcc * n, tmp, n, level, p_size, kcc, h, bmods, true, s))
       return rc;
   return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
 }
@@ -248,7 +257,52 @@ static int linear_transform_hybrid_on_device(int dev, uint64_t* result, const ui
     return 0;
   };
   if (int rc = hybrid_mod_up(dev, ct + level * n, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s)) return rc;
-  return hybrid_mod_down(dev, result, acc, tmp, n, level, p_size, 2, h, bmods, s);
+  return hybrid_mod_down(dev, result, acc, tmp, n, level, p_size, 2, h, bmods, true, s);
+}
+
+// The product of two ciphertexts ct1 = (a0, a1) and ct2 = (b0, b1) (each two components of level limbs, NTT form,
+// device memory), relinearized with keys (digit d's key buffer keys[d]) and stored into result (2 x (level - rescale)
+// limbs): the mod-up of a1 (.) b1, multiplied in the mod-up's first inverse transform; per round, the relinearization
+// multiply-accumulate, whose storing launch adds [P] (a0 b0, a0 b1 + a1 b0) on the data moduli; and one mod-down,
+// by P or, with rescale, by q_{level-1} P (q_{level-1} is the limb of B right before the special limbs).  Scratch: one
+// round of transformed digits plus (level + K) x 2 x n words of products.
+static int multiply_relinearize_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct1, const uint64_t* ct2,
+                                                 uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size,
+                                                 uint64_t alpha, bool rescale, const CachedNtts& h,
+                                                 const uint64_t* bmods, const uint64_t* const* keys, cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, comp = level * n;
+  Scratch ws(s);
+  uint64_t *prod = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&prod, nb * 2 * n)) return rc;                                       // [b][k][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * 2 * n)) return rc;  // [i][k][n], one block
+  auto mac = [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) -> int {
+    const KsModuli mods = ks_mac_moduli(bmods + b0, slots, cnt);
+    RelinTensor tensor{};
+    tensor.ct1 = ct1 + b0 * n;
+    tensor.ct2 = ct2 + b0 * n;
+    tensor.comp = comp;
+    tensor.data = b0 < level ? std::min(cnt, level - b0) : 0;
+    for (uint64_t e = 0; e < tensor.data; ++e) {
+      const uint64_t q = bmods[b0 + e];
+      uint64_t P = 1 % q;
+      for (uint64_t j = 0; j < p_size; ++j) P = mul_mod128(P, bmods[level + j] % q, q);
+      tensor.p[e] = P;
+    }
+    const uint64_t jc = std::min(ks_mac_digits_per_launch(mods, cnt), D);
+    for (uint64_t j0 = 0; j0 < D; j0 += jc) {  // key pointers ride in the kernel parameters
+      const uint64_t jcnt = std::min(jc, D - j0);
+      KeyPointers kp;
+      for (uint64_t j = 0; j < jcnt; ++j) kp.p[j] = keys[j0 + j];
+      const cudaError_t e = launch_ks_relin_mac(prod + b0 * 2 * n, ops + j0 * n, D * n, kp, n, jcnt, kms, cnt, mods,
+                                                tensor, j0 != 0, s);
+      if (e != cudaSuccess) return cuda_fail(e, "MultiplyRelinearizeHybrid: multiply-accumulate launch");
+    }
+    return 0;
+  };
+  if (int rc = hybrid_mod_up(dev, ct1 + comp, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s, ct2 + comp))
+    return rc;
+  if (rescale) return hybrid_mod_down(dev, result, prod, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);
+  return hybrid_mod_down(dev, result, prod, tmp, n, level, p_size, 2, h, bmods, false, s);
 }
 
 // The shape rules of hexl_b200_key_switch_hybrid, without the key handle
@@ -542,6 +596,62 @@ int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* cipherte
       if (int rc = linear_transform_hybrid_on_device(pi.device, result + c * 2 * comp, ciphertexts + c * 2 * comp,
                                                      diagonals, n, level, q_size, p_size, alpha, h, bmods.data(),
                                                      keys.data(), galois_elts, num_elts, (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                          uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                          const uint64_t* moduli, const hexl_b200_keys* relin_keys, int rescale,
+                                          uint64_t batch, void* stream) {
+  const uint64_t level = level_size, alpha = digit_size;
+  REQUIRE(result && ct1 && ct2 && moduli && relin_keys, "Require non-null arguments");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (int rc = hybrid_handle_check(relin_keys, n, q_size, p_size, alpha, 2, "relin_keys")) return rc;
+  REQUIRE(rescale == 0 || rescale == 1, "Require rescale = 0 or 1");
+  // the merged rescale divides by q_{l-1} too: a level to drop, and K + 1 sources of one base conversion
+  REQUIRE(!rescale || level >= 2, "rescale = 1 requires level_size >= 2");
+  REQUIRE(!rescale || p_size < (uint64_t)kParamBlock, "rescale = 1 requires p_size <= %d", kParamBlock - 1);
+  if (batch == 0) return 0;
+  const uint64_t in_words = 2 * level * n, out_words = 2 * (level - rescale) * n;
+  const uint64_t in_total = batch * in_words, out_total = batch * out_words;
+  REQUIRE(ct1 == ct2 || ct1 + in_total <= ct2 || ct2 + in_total <= ct1,
+          "ct1 and ct2 must be the same ciphertexts or not overlap");
+  REQUIRE(result + out_total <= ct1 || ct1 + in_total <= result, "result and ct1 must not overlap");
+  REQUIRE(result + out_total <= ct2 || ct2 + in_total <= result, "result and ct2 must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, ct1, ct2}, &pi)) return rc;
+  auto bound = [&](u64 i) { return moduli[i]; };
+  if (int rc = check_limb_bounds(ct1, 2 * batch, level, n, bound, pi, "ct1")) return rc;
+  if (ct2 != ct1)
+    if (int rc = check_limb_bounds(ct2, 2 * batch, level, n, bound, pi, "ct2")) return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(level + p_size);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  const bool rs = rescale != 0;
+  // host pointers: both ciphertexts of a pair cross PCIe in once (one copy when squaring) and the product comes back
+  // from the same slot
+  if (pi.where == Where::Host) {
+    const bool square = ct1 == ct2;
+    return key_switch_host_batch(result, out_words, false, ct1, in_words, square ? in_words : 2 * in_words,
+                                 &relin_keys, 1, batch,
+                                 [&](int dev, uint64_t* d_res, uint64_t* d_in, const uint64_t* const* const* dk,
+                                     cudaStream_t s) {
+                                   return multiply_relinearize_hybrid_on_device(
+                                       dev, d_res, d_in, square ? d_in : d_in + in_words, n, level, q_size, p_size,
+                                       alpha, rs, h, bmods.data(), dk[0], s);
+                                 },
+                                 nullptr, square ? nullptr : ct2);
+  }
+  std::vector<const uint64_t* const*> dk;
+  if (keys_on_device(&relin_keys, 1, pi.device, &dk) < 1)
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "relin_keys holds no copy on the device of the ciphertexts");
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = multiply_relinearize_hybrid_on_device(pi.device, result + c * out_words, ct1 + c * in_words,
+                                                         ct2 + c * in_words, n, level, q_size, p_size, alpha, rs, h,
+                                                         bmods.data(), dk[0], (cudaStream_t)stream))
         return rc;
     return 0;
   });

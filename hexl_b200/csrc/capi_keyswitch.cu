@@ -202,11 +202,11 @@ uint64_t keys_on_device(const hexl_b200_keys* const* keys, uint64_t count, int d
 // (stage_items), split by ciphertext over the host devices holding every key.  Ciphertext c's result block
 // (res_words words at result + c * res_words, in the slot's buffer 0) crosses PCIe out, and in as well when
 // result_in; in_words words of `in` (in + c * in_words; nothing when in is null) go into the slot's buffer 1, which
-// holds buf_words words.
+// holds buf_words words, followed by in_words words of in2 (in2 + c * in_words) when in2 is not null.
 int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, const uint64_t* in,
                           uint64_t in_words, uint64_t buf_words, const hexl_b200_keys* const* keys,
                           uint64_t num_keys, uint64_t batch, const HostSwitch& run,
-                          const std::function<int(int)>& prepare) {
+                          const std::function<int(int)>& prepare, const uint64_t* in2) {
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
   std::vector<const uint64_t* const*> dk;
@@ -225,6 +225,8 @@ int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, 
       u64 *d_res = sl.buf(0), *d_in = sl.buf(1);
       cudaError_t e = cudaSuccess;
       if (in) e = cudaMemcpyAsync(d_in, in + c * in_words, in_words * 8, cudaMemcpyHostToDevice, sx);
+      if (e == cudaSuccess && in2)
+        e = cudaMemcpyAsync(d_in + in_words, in2 + c * in_words, in_words * 8, cudaMemcpyHostToDevice, sx);
       if (e == cudaSuccess && result_in)
         e = cudaMemcpyAsync(d_res, result + c * res_words, res_words * 8, cudaMemcpyHostToDevice, sx);
       if (e != cudaSuccess) return cuda_fail(e, "KeySwitch H2D");

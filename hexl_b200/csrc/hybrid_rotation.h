@@ -1,6 +1,7 @@
 // Launchers of the two kernels of the hybrid linear transform (seal.cu): the weighted multi-element
-// multiply-accumulate and the weighted permuted sum of the ciphertext's limbs.  Both take two-component ciphertexts
-// (key component count 2) in NTT form, every word canonical, every modulus below 2^61.
+// multiply-accumulate and the weighted permuted sum of the ciphertext's limbs; and of the multiply-accumulate of the
+// multiply-relinearize call, which adds the tensor terms.  All take two-component ciphertexts (key component count 2)
+// in NTT form, every word canonical, every modulus below 2^61.
 #pragma once
 #include "internal.h"
 
@@ -37,5 +38,24 @@ struct PermutedSumElts {
 cudaError_t launch_ks_permuted_sum(u64* result, const u64* ct, u64 n, u64 level, u64 i0, u64 count,
                                    const PermutedSumElts& elts, u64 num_elts, const KsModuli& mods, bool accumulate,
                                    cudaStream_t stream);
+
+// The tensor terms of the multiply-relinearize call for the first `data` moduli of a mod-up round (the data moduli
+// q_i, i = b0 + e): ct1 and ct2 point at limb b0 of component 0 of the two ciphertexts, component 1 is comp words
+// further, and p[e] = [P]_{q_i} for P the product of the special primes.
+struct RelinTensor {
+  const u64* ct1;
+  const u64* ct2;
+  u64 comp;
+  u64 data;
+  u64 p[kParamBlock];
+};
+// For the `count` moduli of a mod-up round (mods as for launch_ks_mac), every slot l and both key components k:
+//   prod[e][k][l] (+)= sum_{j < jcount} ops[e][j][l] keys.p[j][k][c_e][l]  (+ [P]_{q_i} d_k[i][l] when storing and
+//                      e < tensor.data)   mod q_e,
+// d_0 = a0 b0 and d_1 = a0 b1 + a1 b0 at limb i = b0 + e, (a0, a1) = ct1, (b0, b1) = ct2.  The digit sum stays
+// unreduced in 128 bits (the bound of ks_mac_digits_per_launch); the tensor term is reduced on its own and added mod q.
+cudaError_t launch_ks_relin_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPointers& keys, u64 n, u64 jcount,
+                                u64 key_modulus_size, u64 count, const KsModuli& mods, const RelinTensor& tensor,
+                                bool accumulate, cudaStream_t stream);
 
 }  // namespace hexl_b200

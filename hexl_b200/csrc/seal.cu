@@ -246,6 +246,56 @@ __global__ void __launch_bounds__(kThreads)
   out[level * n] = v1;
 }
 
+// ---- Multiply and relinearize: the key products of the tensor's last term, plus [P] times its first two terms.
+// A thread owns one slot l of one modulus e and both key components: it reads each digit word once for both, keeps each
+// component's sum unreduced in 128 bits (jcount within the bound of ks_mac_digits_per_launch) and reduces it.  The
+// storing launch of a data modulus also reads a0, a1, b0, b1 at the slot: d_k and [P] d_k are reduced on their own
+// (products of canonical words, below 2^123) and added mod q, so the digit sums' bound is untouched.
+__global__ void __launch_bounds__(kThreads)
+    ks_relin_mac_kernel(u64* prod, const u64* ops, u64 ops_stride, const __grid_constant__ KeyPointers keys, u64 n,
+                        u64 jcount, u64 key_modulus_size, u64 count, const __grid_constant__ KsModuli mods,
+                        const __grid_constant__ RelinTensor tensor, int accumulate) {
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= n * count) return;
+  const u64 e = g / n, l = g - e * n;
+  const KsModulus& md = mods.m[e];
+  const u64 key_off = n * md.c + l, comp = key_modulus_size * n;
+  const u64* op = ops + e * ops_stride + l;
+  u64 lo0 = 0, hi0 = 0, lo1 = 0, hi1 = 0;
+  for (unsigned j = 0; j < (unsigned)jcount; ++j) {  // at most kParamBlock digits per launch
+    const u64 x = op[j * n];
+    const u64* key = keys.p[j] + key_off;
+    mac128(x, __ldcs(key), lo0, hi0);
+    mac128(x, __ldcs(key + comp), lo1, hi1);
+  }
+  u64 v0 = reduce128(hi0, lo0, md), v1 = reduce128(hi1, lo1, md);
+  u64* out = prod + e * 2 * n + l;
+  if (accumulate) {
+    v0 = csub(v0 + out[0], md.q);
+    v1 = csub(v1 + out[n], md.q);
+  } else if (e < tensor.data) {
+    const u64 s = e * n + l;
+    const u64 a0 = tensor.ct1[s], a1 = tensor.ct1[s + tensor.comp];
+    const u64 b0 = tensor.ct2[s], b1 = tensor.ct2[s + tensor.comp];
+    u64 lo = 0, hi = 0;
+    mac128(a0, b0, lo, hi);
+    const u64 d0 = reduce128(hi, lo, md);
+    lo = hi = 0;
+    mac128(a0, b1, lo, hi);
+    mac128(a1, b0, lo, hi);
+    const u64 d1 = reduce128(hi, lo, md);
+    const u64 P = tensor.p[e];
+    lo = hi = 0;
+    mac128(P, d0, lo, hi);
+    v0 = csub(v0 + reduce128(hi, lo, md), md.q);
+    lo = hi = 0;
+    mac128(P, d1, lo, hi);
+    v1 = csub(v1 + reduce128(hi, lo, md), md.q);
+  }
+  out[0] = v0;
+  out[n] = v1;
+}
+
 // The two halves of the mod-down by the last modulus, shared by the kernels below.
 // round: a coefficient of the last modulus's part (coefficient form, [0, 2 q_last)) rounded and moved into modulus q:
 //   t = (x + q_last/2) mod q_last;  out = (t mod q) + add,  add = q - (q_last/2 mod q);  out < 2q
@@ -381,6 +431,15 @@ cudaError_t launch_ks_permuted_sum(u64* result, const u64* ct, u64 n, u64 level,
                                    cudaStream_t stream) {
   ks_permuted_sum_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(result, ct, n, level, i0, count, elts,
                                                                         num_elts, mods, accumulate);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ks_relin_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPointers& keys, u64 n, u64 jcount,
+                                u64 key_modulus_size, u64 count, const KsModuli& mods, const RelinTensor& tensor,
+                                bool accumulate, cudaStream_t stream) {
+  ks_relin_mac_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(prod, ops, ops_stride, keys, n, jcount,
+                                                                     key_modulus_size, count, mods, tensor, accumulate);
   count_launch();
   return cudaGetLastError();
 }

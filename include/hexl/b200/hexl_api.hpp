@@ -786,6 +786,20 @@ inline void LinearTransformHybrid(uint64_t* result, const uint64_t* ciphertexts,
                                                        moduli, handles.data(), galois_elts, num_elts, diagonals,
                                                        batch, stream));
 }
+
+// extension: ct1 x ct2 relinearized with hybrid keys that switch s^2 to s, for each of `batch` pairs (2 x level_size
+// limbs each), stored into result (2 x (level_size - rescale) limbs per pair); rescale = 1 merges the rescale by the
+// last limb into the mod-down (hexl_b200_multiply_relinearize_hybrid has the formula).  rescale = 0 equals
+// DyadicMultiply followed by KeySwitchHybrid bit for bit; rescale = 1 rounds once and is NOT that chain followed by
+// DivideAndRoundQLast bit for bit.  ct1 == ct2 squares.
+inline void MultiplyRelinearizeHybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                      uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                      const uint64_t* moduli, const KeySwitchKeys& relin_keys, bool rescale,
+                                      uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_multiply_relinearize_hybrid(result, ct1, ct2, n, level_size, q_size, p_size, digit_size,
+                                                           moduli, relin_keys.Handle(), rescale ? 1 : 0, batch,
+                                                           stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

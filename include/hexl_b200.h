@@ -466,6 +466,44 @@ int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* cipherte
                                       const hexl_b200_keys* const* galois_keys, const uint64_t* galois_elts,
                                       uint64_t num_elts, const uint64_t* diagonals, uint64_t batch, void* stream);
 
+/* Ciphertext multiplication with relinearization by hybrid keys (extension; CKKS HMult: SEAL's multiply + relinearize
+ * [+ rescale_to_next], OpenFHE's EvalMult), optionally rescaled in the same mod-down, for each of `batch` pairs.  The
+ * moduli, digits and shape rules are those of hexl_b200_key_switch_hybrid with key_component_count = 2; relin_keys is
+ * a hybrid key handle (dnum = ceil(q_size / digit_size) buffers of 2 x (q_size + p_size) x n words) that switches s^2
+ * to s.  Pair c reads ct1 + c * 2 * l * n and ct2 + c * 2 * l * n (two components of l = level_size limbs each, NTT
+ * form, canonical) and its product is STORED at result + c * 2 * l' * n, l' = l - rescale.  With (a0, a1) = ct1,
+ * (b0, b1) = ct2, the mod-up D_{d,m}, keys K and slot(m) of hexl_b200_key_switch_hybrid, and P = prod p_j:
+ *   d0 = a0 (.) b0,  d1 = a0 (.) b1 + a1 (.) b0,  t = a1 (.) b1           per data limb, canonical
+ *   prod_{m,k} = sum_d D_{d,m}(t) (.) K[d][k][slot(m)]  mod m,             every m in B
+ *   ext_{m,k}  = prod_{m,k} + [P]_m d_{k,m} for m = q_i, i < l;  ext_{p_j,k} = prod_{p_j,k}
+ *   T = {p_0..p_{K-1}} (rescale = 0) or {q_{l-1}, p_0..p_{K-1}} (rescale = 1),  P_T = prod T
+ *   x_t = INTT_t(ext_{t,k}),  z_t = [(x_t + floor(P_T/2)) (P_T/t)^-1]_t                          every t in T
+ *   c_i = [ sum_t z_t [P_T/t]_{q_i} - floor(P_T/2) ]_{q_i},  result_{k,i} = (ext_{q_i,k} - NTT_{q_i}(c_i)) P_T^-1
+ *   mod q_i, canonical, for i < l'.
+ * rescale = 0 is bit for bit hexl_b200_dyadic_multiply followed by hexl_b200_key_switch_hybrid of d2 into (d0, d1): the
+ * mod-down reads only the special limbs, where ext = prod, and (prod + P d - NTT(c)) P^-1 = (prod - NTT(c)) P^-1 + d
+ * mod q_i with both sides canonical.  At digit_size = 1 with one special prime it is therefore hexl_b200_dyadic_multiply
+ * followed by hexl_b200_key_switch_resident (SEAL's multiply + relinearize) bit for bit.  rescale = 1 is NOT that
+ * chain followed by hexl_b200_divide_and_round_q_last bit for bit: it rounds once, by q_{l-1} P, where the chain rounds
+ * by P and then by q_{l-1}.  It decrypts to round(phase(ct1) phase(ct2) / q_{l-1}) within the key switch's error
+ * divided by q_{l-1} plus one rounding term of K + 1 sources.  ct1 == ct2 (squaring) is allowed; any other overlap
+ * of the inputs, and any overlap of result with an input, is refused.  HEXL_B200_ERR_INVALID_ARG on the refusals of
+ * hexl_b200_key_switch_hybrid with key_component_count = 2, on rescale other than 0 or 1, on rescale = 1 with
+ * level_size < 2 or p_size > 63 (the merged mod-down converts from K + 1 <= 64 moduli), and on those overlaps.
+ * batch = 0 does nothing.  Inputs are checked below their modulus under hexl_b200_set_debug(1).  On the device, per
+ * pair: the mod-up of hexl_b200_key_switch_hybrid applied to t, whose first inverse transform multiplies a1 by b1 on
+ * load (t is never written); per round of moduli of B, one multiply-accumulate launch per chunk of digits within the
+ * 128-bit bound, the first of which reads a0, a1, b0, b1 on the data moduli and adds [P] d; then one mod-down by P_T
+ * that stores into result.  These are the launches of hexl_b200_key_switch_hybrid, with K + 1 special limbs and l - 1
+ * targets in the mod-down when rescale = 1.  Library scratch: one round of converted digits plus (l + p_size) x 2 x n
+ * words of products.  Device calls capture into a CUDA graph once the transforms are warm.  Host buffers: both
+ * ciphertexts of a pair cross PCIe in once (one copy when squaring) and the product comes back on the same staging
+ * stream, split by pair over the devices of hexl_b200_set_host_devices where the handle holds a copy. */
+int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                          uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                          const uint64_t* moduli, const hexl_b200_keys* relin_keys, int rescale,
+                                          uint64_t batch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
