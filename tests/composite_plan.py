@@ -1,5 +1,5 @@
-"""The scratch rounds of the RNS composites (hexl_b200/csrc/capi_keyswitch.cu, capi_galois.cu) restated in Python, and the shapes of
-tests/test_gpu_composite_rounds.py.
+"""The scratch rounds of the RNS composites (hexl_b200/csrc/capi_keyswitch.cu, capi_galois.cu, capi_hybrid.cu) restated
+in Python, and the shapes of tests/test_gpu_composite_rounds.py and tests/test_gpu_hybrid_rounds.py.
 
 Each composite splits one device call into rounds that fit about 256 MiB of pool scratch:
 
@@ -7,6 +7,17 @@ Each composite splits one device call into rounds that fit about 256 MiB of pool
     galois_inplace_rounds   apply_galois_on_device, in place: polynomials copied into scratch per round
     key_switch_rounds       key_switch_on_device, step 2: RNS moduli per round
     ks_mac_launches         the digits of each ks_mac_kernel launch within one round (ks_mac_digits_per_launch)
+
+and the hybrid family (KeySwitchHybrid, the hoisted hybrid rotations, LinearTransformHybrid and
+MultiplyRelinearizeHybrid) around one mod-up and one mod-down:
+
+    hybrid_mod_up_rounds    hybrid_mod_up: moduli of the extended basis B per round, and hybrid_round_slots their keys
+    base_conv_blocks        base_convert_on_device: targets per launch (base_conv_targets of the source count)
+    hybrid_mod_down_blocks  hybrid_mod_down: blocks of 64 data moduli, each in base-conversion launches from K (or
+                            K + 1 with the merged rescale) special limbs
+    relin_mac_launches, weighted_mac_launches, ks_mac_launches
+                            the multiply-accumulate launches of one round of each call
+    hybrid_launches         the kernel launches of one ciphertext of each call, from all of the above
 
 Every function returns the list of round (or launch) sizes.  SOURCE holds the source file under hexl_b200/csrc and the
 lines of it each formula restates;
@@ -31,6 +42,38 @@ SOURCE = {
     "ks_mac": ("capi_keyswitch.cu",
                ["const unsigned __int128 largest_product = (unsigned __int128)(4 * q - 1) * (q - 1);",
                 "return (uint64_t)std::min<unsigned __int128>(kParamBlock, ~(unsigned __int128)0 / largest_product);"]),
+    # ks_mac_products, which the hybrid switch and the hoisted hybrid rotations run once per mod-up round
+    "ks_mac_products": ("capi_keyswitch.cu",
+                        ["const uint64_t per_mod = decomp * n, jmax = ks_mac_digits_per_launch(mods, cnt);",
+                         "for (uint64_t r = 0; r < elts; ++r)",
+                         "for (uint64_t j0 = 0; j0 < decomp; j0 += jmax) {"]),
+    "base_conv_targets": ("internal.h",
+                          ["constexpr int kBaseConvWords = 480;",
+                           "inline u64 base_conv_targets(u64 from) { return (kBaseConvWords - 4 * from) / (5 + from); }"]),
+    "base_conv_blocks": ("capi_hybrid.cu",
+                         ["const uint64_t F = from_count, block = base_conv_targets(F);",
+                          "for (uint64_t e0 = 0; e0 < to_count; e0 += block) {",
+                          "const uint64_t cnt = std::min(block, to_count - e0);"]),
+    "hybrid_mod_up": ("capi_hybrid.cu",
+                      ["const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size;",
+                       "const uint64_t per_mod = D * n;",
+                       "uint64_t ichunk = std::max<uint64_t>(1, (256ull << 20) / (per_mod * 8));",
+                       "ichunk = std::min<uint64_t>({ichunk, nb, (uint64_t)kParamBlock});",
+                       "const uint64_t lo = d * alpha, width = std::min(alpha, level - lo);",
+                       "for (uint64_t e = 0; e < cnt; ++e) slots[e] = b0 + e < level ? b0 + e : q_size + (b0 + e - level);"]),
+    "hybrid_mod_down": ("capi_hybrid.cu",
+                        ["for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {",
+                         "const uint64_t cnt = std::min<uint64_t>(kParamBlock, level - i0);",
+                         "if (rescale) return hybrid_mod_down(dev, result, prod, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);"]),
+    "relin_mac": ("capi_hybrid.cu",
+                  ["tensor.data = b0 < level ? std::min(cnt, level - b0) : 0;",
+                   "const uint64_t jc = std::min(ks_mac_digits_per_launch(mods, cnt), D);",
+                   "for (uint64_t j0 = 0; j0 < D; j0 += jc) {  // key pointers ride in the kernel parameters"]),
+    "weighted_mac": ("capi_hybrid.cu",
+                     ["for (uint64_t r0 = 0; r0 < elts; r0 += kParamBlock) {",
+                      "const uint64_t per = std::max<uint64_t>(1, kParamBlock / jc);",
+                      "for (uint64_t j0 = 0; j0 < D; j0 += jc) {",
+                      "for (uint64_t k0 = 0; k0 < keyed.size(); k0 += per) {"]),
 }
 
 
@@ -67,6 +110,98 @@ def ks_mac_launches(decomp, largest_q):
     return _split(decomp, ks_mac_digits_per_launch(largest_q))
 
 
+# ------------------------------------------------------------------------------ the hybrid family (capi_hybrid.cu)
+BASE_CONV_WORDS = 480     # internal.h: kBaseConvWords, the parameter table of one base-conversion launch
+
+
+def base_conv_targets(from_count):
+    """targets one base-conversion launch takes: 4 words per source, 5 + from_count per target"""
+    return (BASE_CONV_WORDS - 4 * from_count) // (5 + from_count)
+
+
+def base_conv_blocks(from_count, to_count):
+    """the targets of each launch of base_convert_on_device"""
+    return _split(to_count, base_conv_targets(from_count))
+
+
+def hybrid_digit_widths(level, alpha):
+    """the moduli of each digit at `level`: alpha each, the last one partial"""
+    return [min(alpha, level - lo) for lo in range(0, level, alpha)]
+
+
+def hybrid_mod_up_rounds(n, level, K, alpha):
+    """hybrid_mod_up: the moduli of B = {q_0..q_{level-1}, p_0..p_{K-1}} per round, every digit (D x n words per
+    modulus) under `ichunk` moduli at a time, at most one parameter block"""
+    D, nb = -(-level // alpha), level + K
+    ichunk = min(max(1, SCRATCH_BYTES // (D * n * 8)), nb, PARAM_BLOCK)
+    return _split(nb, ichunk)
+
+
+def hybrid_round_slots(level, q_size, b0, cnt):
+    """the key slot of each modulus of the round starting at b0: data modulus b < level in slot b, special prime j in
+    slot q_size + j"""
+    return [b if b < level else q_size + (b - level) for b in range(b0, b0 + cnt)]
+
+
+def hybrid_mod_down_blocks(level, K, rescale=False):
+    """hybrid_mod_down: per block of 64 data moduli, the targets of each base-conversion launch, from K special limbs,
+    or K + 1 with the merged rescale (q_{level-1} joins P and leaves the targets)"""
+    targets, sources = level - int(rescale), K + int(rescale)
+    return [base_conv_blocks(sources, cnt) for cnt in _split(targets, PARAM_BLOCK)]
+
+
+def relin_tensor_data(level, b0, cnt):
+    """the data limbs of a mod-up round that the relinearization's storing launch adds the tensor terms into"""
+    return min(cnt, level - b0) if b0 < level else 0
+
+
+def relin_mac_launches(D, largest_q):
+    """MultiplyRelinearizeHybrid: the digits of each ks_relin_mac launch of one round"""
+    return _split(D, min(ks_mac_digits_per_launch(largest_q), D))
+
+
+def weighted_mac_launches(D, keyed, largest_q):
+    """LinearTransformHybrid: (digits, elements) of each ks_weighted_mac launch of one round: a digit chunk within the
+    128-bit bound, times chunks of 64 // jc keyed elements"""
+    jc = min(ks_mac_digits_per_launch(largest_q), D)
+    per = max(1, PARAM_BLOCK // jc)
+    return [(j, e) for j in _split(D, jc) for e in _split(keyed, per)]
+
+
+def hybrid_launches(call, n, level, K, alpha, basis, ntt, elts=1, keyed=None, rescale=False, kcc=2):
+    """kernel launches of one ciphertext of `call` ("switch", "hoisted", "linear", "mul_relin"): basis holds the moduli
+    of B (level data, then K special); ntt(forward, units) is the launch count of one multi-modulus transform of
+    `units` polynomials.  "switch" and "hoisted" run `elts` switches over one mod-up; "linear" takes `elts` elements,
+    `keyed` of them with keys."""
+    D = -(-level // alpha)
+    total = 0
+    if call == "hoisted":
+        total += elts                                                      # one automorphism launch per element
+    if call == "linear":
+        total += -(-level // PARAM_BLOCK) * -(-elts // PARAM_BLOCK)        # the permuted sums
+        if not keyed:
+            return total
+    total += sum(ntt(False, cnt) for cnt in _split(level, PARAM_BLOCK))   # the target back to coefficients
+    b0 = 0
+    for cnt in hybrid_mod_up_rounds(n, level, K, alpha):
+        total += sum(len(base_conv_blocks(w, cnt)) for w in hybrid_digit_widths(level, alpha))
+        total += ntt(True, cnt * D)
+        largest = max(basis[b0:b0 + cnt])
+        if call == "mul_relin":
+            total += len(relin_mac_launches(D, largest))
+        elif call == "linear":
+            total += len(weighted_mac_launches(D, keyed, largest))
+        else:
+            total += elts * len(ks_mac_launches(D, largest))
+        b0 += cnt
+    downs = 1 if call in ("linear", "mul_relin") else elts
+    k_down, kk = K + int(rescale), (kcc if call == "switch" else 2)
+    down = ntt(False, k_down * kk)
+    for cnt, blocks in zip(_split(level - int(rescale), PARAM_BLOCK), hybrid_mod_down_blocks(level, K, rescale)):
+        down += len(blocks) + ntt(True, cnt * kk) + 1                       # base conversions, transform, finish
+    return total + downs * down
+
+
 # ------------------------------------------------------------------------------ the GPU test's shapes
 # name -> (n, chain, limbs, count): the rescale in NTT and coefficient form
 RESCALE_SHAPES = {
@@ -79,4 +214,12 @@ GALOIS_SHAPE = (1 << 16, "seal", 31, 35)        # rounds 16, 16, 3
 KS_SHAPES = {
     "ckks_n16": (16, 30),   # moduli rounds 17, 14; digits per launch 16, 14
     "ckks_n17": (17, 29),   # moduli rounds 8, 8, 8, 6
+}
+# name -> (log2 n, L, K, alpha, data prime bits, special prime bits, levels): the hybrid calls of
+# tests/test_gpu_hybrid_rounds.py; tests/test_composite_plan.py pins the plan each name stands for
+HYBRID_SHAPES = {
+    "bench_rescale": (16, 30, 10, 10, 50, 50, (30,)),   # one round; merged rescale's mod-down targets 27 + 2
+    "budget_a2": (16, 30, 10, 2, 50, 50, (30, 29)),     # rounds 34 + 6, and 34 + 5 with a one-modulus last digit
+    "budget_a3": (17, 30, 3, 3, 50, 50, (30, 28)),      # rounds 25 + 8, and 25 + 6 mixing data and special moduli
+    "mixed_chunks": (16, 24, 2, 1, 50, 60, (24,)),      # rounds 21 + 5; multiply-accumulate 1, then 16 + 8 launches
 }

@@ -47,6 +47,20 @@ def fast_base_convert(port, x, n, from_moduli, to_moduli, add=None, sub=None):
     return np.concatenate(out)
 
 
+def fast_base_convert_int(x, n, from_moduli, to_moduli):
+    """The definition of hexl_b200_fast_base_convert in plain Python integers, for its whole domain (pairwise-coprime
+    sources and any targets in (1, 2^61), neither needing to be prime, odd or NTT-friendly):
+        result_t = (sum_i [x_i (Q/q_i)^-1]_{q_i} (Q/q_i)) mod t
+    One polynomial of len(from_moduli) limbs of n words; returns len(to_moduli) limbs."""
+    src = [int(q) for q in from_moduli]
+    Q = _prod(src)
+    x = np.asarray(x, dtype=U64).reshape(len(src), n).astype(object)
+    total = np.zeros(n, dtype=object)
+    for i, q in enumerate(src):
+        total = total + (x[i] * pow(Q // q, -1, q)) % q * (Q // q)
+    return np.concatenate([(total % int(t)).astype(U64) for t in to_moduli])
+
+
 def digits(level, alpha):
     """S_d = [d alpha, min((d + 1) alpha, level)) for d < ceil(level / alpha)"""
     return [list(range(lo, min(lo + alpha, level))) for lo in range(0, level, alpha)]

@@ -6,7 +6,9 @@ the three word classes of the transforms, 70 data moduli in one 64-modulus digit
 base conversion), primes just below 2^61 with every word q - 1, levels L, a partial digit and 1, key component counts
 1 to 3, and every degree from 2 to 2^17.  At alpha = 1 and K = 1 the call equals KeySwitchResident bit for bit.  Device,
 pageable and pinned host, split host and managed buffers, graph replay, launch counts, decryption and the argument
-refusals are pinned."""
+refusals are pinned.  tests/test_gpu_hybrid_rounds.py runs the call at production sizes whose mod-up takes several
+rounds, at every level, over wrapping host batches, offset views and threads; tests/test_gpu_base_convert_domain.py
+runs FastBaseConvert across its whole domain against plain integers."""
 import os
 import shutil
 import subprocess

@@ -8,7 +8,9 @@ ciphertexts, keys and diagonals (digit chunks of the 128-bit bound as well), the
 repeated elements and identity terms without keys, and device, pageable, pinned, split-host and managed buffers.
 Also pinned: equality with ApplyGaloisKeySwitchHoisted at digit size 1 and one special prime, with
 [c0, 0] + KeySwitchHybrid(c1) at g = 1, and between the two calls for one element with a unit diagonal; graph replay
-with new data; launch counts; the argument refusals; and a C++ caller."""
+with new data; launch counts; the argument refusals; and a C++ caller.  tests/test_gpu_hybrid_rounds.py runs both calls at production sizes whose mod-up takes several
+rounds, at every level, over wrapping host batches, offset views and threads, with launch counts from
+tests/composite_plan.py."""
 import os
 import shutil
 import subprocess

@@ -7,7 +7,9 @@ mod-down), primes just below 2^61 with every ciphertext and key word q - 1 (20 d
 the 128-bit bound), squaring, batch 3, and device, pageable, pinned, split-host and managed buffers.  Also pinned:
 rescale = 0 equals DyadicMultiply followed by KeySwitchHybrid bit for bit (at the production shape N = 2^16, L = 30,
 alpha = K = 10 too), and at digit size 1 with one special prime DyadicMultiply followed by KeySwitchResident; the inputs
-are left unchanged; graph replay with new data; launch counts; the argument refusals; and a C++ caller."""
+are left unchanged; graph replay with new data; launch counts; the argument refusals; and a C++ caller.  tests/test_gpu_hybrid_rounds.py runs the call with both rescale modes at N = 2^16, (30, 10, 10),
+where the merged rescale's mod-down converts into 27 + 2 targets, at budget-limited multi-round shapes, at every
+level, over wrapping host batches, offset views and threads."""
 import os
 import shutil
 import subprocess

@@ -1,5 +1,6 @@
 """The hybrid key-switch model (tests/hybrid_exact.py) against big-integer arithmetic, against the exact key switch, and
-against decryption; and the compiler's resource report of the base-conversion kernel.  CPU only."""
+against decryption; the plain-integer base conversion of the GPU domain tests against the modular model; and the
+compiler's resource report of the base-conversion kernel.  CPU only."""
 import numpy as np
 import pytest
 
@@ -105,3 +106,23 @@ def test_base_conversion_kernel_keeps_no_local_memory():
     bad = [f"{name}: {frame} B frame, {st} B spill stores" for name, (frame, st, ld) in res.items()
            if frame > max(st, ld)]
     assert not bad, bad
+
+
+@pytest.mark.parametrize("sizes, bits", [((1, 3), 50), ((3, 5), 50), ((10, 29), 60), ((64, 3), 60)])
+def test_integer_base_conversion_equals_the_modular_model_on_primes(port, sizes, bits):
+    """the plain-integer reference of the GPU's base-conversion domain tests, pinned to the modular model on NTT primes
+    (where both apply), with every word q - 1 and with uniform words"""
+    mods = [int(q) for q in port.generate_primes(sum(sizes), bits, bits < 60, 2)]
+    src, dst = mods[:sizes[0]], mods[sizes[0]:]
+    n = 65
+    for x in (np.concatenate([uniform_below(7 * i + 1, n, q) for i, q in enumerate(src)]),
+              np.concatenate([np.full(n, q - 1, dtype=np.uint64) for q in src])):
+        assert (hx.fast_base_convert_int(x, n, src, dst) == hx.fast_base_convert(port, x, n, src, dst)).all()
+
+
+def test_integer_base_conversion_on_small_numbers():
+    """sources 3, 5 (Q = 15) into 2, 4, 7 and 15 itself: the sum of y_i (Q/q_i) over the integers, reduced"""
+    x = np.array([2, 1, 0, 4], dtype=np.uint64)  # limb 3: 5 and 4 mod 3, limb 5: 5 and 4 mod 5
+    out = hx.fast_base_convert_int(x, 2, [3, 5], [2, 4, 7, 15]).reshape(4, 2)
+    # X = 5: y = (2 * 5^-1 mod 3, 0) = (1, 0), sum 5;  X = 4: y = (1 * 2 mod 3, 4 * 3^-1 mod 5) = (2, 3), sum 10 + 9 = 19
+    assert out.tolist() == [[1, 1], [1, 3], [5, 5], [5, 4]]
