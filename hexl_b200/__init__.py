@@ -133,6 +133,8 @@ _sig("hexl_b200_apply_galois_key_switch_hybrid_hoisted", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _u64, _vp])
 _sig("hexl_b200_linear_transform_hybrid", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _u64, _vp])
+_sig("hexl_b200_linear_transform_hybrid_bsgs", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _int, _u64, _vp])
 _sig("hexl_b200_multiply_relinearize_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
 
@@ -682,6 +684,42 @@ def LinearTransformHybrid(result, ciphertexts, n, level_size, q_size, p_size, di
     _check(_lib.hexl_b200_linear_transform_hybrid(rp, cp, n, level_size, q_size, p_size, digit_size, mods.ctypes.data,
                                                   keys, elts.ctypes.data, elts.size, dp, batch,
                                                   _stream(stream, rc or cc or dc)))
+    return result
+
+
+def LinearTransformHybridBSGS(result, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, baby_keys,
+                              baby_elts, giant_keys, giant_elts, diagonals, rescale=False, batch=1, stream=None):
+    """sum_j sigma_{h_j}(sum_i w_{j,i} (.) sigma_{b_i}(ct)) with hybrid keys, baby-step giant-step and double-hoisted
+    (hexl_b200_linear_transform_hybrid_bsgs): ciphertext c of `ciphertexts` (2*level_size*n words each) is stored at
+    result[c * 2*l'*n:], l' = level_size - rescale.  diagonals lists len(giant_elts) x len(baby_elts) buffers (flat,
+    row j = giant j, or one list per giant), each None (absent) or (level_size + p_size) x n words in NTT form.  A key
+    of None is an identity term (element 1) on either side.  rescale=True divides by the last limb in the final
+    mod-down."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    be = np.ascontiguousarray(baby_elts, dtype=np.uint64)
+    ge = np.ascontiguousarray(giant_elts, dtype=np.uint64)
+    rp, rn, rc = _buf(result); cp, cn, cc = _buf(ciphertexts)
+    flat = [d for row in diagonals for d in row] if diagonals and isinstance(diagonals[0], (list, tuple)) \
+        else list(diagonals)
+    per, dwords = 2 * level_size * n, (level_size + p_size) * n
+    _need("moduli", mods.size, q_size + p_size)
+    _need("baby_keys", len(baby_keys), be.size); _need("giant_keys", len(giant_keys), ge.size)
+    _need("diagonals", len(flat), be.size * ge.size)
+    _need("result", rn, batch * 2 * (level_size - int(bool(rescale))) * n); _need("ciphertexts", cn, batch * per)
+    ptrs, any_cuda = [], False
+    for r, d in enumerate(flat[:be.size * ge.size]):
+        dp, dn, dc = _buf(d)
+        if dp is not None:
+            _need(f"diagonals[{r}]", dn, dwords)
+        ptrs.append(dp)
+        any_cuda = any_cuda or bool(dc)
+    table = (_vp * max(1, len(ptrs)))(*ptrs)
+    babies = (_vp * max(1, len(baby_keys)))(*[k._h if k is not None else None for k in baby_keys])
+    giants = (_vp * max(1, len(giant_keys)))(*[k._h if k is not None else None for k in giant_keys])
+    _check(_lib.hexl_b200_linear_transform_hybrid_bsgs(rp, cp, n, level_size, q_size, p_size, digit_size,
+                                                       mods.ctypes.data, babies, be.ctypes.data, be.size, giants,
+                                                       ge.ctypes.data, ge.size, table, int(bool(rescale)), batch,
+                                                       _stream(stream, rc or cc or any_cuda)))
     return result
 
 

@@ -387,7 +387,8 @@ int key_switch_on_device(int dev, uint64_t* result, const uint64_t* t_target, ui
 // The multiply-accumulate of one step-2 round: ops ([e][j][n], lazily transformed digits under the round's cnt moduli,
 // hs[e] their transforms and slots[e] their slots in keys of kms slots) times the keys of each of `elts` switches,
 // into prod + r * prod_stride ([e][k][n]); chunked by ks_mac_digits_per_launch.  keys[r][j]: digit j's key of switch
-// r; galois_elts[r] (nullptr: none) makes switch r read the digits permuted by pi_g.
+// r; galois_elts[r] (nullptr: none) makes switch r read the digits permuted by pi_g.  accumulate: every launch adds
+// into prod, the first digit chunk's too (otherwise that one stores).
 // The multiply-accumulate's constants of cnt <= kParamBlock moduli: q, floor(2^64 / q), 2^64 mod q and its Shoup
 // factor, and c = slots[e] (0 when slots is null)
 KsModuli ks_mac_moduli(const uint64_t* moduli, const uint64_t* slots, uint64_t cnt);
@@ -396,7 +397,8 @@ KsModuli ks_mac_moduli(const uint64_t* moduli, const uint64_t* slots, uint64_t c
 uint64_t ks_mac_digits_per_launch(const KsModuli& mods, uint64_t count);
 int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cnt, uint64_t kms, const uint64_t* ops,
                     uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod, uint64_t prod_stride,
-                    const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s);
+                    const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s,
+                    bool accumulate = false);
 int key_switch_elts_on_device(int dev, uint64_t* const* results, const uint64_t* t_target, uint64_t n, uint64_t decomp,
                               uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
                               const uint64_t* const* const* d_key_ptrs, const uint64_t* galois_elts, uint64_t elts,

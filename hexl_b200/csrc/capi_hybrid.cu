@@ -1,7 +1,8 @@
 // Hybrid key switching (OpenFHE's KeySwitchHYBRID): digits of up to 64 data moduli and up to 64 special primes, the
 // mod-up and the mod-down by fast base conversion (rns.cu); the base conversion on its own; and the rotations with
-// hybrid keys: hoisted, and the diagonal-weighted sum of rotations under one mod-down (the linear transform); and the
-// ciphertext product relinearized with hybrid keys, its rescale optionally merged into the mod-down.
+// hybrid keys: hoisted, the diagonal-weighted sum of rotations under one mod-down (the linear transform) and its
+// double-hoisted baby-step giant-step form; and the ciphertext product relinearized with hybrid keys, its rescale
+// optionally merged into the mod-down.
 #include <cstdio>
 #include <numeric>
 
@@ -258,6 +259,129 @@ static int linear_transform_hybrid_on_device(int dev, uint64_t* result, const ui
   };
   if (int rc = hybrid_mod_up(dev, ct + level * n, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s)) return rc;
   return hybrid_mod_down(dev, result, acc, tmp, n, level, p_size, 2, h, bmods, true, s);
+}
+
+// The baby-step giant-step transform of one ciphertext ct (as above) into result (2 x (level - rescale) x n words):
+// diag[j * n1 + i] is the (giant j, baby i) diagonal on this device ((level + K) x n words) or nullptr when absent;
+// baby_keys[i] / giant_keys[j] a handle's copy, or nullptr for an identity term.  X (data limbs, in result, or in
+// scratch with the rescale) and Y (two components over B) stay apart; include/hexl_b200.h has the definitions.
+//   1. when some keyed baby has a diagonal: one mod-up of c1, its products with every such baby's keys stored
+//      ([i][b][k][n]);
+//   2. per giant step with a present baby: the sum launches (per block of 64 moduli of B, only the data moduli when
+//      the row has no keyed baby, and per chunk of 64 present babies);
+//   3. per keyed giant step: the mod-down of y_1 into x_1 (kcc = 1; none without a keyed baby), then the mod-up of
+//      c1' = x_1 with its multiply-accumulate reading pi_h and adding into Y;
+//   4. one mod-down of Y into result (none while Y is empty), or with the rescale, [P] X folded into Y's data limbs by
+//      the last sum launch and the mod-down by q_{level-1} P that stores.
+static int bsgs_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct, const uint64_t* const* diag,
+                                 uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size, uint64_t alpha,
+                                 bool rescale, const CachedNtts& h, const uint64_t* bmods,
+                                 const uint64_t* const* const* baby_keys, const uint64_t* baby_elts, uint64_t n1,
+                                 const uint64_t* const* const* giant_keys, const uint64_t* giant_elts, uint64_t n2,
+                                 cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, comp = level * n;
+  const uint64_t stride = nb * 2 * n;  // one baby's stored products
+  // the keyed babies with a diagonal, in baby order: their index among the stored products
+  std::vector<uint64_t> stored(n1, kBsgsNoProducts), used_elts;
+  std::vector<const uint64_t* const*> used_keys;
+  for (uint64_t i = 0; i < n1; ++i) {
+    if (!baby_keys[i]) continue;
+    for (uint64_t j = 0; j < n2; ++j)
+      if (diag[j * n1 + i]) {
+        stored[i] = used_keys.size();
+        used_keys.push_back(baby_keys[i]);
+        used_elts.push_back(baby_elts[i]);
+        break;
+      }
+  }
+  uint64_t last_row = n2;  // the last giant step with a present baby: its sums fold X into Y under the rescale
+  for (uint64_t j = 0; j < n2; ++j)
+    for (uint64_t i = 0; i < n1; ++i)
+      if (diag[j * n1 + i]) last_row = j;
+  Scratch ws(s);
+  uint64_t *prods = nullptr, *y = nullptr, *x = result, *x1 = nullptr, *y1 = nullptr, *tmp = nullptr;
+  if (!used_keys.empty())
+    if (int rc = ws.get(&prods, used_keys.size() * stride)) return rc;  // [i][b][k][n]
+  if (int rc = ws.get(&y, stride)) return rc;                           // [b][k][n]
+  if (rescale)
+    if (int rc = ws.get(&x, 2 * comp)) return rc;  // [k][i][n]
+  if (int rc = ws.get(&x1, comp)) return rc;       // [i][n]
+  if (int rc = ws.get(&y1, nb * n)) return rc;     // [b][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * 2 * n)) return rc;  // [i][k][n], one block
+  CU(cudaMemsetAsync(y, 0, stride * sizeof(uint64_t), s));
+  CU(cudaMemsetAsync(x, 0, 2 * comp * sizeof(uint64_t), s));
+  // 1. the baby products
+  if (!used_keys.empty()) {
+    Scratch wu(s);
+    if (int rc = hybrid_mod_up(dev, ct + comp, n, level, q_size, p_size, alpha, h, bmods, wu,
+                               [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) {
+                                 return ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, 2,
+                                                        prods + b0 * 2 * n, stride, used_keys.data(),
+                                                        used_elts.data(), used_keys.size(), s);
+                               },
+                               s))
+      return rc;
+  }
+  bool y_used = false;
+  for (uint64_t j = 0; j < n2; ++j) {
+    std::vector<uint64_t> present;
+    bool keyed_baby = false;
+    for (uint64_t i = 0; i < n1; ++i)
+      if (diag[j * n1 + i]) {
+        present.push_back(i);
+        keyed_baby = keyed_baby || baby_keys[i];
+      }
+    if (present.empty()) continue;  // an absent row costs nothing
+    const bool keyed_giant = giant_keys[j] != nullptr, fold = rescale && j == last_row;
+    // 2. the giant step's sums; without a keyed baby the special limbs would only add zeros
+    const uint64_t span = keyed_baby ? nb : level;
+    for (uint64_t b0 = 0; b0 < span; b0 += kParamBlock) {
+      const uint64_t cnt = std::min<uint64_t>(kParamBlock, span - b0);
+      KsModuli mods = ks_mac_moduli(bmods + b0, nullptr, cnt);
+      if (fold)
+        for (uint64_t e = 0; e < cnt && b0 + e < level; ++e) {
+          const uint64_t q = bmods[b0 + e];
+          uint64_t P = 1 % q;
+          for (uint64_t k = 0; k < p_size; ++k) P = mul_mod128(P, bmods[level + k] % q, q);
+          mods.m[e].c = P;
+        }
+      for (uint64_t r0 = 0; r0 < present.size(); r0 += kParamBlock) {
+        const uint64_t rcnt = std::min<uint64_t>(kParamBlock, present.size() - r0);
+        BsgsSumTerms terms{};
+        for (uint64_t r = 0; r < rcnt; ++r) {
+          const uint64_t i = present[r0 + r];
+          terms.diag[r] = diag[j * n1 + i] + b0 * n;
+          terms.elt[r] = (unsigned)baby_elts[i];
+          terms.prod[r] = (unsigned)stored[i];
+        }
+        int mode = keyed_giant ? kBsgsKeyedGiant : 0;
+        if (r0 == 0) mode |= kBsgsStore1;
+        if (fold && r0 + rcnt == present.size()) mode |= kBsgsFold;
+        const cudaError_t e = launch_ks_bsgs_sum(x, y, x1, y1, ct, prods, stride, n, level, b0, cnt, giant_elts[j],
+                                                 terms, rcnt, mods, mode, s);
+        if (e != cudaSuccess) return cuda_fail(e, "LinearTransformHybridBSGS: sum launch");
+      }
+    }
+    y_used = y_used || keyed_baby || keyed_giant;
+    if (!keyed_giant) continue;
+    // 3. the giant step's own switch: c1' = x_1 + ModDown_P(y_1), then its mod-up multiplied with the giant's keys
+    //    through pi_h and added into Y
+    if (keyed_baby)
+      if (int rc = hybrid_mod_down(dev, x1, y1, tmp, n, level, p_size, 1, h, bmods, true, s)) return rc;
+    Scratch wu(s);
+    const uint64_t h_elt = giant_elts[j];
+    if (int rc = hybrid_mod_up(dev, x1, n, level, q_size, p_size, alpha, h, bmods, wu,
+                               [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) {
+                                 return ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, 2, y + b0 * 2 * n,
+                                                        stride, &giant_keys[j], &h_elt, 1, s, true);
+                               },
+                               s))
+      return rc;
+  }
+  // 4. the final mod-down
+  if (rescale) return hybrid_mod_down(dev, result, y, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);
+  if (!y_used) return 0;
+  return hybrid_mod_down(dev, result, y, tmp, n, level, p_size, 2, h, bmods, true, s);
 }
 
 // The product of two ciphertexts ct1 = (a0, a1) and ct2 = (b0, b1) (each two components of level limbs, NTT form,
@@ -596,6 +720,108 @@ int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* cipherte
       if (int rc = linear_transform_hybrid_on_device(pi.device, result + c * 2 * comp, ciphertexts + c * 2 * comp,
                                                      diagonals, n, level, q_size, p_size, alpha, h, bmods.data(),
                                                      keys.data(), galois_elts, num_elts, (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+int hexl_b200_linear_transform_hybrid_bsgs(uint64_t* result, const uint64_t* ciphertexts, uint64_t n,
+                                           uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                           const uint64_t* moduli, const hexl_b200_keys* const* baby_keys,
+                                           const uint64_t* baby_elts, uint64_t num_baby,
+                                           const hexl_b200_keys* const* giant_keys, const uint64_t* giant_elts,
+                                           uint64_t num_giant, const uint64_t* const* diagonals, int rescale,
+                                           uint64_t batch, void* stream) {
+  const uint64_t level = level_size, alpha = digit_size, n1 = num_baby, n2 = num_giant;
+  REQUIRE(result && ciphertexts && moduli, "Require non-null arguments");
+  REQUIRE(n1 == 0 || (baby_keys && baby_elts), "Require baby_keys, baby_elts != nullptr");
+  REQUIRE(n2 == 0 || (giant_keys && giant_elts), "Require giant_keys, giant_elts != nullptr");
+  REQUIRE(n1 * n2 == 0 || diagonals, "Require diagonals != nullptr");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (int rc = hybrid_elts_check(n, q_size, p_size, alpha, baby_keys, baby_elts, n1, true)) return rc;
+  if (int rc = hybrid_elts_check(n, q_size, p_size, alpha, giant_keys, giant_elts, n2, true)) return rc;
+  REQUIRE(rescale == 0 || rescale == 1, "Require rescale = 0 or 1");
+  REQUIRE(!rescale || level >= 2, "rescale = 1 requires level_size >= 2");
+  REQUIRE(!rescale || p_size < (uint64_t)kParamBlock, "rescale = 1 requires p_size <= %d", kParamBlock - 1);
+  if (n1 == 0 || n2 == 0 || batch == 0) return 0;
+  const uint64_t comp = level * n, nb = level + p_size, in_words = 2 * comp, out_words = 2 * (level - rescale) * n;
+  const uint64_t in_total = batch * in_words, out_total = batch * out_words, dwords = nb * n;
+  REQUIRE(result + out_total <= ciphertexts || ciphertexts + in_total <= result,
+          "result and ciphertexts must not overlap");
+  std::vector<uint64_t> present;  // the indices of the present diagonals in diagonals[]
+  for (uint64_t r = 0; r < n1 * n2; ++r)
+    if (diagonals[r]) {
+      present.push_back(r);
+      REQUIRE(result + out_total <= diagonals[r] || diagonals[r] + dwords <= result,
+              "result and diagonals[%llu] must not overlap", (unsigned long long)r);
+    }
+  PtrInfo pi;
+  if (int rc = classify_all({result, ciphertexts}, &pi)) return rc;
+  for (uint64_t r : present) {
+    PtrInfo pd;
+    if (int rc = classify_all({result, diagonals[r]}, &pd)) return rc;
+  }
+  if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
+                                 "ciphertexts"))
+    return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(nb);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  for (uint64_t r : present)
+    if (int rc = check_limb_bounds(diagonals[r], 1, nb, n, [&](u64 i) { return bmods[i]; }, pi, "diagonals")) return rc;
+  // the handles that switch keys: the keyed babies', then the keyed giants'
+  std::vector<const hexl_b200_keys*> keyed;
+  for (uint64_t i = 0; i < n1; ++i)
+    if (baby_keys[i]) keyed.push_back(baby_keys[i]);
+  const uint64_t keyed_babies = keyed.size();
+  for (uint64_t j = 0; j < n2; ++j)
+    if (giant_keys[j]) keyed.push_back(giant_keys[j]);
+  const bool rs = rescale != 0;
+  if (pi.where == Where::Host) {
+    // host pointers: the present diagonals go to each device of the split once, before its first ciphertext; each
+    // ciphertext crosses PCIe in once and its result comes back from the same slot
+    std::vector<std::pair<int, uint64_t*>> uploaded;
+    std::vector<std::vector<const uint64_t*>> tables;  // per uploaded device: diagonals[] on that device
+    const int rc = key_switch_host_batch(
+        result, out_words, false, ciphertexts, in_words, in_words, keyed.data(), keyed.size(), batch,
+        [&](int dev, uint64_t* d_res, uint64_t* d_ct, const uint64_t* const* const* dk, cudaStream_t s) {
+          const std::vector<const uint64_t*>* d_diag = nullptr;
+          for (size_t u = 0; u < uploaded.size(); ++u)
+            if (uploaded[u].first == dev) d_diag = &tables[u];
+          const auto babies = per_element(baby_keys, n1, dk);
+          const auto giants = per_element(giant_keys, n2, dk + keyed_babies);
+          return bsgs_hybrid_on_device(dev, d_res, d_ct, d_diag->data(), n, level, q_size, p_size, alpha, rs, h,
+                                       bmods.data(), babies.data(), baby_elts, n1, giants.data(), giant_elts, n2, s);
+        },
+        [&](int dev) -> int {
+          uint64_t* p = nullptr;
+          CU(cudaMalloc(&p, std::max<uint64_t>(1, present.size()) * dwords * sizeof(uint64_t)));
+          uploaded.emplace_back(dev, p);
+          tables.emplace_back(n1 * n2, nullptr);
+          for (size_t k = 0; k < present.size(); ++k) {
+            CU(cudaMemcpy(p + k * dwords, diagonals[present[k]], dwords * sizeof(uint64_t), cudaMemcpyHostToDevice));
+            tables.back()[present[k]] = p + k * dwords;
+          }
+          CU(cudaStreamSynchronize(nullptr));  // the staging streams do not wait for the legacy stream's copies
+          return 0;
+        });
+    for (auto& u : uploaded) {
+      DeviceGuard g;
+      if (g.enter(u.first) == 0) cudaFree(u.second);
+    }
+    return rc;
+  }
+  std::vector<const uint64_t* const*> dk;
+  const uint64_t found = keys_on_device(keyed.data(), keyed.size(), pi.device, &dk);
+  if (found < keyed.size())
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "a key handle holds no copy on the device of the ciphertexts");
+  const auto babies = per_element(baby_keys, n1, dk.data());
+  const auto giants = per_element(giant_keys, n2, dk.data() + keyed_babies);
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = bsgs_hybrid_on_device(pi.device, result + c * out_words, ciphertexts + c * in_words, diagonals, n,
+                                         level, q_size, p_size, alpha, rs, h, bmods.data(), babies.data(), baby_elts,
+                                         n1, giants.data(), giant_elts, n2, (cudaStream_t)stream))
         return rc;
     return 0;
   });

@@ -67,7 +67,8 @@ KsModuli ks_mac_moduli(const uint64_t* moduli, const uint64_t* slots, uint64_t c
 
 int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cnt, uint64_t kms, const uint64_t* ops,
                     uint64_t decomp, uint64_t n, uint64_t kcc, uint64_t* prod, uint64_t prod_stride,
-                    const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s) {
+                    const uint64_t* const* const* keys, const uint64_t* galois_elts, uint64_t elts, cudaStream_t s,
+                    bool accumulate) {
   uint64_t q[kParamBlock];
   for (uint64_t e = 0; e < cnt; ++e) q[e] = hs[e]->q;
   const KsModuli mods = ks_mac_moduli(q, slots, cnt);
@@ -78,7 +79,7 @@ int ks_mac_products(hexl_b200_ntt* const* hs, const uint64_t* slots, uint64_t cn
       KeyPointers kp;
       for (uint64_t j = 0; j < jc; ++j) kp.p[j] = keys[r][j0 + j];
       const cudaError_t e = launch_ks_mac(prod + r * prod_stride, ops + j0 * n, per_mod, kp, n, jc, kcc, kms, cnt,
-                                          mods, j0 != 0, s, galois_elts ? galois_elts[r] : 0);
+                                          mods, accumulate || j0 != 0, s, galois_elts ? galois_elts[r] : 0);
       if (e != cudaSuccess) return cuda_fail(e, "KeySwitch: multiply-accumulate launch");
     }
   return 0;

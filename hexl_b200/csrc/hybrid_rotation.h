@@ -1,6 +1,7 @@
 // Launchers of the two kernels of the hybrid linear transform (seal.cu): the weighted multi-element
-// multiply-accumulate and the weighted permuted sum of the ciphertext's limbs; and of the multiply-accumulate of the
-// multiply-relinearize call, which adds the tensor terms.  All take two-component ciphertexts (key component count 2)
+// multiply-accumulate and the weighted permuted sum of the ciphertext's limbs; of the giant-step sums of the
+// baby-step giant-step transform; and of the multiply-accumulate of the multiply-relinearize call, which adds the
+// tensor terms.  All take two-component ciphertexts (key component count 2)
 // in NTT form, every word canonical, every modulus below 2^61.
 #pragma once
 #include "internal.h"
@@ -38,6 +39,31 @@ struct PermutedSumElts {
 cudaError_t launch_ks_permuted_sum(u64* result, const u64* ct, u64 n, u64 level, u64 i0, u64 count,
                                    const PermutedSumElts& elts, u64 num_elts, const KsModuli& mods, bool accumulate,
                                    cudaStream_t stream);
+
+// Up to kParamBlock present (giant, baby) pairs of one giant step: diag[r] the pair's diagonal at the limb of the
+// block's first modulus, elt[r] the baby's Galois element, prod[r] the index of the baby's stored products among the
+// keyed babies, or kBsgsNoProducts for an identity baby (element 1 without a key).
+constexpr unsigned kBsgsNoProducts = ~0u;
+struct BsgsSumTerms {
+  const u64* diag[kParamBlock];
+  unsigned elt[kParamBlock];
+  unsigned prod[kParamBlock];
+};
+// mode bits: kBsgsKeyedGiant: component 1 goes to (x1, y1) for the giant's own key switch instead of into (X1, Y1);
+// kBsgsStore1: store into (x1, y1) (the giant's first chunk of babies) instead of adding; kBsgsFold: the last sum
+// launch of X with the merged rescale, which adds [P]_{q_i} X_{k,i} into Y's data limbs (mods.m[e].c = [P]_{q_i})
+// and leaves X unwritten.
+enum : int { kBsgsKeyedGiant = 1, kBsgsStore1 = 2, kBsgsFold = 4 };
+// One giant step h over the moduli [b0, b0 + count) of B = {q_0..q_{l-1}, p_0..p_{K-1}} (l = level; mods.m[e] describes
+// modulus b0 + e with a, b = 2^64 mod q and its Shoup factor), every slot l, the sums over the terms r (babies b_r):
+//   X0_i[l]   += sum_r w_r[pi_h(l)] c0_i[pi_{b_r}(pi_h(l))]                       data limbs, x ([k][i][n])
+//   Y0_b[l]   += sum_{r keyed} w_r[pi_h(l)] prod_r[b][0][pi_h(l)]                  every b, y ([b][k][n])
+//   s1_i[l]    = sum_{r identity} w_r[l] c1_i[l],  t1_b[l] = sum_{r keyed} w_r[l] prod_r[b][1][l]
+// s1 and t1 go into X1 and Y1, or into x1 ([i][n]) and y1 ([b][n]) under kBsgsKeyedGiant.  prod_r is
+// prods + terms.prod[r] * prod_stride, laid out [b][k][n].  Everything canonical; ct is two components of level limbs.
+cudaError_t launch_ks_bsgs_sum(u64* x, u64* y, u64* x1, u64* y1, const u64* ct, const u64* prods, u64 prod_stride,
+                               u64 n, u64 level, u64 b0, u64 count, u64 giant, const BsgsSumTerms& terms,
+                               u64 num_terms, const KsModuli& mods, int mode, cudaStream_t stream);
 
 // The tensor terms of the multiply-relinearize call for the first `data` moduli of a mod-up round (the data moduli
 // q_i, i = b0 + e): ct1 and ct2 point at limb b0 of component 0 of the two ciphertexts, component 1 is comp words

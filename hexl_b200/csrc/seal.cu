@@ -246,6 +246,67 @@ __global__ void __launch_bounds__(kThreads)
   out[level * n] = v1;
 }
 
+// ---- The baby-step giant-step linear transform: one giant step's sums over its present babies.
+// A thread owns one slot l of one modulus b = b0 + e of B.  Component 0 is read at pi_h(l), so the giant rotation is
+// applied on load: the diagonal and the stored baby products at pi_h(l), c0 at pi_{b_i}(pi_h(l)) on the data limbs.
+// Component 1 is read at l.  Each of the four sums (data-limb and extended-basis part of each component) takes at most
+// 64 canonical products in 128 bits, which cannot wrap below 2^61, and is reduced once.
+__global__ void __launch_bounds__(kThreads)
+    ks_bsgs_sum_kernel(u64* x, u64* y, u64* x1, u64* y1, const u64* ct, const u64* prods, u64 prod_stride, u64 n,
+                       u64 level, u64 b0, u64 count, unsigned giant, const __grid_constant__ BsgsSumTerms terms,
+                       u64 num_terms, const __grid_constant__ KsModuli mods, int mode) {
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= n * count) return;
+  const u64 e = g / n, l = g - e * n, b = b0 + e;
+  const KsModulus& md = mods.m[e];
+  const int log_n = __ffsll((long long)n) - 1;
+  const unsigned mask = (unsigned)(2 * n - 1);
+  const u64 pl = ntt_source((unsigned)l, giant, mask, log_n);
+  const bool data = b < level;
+  const u64* c0 = ct + b * n;
+  const u64 c1 = data ? ct[(level + b) * n + l] : 0;
+  const u64* prod_b = prods + b * 2 * n;
+  u64 slo0 = 0, shi0 = 0, slo1 = 0, shi1 = 0, tlo0 = 0, thi0 = 0, tlo1 = 0, thi1 = 0;
+  for (unsigned r = 0; r < (unsigned)num_terms; ++r) {  // at most kParamBlock terms per launch
+    const u64* w = terms.diag[r] + e * n;
+    const u64 w0 = w[pl], w1 = w[l];
+    if (data) mac128(w0, c0[ntt_source((unsigned)pl, terms.elt[r], mask, log_n)], slo0, shi0);
+    if (terms.prod[r] != kBsgsNoProducts) {
+      const u64* p = prod_b + terms.prod[r] * prod_stride;
+      mac128(w0, __ldcs(p + pl), tlo0, thi0);
+      mac128(w1, __ldcs(p + n + l), tlo1, thi1);
+    } else if (data) {
+      mac128(w1, c1, slo1, shi1);
+    }
+  }
+  const u64 s0 = reduce128(shi0, slo0, md), s1 = reduce128(shi1, slo1, md);
+  const u64 t0 = reduce128(thi0, tlo0, md), t1 = reduce128(thi1, tlo1, md);
+  const bool keyed = mode & kBsgsKeyedGiant, store1 = mode & kBsgsStore1;
+  u64* yb = y + b * 2 * n + l;
+  u64 v0 = csub(yb[0] + t0, md.q), v1 = yb[n];
+  if (!keyed) v1 = csub(v1 + t1, md.q);
+  if (data) {
+    u64* xb = x + b * n + l;
+    const u64 x0 = csub(xb[0] + s0, md.q);
+    const u64 xs1 = keyed ? xb[level * n] : csub(xb[level * n] + s1, md.q);
+    if (mode & kBsgsFold) {  // the last sum of X: y_{q_i} += [P]_{q_i} X, md.c = [P]_{q_i}; X itself is not stored
+      u64 lo = 0, hi = 0;
+      mac128(md.c, x0, lo, hi);
+      v0 = csub(v0 + reduce128(hi, lo, md), md.q);
+      lo = hi = 0;
+      mac128(md.c, xs1, lo, hi);
+      v1 = csub(v1 + reduce128(hi, lo, md), md.q);
+    } else {
+      xb[0] = x0;
+      if (!keyed) xb[level * n] = xs1;
+    }
+    if (keyed) x1[b * n + l] = store1 ? s1 : csub(x1[b * n + l] + s1, md.q);
+  }
+  if (keyed) y1[b * n + l] = store1 ? t1 : csub(y1[b * n + l] + t1, md.q);
+  yb[0] = v0;
+  yb[n] = v1;
+}
+
 // ---- Multiply and relinearize: the key products of the tensor's last term, plus [P] times its first two terms.
 // A thread owns one slot l of one modulus e and both key components: it reads each digit word once for both, keeps each
 // component's sum unreduced in 128 bits (jcount within the bound of ks_mac_digits_per_launch) and reduces it.  The
@@ -431,6 +492,16 @@ cudaError_t launch_ks_permuted_sum(u64* result, const u64* ct, u64 n, u64 level,
                                    cudaStream_t stream) {
   ks_permuted_sum_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(result, ct, n, level, i0, count, elts,
                                                                         num_elts, mods, accumulate);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ks_bsgs_sum(u64* x, u64* y, u64* x1, u64* y1, const u64* ct, const u64* prods, u64 prod_stride,
+                               u64 n, u64 level, u64 b0, u64 count, u64 giant, const BsgsSumTerms& terms,
+                               u64 num_terms, const KsModuli& mods, int mode, cudaStream_t stream) {
+  ks_bsgs_sum_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(x, y, x1, y1, ct, prods, prod_stride, n, level, b0,
+                                                                    count, (unsigned)giant, terms, num_terms, mods,
+                                                                    mode);
   count_launch();
   return cudaGetLastError();
 }

@@ -787,6 +787,26 @@ inline void LinearTransformHybrid(uint64_t* result, const uint64_t* ciphertexts,
                                                        batch, stream));
 }
 
+// extension: the baby-step giant-step linear transform sum_j sigma_{h_j}(sum_i w_{j,i} (.) sigma_{b_i}(ct)) with
+// hybrid keys, double-hoisted: one mod-up for the babies, sums kept in the extended basis, one final mod-down.
+// diagonals holds num_giant x num_baby pointers (diagonals[j * num_baby + i] null when absent, else (level_size +
+// p_size) x n words in NTT form); a null key with element 1 is an identity term on either side.  The result is stored,
+// 2 x (level_size - rescale) limbs per ciphertext (hexl_b200_linear_transform_hybrid_bsgs has the formula).
+inline void LinearTransformHybridBSGS(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                                      uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                      const KeySwitchKeys* const* baby_keys, const uint64_t* baby_elts,
+                                      uint64_t num_baby, const KeySwitchKeys* const* giant_keys,
+                                      const uint64_t* giant_elts, uint64_t num_giant,
+                                      const uint64_t* const* diagonals, bool rescale, uint64_t batch = 1,
+                                      void* stream = nullptr) {
+  std::vector<const hexl_b200_keys*> babies(num_baby), giants(num_giant);
+  for (uint64_t i = 0; i < num_baby; ++i) babies[i] = baby_keys[i] ? baby_keys[i]->Handle() : nullptr;
+  for (uint64_t j = 0; j < num_giant; ++j) giants[j] = giant_keys[j] ? giant_keys[j]->Handle() : nullptr;
+  b200_detail::Throw(hexl_b200_linear_transform_hybrid_bsgs(
+      result, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, babies.data(), baby_elts, num_baby,
+      giants.data(), giant_elts, num_giant, diagonals, rescale ? 1 : 0, batch, stream));
+}
+
 // extension: ct1 x ct2 relinearized with hybrid keys that switch s^2 to s, for each of `batch` pairs (2 x level_size
 // limbs each), stored into result (2 x (level_size - rescale) limbs per pair); rescale = 1 merges the rescale by the
 // last limb into the mod-down (hexl_b200_multiply_relinearize_hybrid has the formula).  rescale = 0 equals

@@ -466,6 +466,66 @@ int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* cipherte
                                       const hexl_b200_keys* const* galois_keys, const uint64_t* galois_elts,
                                       uint64_t num_elts, const uint64_t* diagonals, uint64_t batch, void* stream);
 
+/* Baby-step giant-step linear transform with hybrid keys, double-hoisted (extension; Bossuat et al., Eurocrypt 2021,
+ * Alg. 6; Lattigo's MultiplyByDiagMatrixBSGS; OpenFHE's EvalFastRotationExt + KeySwitchDown): the plaintext-matrix x
+ * ciphertext product sum_j sigma_{h_j}( sum_i w_{j,i} (.) sigma_{b_i}(ct) ) over a num_giant x num_baby grid of
+ * diagonals, for each of `batch` ciphertexts, with n1 + n2 Galois keys instead of the n1 n2 of
+ * hexl_b200_linear_transform_hybrid.  The baby rotations' mod-up runs once, their products and the inner sums stay in
+ * the extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}}, each giant step takes only its c1 part down to Q, and the result
+ * is rounded once at the end.  The moduli, digits, shape rules, key handles and layouts are those of
+ * hexl_b200_apply_galois_key_switch_hybrid_hoisted: baby_keys[i] switches s(X^{b_i}) to s for b_i = baby_elts[i], and
+ * giant_keys[j] s(X^{h_j}) to s for h_j = giant_elts[j].  A null handle is an identity term, allowed for the element 1
+ * only, on either side.  Every element is odd and in [1, 2n); elements may repeat.  diagonals is a host array of
+ * num_giant x num_baby pointers: diagonals[j * num_baby + i] is null (the pair is absent and costs nothing) or points at
+ * (l + p_size) x n words in NTT form, canonical, limb i < l under q_i and limb l + j under p_j, in the memory kind of
+ * the ciphertexts.  Ciphertext c (two components of l = level_size limbs, NTT form, canonical) is read at
+ * ciphertexts + c * 2 * l * n and its result STORED at result + c * 2 * l' * n, l' = l - rescale.
+ * With the mod-up D_{d,m} of hexl_b200_key_switch_hybrid, prod^b_{m,k} = sum_d pi_b(D_{d,m}(c1)) (.) K_b[d][k][slot(m)]
+ * the products of the hoisted call, and R_j the babies with a diagonal in row j, a pair (X, Y) with X on the data limbs
+ * (from 0) and Y two components over B (from empty):
+ *   x0_j  = sum_{i in R_j} w_{j,i} (.) sigma_{b_i}(c0),  x1_j = sum_{i in R_j, b_i identity} w_{j,i} (.) c1
+ *   y_j,k = sum_{i in R_j, b_i keyed} w_{j,i} (.) prod^{b_i}_k                                     every m in B
+ *   identity giant:  X += (x0_j, x1_j);  Y += (y_j,0, y_j,1)
+ *   keyed giant h:   c1'_j = x1_j + ModDown_P(y_j,1)          (no ModDown when R_j has no keyed baby)
+ *                    X0 += sigma_h(x0_j);  Y0 += sigma_h(y_j,0)   (pi_h on the special limbs too)
+ *                    Y_k += sum_d pi_h(D_{d,m}(c1'_j)) (.) K_h[d][k][slot(m)]  (a fresh mod-up of c1'_j)
+ *   rescale = 0:     result = X + ModDown_P(Y)                  (result = X while Y is empty)
+ *   rescale = 1:     ext_{q_i,k} = Y_{q_i,k} + [P]_{q_i} X_{k,i},  ext_{p_j,k} = Y_{p_j,k};  result = the mod-down of
+ *                    ext by q_{l-1} P of hexl_b200_multiply_relinearize_hybrid (l - 1 limbs)
+ * canonical; a row without a present diagonal adds nothing.  X is kept apart from Y because ModDown_P(P x) need not
+ * be x for K > 1 (its rounded base conversion of zero special limbs gives u P, 0 <= u < K), while
+ * ModDown_P(P x + y) = x + ModDown_P(y) bit for bit.  Hence, bit for bit: with one identity giant (element 1, null key)
+ * this is hexl_b200_linear_transform_hybrid over the babies with the absent diagonals as zero ones; with one identity
+ * baby and every diagonal word 1 it is hexl_b200_linear_transform_hybrid over the giants with unit diagonals, and with
+ * one giant as well, hexl_b200_apply_galois_key_switch_hybrid_hoisted.  It decrypts to
+ * sum_j sigma_{h_j}(sum_i w_{j,i} (.) sigma_{b_i}(phase(ct))), divided by q_{l-1} and rounded with rescale = 1, within
+ * the linear transform's bound plus, per keyed giant, one key switch and the rounding of c1'_j times s.
+ * HEXL_B200_ERR_INVALID_ARG on the refusals of the hoisted call applied to every non-null handle (another shape,
+ * sharded by modulus), a null handle for an element other than 1, rescale other than 0 or 1, rescale = 1 with
+ * level_size < 2 or p_size > 63, a null diagonals array when num_baby x num_giant > 0, and result overlapping the
+ * ciphertexts or a present diagonal.  num_baby = 0, num_giant = 0 or batch = 0 does nothing.  Inputs, the present
+ * diagonals included, are checked below their modulus under hexl_b200_set_debug(1).
+ * On the device, per ciphertext: (1) when some keyed baby has a diagonal, the mod-up of c1 once, and per round the
+ * multiply-accumulates of those babies, their products stored; (2) per giant step with a present diagonal, one sum
+ * launch per block of 64 moduli of B (of the data moduli only when the row has no keyed baby) and chunk of 64 present
+ * babies, which applies pi_h on load; (3) per keyed giant step, the mod-down of y_j,1 into x1_j (one component, none
+ * without a keyed baby), then the mod-up of c1'_j with multiply-accumulates adding into Y through pi_h; (4) the
+ * mod-down of Y, adding into result (none while Y is empty), or with rescale = 1 the [P] X fold in the last sum launch
+ * and the mod-down by q_{l-1} P that stores.  Library scratch: n1' x (l + p_size) x 2 x n words of stored baby
+ * products, n1' the keyed babies with a diagonal (336 MB at n1' = 8, l = 30, K = 10, n = 2^16), plus Y, one round of
+ * converted digits and a few l x n buffers.  Device calls capture into a CUDA graph once the transforms are warm.
+ * Host buffers: the present diagonals go to each device once per call, before its first ciphertext; the ciphertexts
+ * are pipelined and split by ciphertext over the devices of hexl_b200_set_host_devices where every non-null handle
+ * holds a copy.  Managed buffers take the device path.  Not covered: keys sharded by modulus (refused), encoding the
+ * diagonals (pre-rotating them by -h_j is the caller's), and mapping rotation steps to elements. */
+int hexl_b200_linear_transform_hybrid_bsgs(uint64_t* result, const uint64_t* ciphertexts, uint64_t n,
+                                           uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                           const uint64_t* moduli, const hexl_b200_keys* const* baby_keys,
+                                           const uint64_t* baby_elts, uint64_t num_baby,
+                                           const hexl_b200_keys* const* giant_keys, const uint64_t* giant_elts,
+                                           uint64_t num_giant, const uint64_t* const* diagonals, int rescale,
+                                           uint64_t batch, void* stream);
+
 /* Ciphertext multiplication with relinearization by hybrid keys (extension; CKKS HMult: SEAL's multiply + relinearize
  * [+ rescale_to_next], OpenFHE's EvalMult), optionally rescaled in the same mod-down, for each of `batch` pairs.  The
  * moduli, digits and shape rules are those of hexl_b200_key_switch_hybrid with key_component_count = 2; relin_keys is
