@@ -1,5 +1,6 @@
 """The scratch rounds of the RNS composites (hexl_b200/csrc/capi_keyswitch.cu, capi_galois.cu, capi_hybrid.cu) restated
-in Python, and the shapes of tests/test_gpu_composite_rounds.py and tests/test_gpu_hybrid_rounds.py.
+in Python, and the shapes of tests/test_gpu_composite_rounds.py, tests/test_gpu_hybrid_rounds.py and
+tests/test_gpu_bsgs_rounds.py.
 
 Each composite splits one device call into rounds that fit about 256 MiB of pool scratch:
 
@@ -18,6 +19,8 @@ MultiplyRelinearizeHybrid) around one mod-up and one mod-down:
     relin_mac_launches, weighted_mac_launches, ks_mac_launches
                             the multiply-accumulate launches of one round of each call
     hybrid_launches         the kernel launches of one ciphertext of each call, from all of the above
+    bsgs_launches           the same for LinearTransformHybridBSGS: a baby mod-up, per row the sums, per keyed giant
+                            a one-component mod-down and a mod-up, and the final mod-down (bsgs_rows: what it runs)
 
 Every function returns the list of round (or launch) sizes.  SOURCE holds the source file under hexl_b200/csrc and the
 lines of it each formula restates;
@@ -74,6 +77,20 @@ SOURCE = {
                       "const uint64_t per = std::max<uint64_t>(1, kParamBlock / jc);",
                       "for (uint64_t j0 = 0; j0 < D; j0 += jc) {",
                       "for (uint64_t k0 = 0; k0 < keyed.size(); k0 += per) {"]),
+    "bsgs": ("capi_hybrid.cu",
+             ["if (!baby_keys[i]) continue;",                                         # stored: a keyed baby ...
+              "if (diag[j * n1 + i]) {\n        stored[i] = used_keys.size();",       # ... with a diagonal
+              "used_elts.data(), used_keys.size(), s);",                             # their products per round
+              "if (present.empty()) continue;  // an absent row costs nothing",
+              "const uint64_t span = keyed_baby ? nb : level;",
+              "for (uint64_t b0 = 0; b0 < span; b0 += kParamBlock) {",
+              "for (uint64_t r0 = 0; r0 < present.size(); r0 += kParamBlock) {",
+              "if (!keyed_giant) continue;",
+              "if (keyed_baby)\n"
+              "      if (int rc = hybrid_mod_down(dev, x1, y1, tmp, n, level, p_size, 1, h, bmods, true, s))",
+              "stride, &giant_keys[j], &h_elt, 1, s, true);",                         # one set per giant round
+              "if (rescale) return hybrid_mod_down(dev, result, y, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);",
+              "if (!y_used) return 0;"]),
 }
 
 
@@ -168,12 +185,34 @@ def weighted_mac_launches(D, keyed, largest_q):
     return [(j, e) for j in _split(D, jc) for e in _split(keyed, per)]
 
 
+def hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs):
+    """hybrid_mod_up: the target's inverse transform, then per round one base conversion per digit and block of
+    targets, the forward transform of the round's digits and macs(D, largest) multiply-accumulate launches, largest the
+    round's largest modulus"""
+    D = -(-level // alpha)
+    total = sum(ntt(False, cnt) for cnt in _split(level, PARAM_BLOCK))    # the target back to coefficients
+    b0 = 0
+    for cnt in hybrid_mod_up_rounds(n, level, K, alpha):
+        total += sum(len(base_conv_blocks(w, cnt)) for w in hybrid_digit_widths(level, alpha))
+        total += ntt(True, cnt * D) + macs(D, max(basis[b0:b0 + cnt]))
+        b0 += cnt
+    return total
+
+
+def hybrid_mod_down_launches(level, K, kcc, ntt, rescale=False):
+    """hybrid_mod_down of kcc components: the special limbs' inverse transform, then per block of 64 data moduli the
+    rounding base conversions, a forward transform and the finish; with the merged rescale q_{level-1} joins P"""
+    total = ntt(False, (K + int(rescale)) * kcc)
+    for cnt, blocks in zip(_split(level - int(rescale), PARAM_BLOCK), hybrid_mod_down_blocks(level, K, rescale)):
+        total += len(blocks) + ntt(True, cnt * kcc) + 1
+    return total
+
+
 def hybrid_launches(call, n, level, K, alpha, basis, ntt, elts=1, keyed=None, rescale=False, kcc=2):
     """kernel launches of one ciphertext of `call` ("switch", "hoisted", "linear", "mul_relin"): basis holds the moduli
     of B (level data, then K special); ntt(forward, units) is the launch count of one multi-modulus transform of
     `units` polynomials.  "switch" and "hoisted" run `elts` switches over one mod-up; "linear" takes `elts` elements,
     `keyed` of them with keys."""
-    D = -(-level // alpha)
     total = 0
     if call == "hoisted":
         total += elts                                                      # one automorphism launch per element
@@ -181,25 +220,56 @@ def hybrid_launches(call, n, level, K, alpha, basis, ntt, elts=1, keyed=None, re
         total += -(-level // PARAM_BLOCK) * -(-elts // PARAM_BLOCK)        # the permuted sums
         if not keyed:
             return total
-    total += sum(ntt(False, cnt) for cnt in _split(level, PARAM_BLOCK))   # the target back to coefficients
-    b0 = 0
-    for cnt in hybrid_mod_up_rounds(n, level, K, alpha):
-        total += sum(len(base_conv_blocks(w, cnt)) for w in hybrid_digit_widths(level, alpha))
-        total += ntt(True, cnt * D)
-        largest = max(basis[b0:b0 + cnt])
+
+    def macs(D, largest):
         if call == "mul_relin":
-            total += len(relin_mac_launches(D, largest))
-        elif call == "linear":
-            total += len(weighted_mac_launches(D, keyed, largest))
-        else:
-            total += elts * len(ks_mac_launches(D, largest))
-        b0 += cnt
+            return len(relin_mac_launches(D, largest))
+        if call == "linear":
+            return len(weighted_mac_launches(D, keyed, largest))
+        return elts * len(ks_mac_launches(D, largest))
+
+    total += hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs)
     downs = 1 if call in ("linear", "mul_relin") else elts
-    k_down, kk = K + int(rescale), (kcc if call == "switch" else 2)
-    down = ntt(False, k_down * kk)
-    for cnt, blocks in zip(_split(level - int(rescale), PARAM_BLOCK), hybrid_mod_down_blocks(level, K, rescale)):
-        down += len(blocks) + ntt(True, cnt * kk) + 1                       # base conversions, transform, finish
-    return total + downs * down
+    return total + downs * hybrid_mod_down_launches(level, K, kcc if call == "switch" else 2, ntt, rescale)
+
+
+def bsgs_rows(babies, giants, present):
+    """the present babies of each giant's row, and the keyed babies with a diagonal (whose products the baby mod-up
+    stores), in baby order"""
+    rows = [[i for i in range(len(babies)) if present is None or (j, i) in present] for j in range(len(giants))]
+    return rows, [i for i, keyed in enumerate(babies) if keyed and any(i in row for row in rows)]
+
+
+def bsgs_launches(n, level, K, alpha, basis, ntt, babies, giants, present, rescale=False):
+    """LinearTransformHybridBSGS: kernel launches of one ciphertext.  babies[i] (giants[j]) is true for a keyed term,
+    false for an identity one; present is the set of (giant j, baby i) pairs with a diagonal, or None for all of them.
+      - the baby mod-up only when some keyed baby has a pair, storing the products of each such baby per round;
+      - per row with a pair, one sum launch per block of 64 moduli of the span (B with a keyed baby in the row, the
+        data moduli without) and chunk of 64 present babies;
+      - per keyed giant with a pair, the one-component (kcc = 1) mod-down of y_1 when the row has a keyed baby, then a
+        mod-up with one multiply-accumulate set per round;
+      - the final mod-down: none while Y is empty, or over (level - 1, K + 1) with the merged rescale."""
+    rows, stored = bsgs_rows(babies, giants, present)
+    stored = len(stored)
+    total = 0
+    if stored:
+        total += hybrid_mod_up_launches(n, level, K, alpha, basis, ntt,
+                                        lambda D, q: stored * len(ks_mac_launches(D, q)))
+    y_used = False
+    for row, keyed_giant in zip(rows, giants):
+        if not row:
+            continue
+        keyed_baby = any(babies[i] for i in row)
+        span = level + K if keyed_baby else level
+        total += -(-span // PARAM_BLOCK) * -(-len(row) // PARAM_BLOCK)
+        y_used = y_used or keyed_baby or bool(keyed_giant)
+        if keyed_giant:
+            if keyed_baby:
+                total += hybrid_mod_down_launches(level, K, 1, ntt)
+            total += hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, lambda D, q: len(ks_mac_launches(D, q)))
+    if rescale:
+        return total + hybrid_mod_down_launches(level, K, 2, ntt, True)
+    return total + (hybrid_mod_down_launches(level, K, 2, ntt) if y_used else 0)
 
 
 # ------------------------------------------------------------------------------ the GPU test's shapes
@@ -223,3 +293,14 @@ HYBRID_SHAPES = {
     "budget_a3": (17, 30, 3, 3, 50, 50, (30, 28)),      # rounds 25 + 8, and 25 + 6 mixing data and special moduli
     "mixed_chunks": (16, 24, 2, 1, 50, 60, (24,)),      # rounds 21 + 5; multiply-accumulate 1, then 16 + 8 launches
 }
+# the grids of LinearTransformHybridBSGS in tests/test_gpu_bsgs_rounds.py: (keyed babies, keyed giants, present pairs
+# (giant j, baby i), None for all).  BSGS_SPARSE runs at every HYBRID_SHAPES level: the identity baby under the identity
+# giant, keyed babies under it, a keyed giant over the identity baby alone (no kcc = 1 mod-down), a keyed giant over
+# keyed babies (baby 5 repeats baby 1's element), a keyed baby without a diagonal (stored index != baby index) and an
+# absent last row (the rescale folds into row 2, not the last).  BSGS_SWEEP runs at every level of the sweep, its keyed
+# giants over keyed babies; BSGS_BENCH is tools/bsgs_bench.py's full 8 x 8 grid, the first baby and giant identities.
+BSGS_SPARSE = ((False, True, True, True, True, True), (False, True, True, True),
+               {(0, 0), (0, 1), (0, 5), (1, 0), (2, 0), (2, 3), (2, 4), (2, 5)})
+BSGS_SWEEP = ((False, True, True), (False, True, True), {(0, 0), (0, 1), (1, 0), (1, 2), (2, 1)})
+BSGS_BENCH = ((False,) + (True,) * 7, (False,) + (True,) * 7, None)
+BSGS_BENCH_SHAPE = (16, 30, 10, 10, 50, 50, 30)   # (log2 n, L, K, alpha, data bits, special bits, level)

@@ -173,3 +173,148 @@ def test_every_level_sweep_crosses_each_block_boundary():
     assert len(plan.hybrid_mod_down_blocks(29, 10)[0]) == 1 and len(plan.hybrid_mod_down_blocks(30, 10)[0]) == 2
     assert len(plan.hybrid_mod_down_blocks(28, 10, True)[0]) == 1
     assert len(plan.hybrid_mod_down_blocks(29, 10, True)[0]) == 2
+
+
+# ------------------------------------------------------------------------------ LinearTransformHybridBSGS
+def _one(forward, units):
+    return 1
+
+
+def test_bsgs_spot_values():
+    below60, above60 = [(1 << 45) + 1] * 8, [(1 << 61) - 1] * 40
+    n = 1 << 12
+    # (6, 2, 2): one mod-up round of 3 digits (1 + 3 + 1 + 1 launches) and one mod-down block (1 + 1 + 1 + 1)
+    babies, giants = (False, True), (False, True)
+    # row 0: the identity over the identity, 1 sum launch; row 1: keyed over keyed: baby mod-up 6, 1 sum launch over B,
+    # the kcc = 1 mod-down 4, the giant's mod-up 6; the final mod-down 4
+    assert plan.bsgs_launches(n, 6, 2, 2, below60, _one, babies, giants, {(0, 0), (1, 1)}) == 6 + 1 + 1 + 4 + 6 + 4
+    assert plan.bsgs_launches(n, 6, 2, 2, below60, _one, babies, giants, {(0, 0), (1, 1)}, True) == 22
+    # identity rows only: the sums alone, and with the rescale the mod-down by q_5 P of X folded into Y
+    assert plan.bsgs_launches(n, 6, 2, 2, below60, _one, babies, giants, {(0, 0)}) == 1
+    assert plan.bsgs_launches(n, 6, 2, 2, below60, _one, babies, giants, {(0, 0)}, True) == 1 + 4
+    # a keyed giant over the identity baby: no baby mod-up, no kcc = 1 mod-down
+    assert plan.bsgs_launches(n, 6, 2, 2, below60, _one, babies, giants, {(1, 0)}) == 1 + 6 + 4
+    # no pair at all: nothing
+    assert plan.bsgs_launches(n, 6, 2, 2, below60, _one, babies, giants, set()) == 0
+    # 30 one-modulus digits below 2^61: 16 + 14 digits per multiply-accumulate, per stored baby and per giant; 65
+    # babies in a row: two chunks of sums per block of moduli
+    grid = ((True,) * 65, (True,), None)
+    up = 1 + 30 * 1 + 1                                                      # one round of 40 moduli at n = 2^12
+    down1, down2 = 1 + 2 + 1 + 1, 1 + 2 + 1 + 1                              # base_conv_blocks(10, 30) == [29, 1]
+    assert plan.bsgs_launches(n, 30, 10, 1, above60, _one, *grid) == \
+        (up + 65 * 2) + 2 * 1 + down1 + (up + 2) + down2
+    # every launch of a transform counts: the plan asks for each transform's units
+    seen = []
+    plan.bsgs_launches(n, 6, 2, 2, below60, lambda f, u: seen.append((f, u)) or 1, babies, giants, {(1, 1)}, True)
+    assert seen == [(False, 6), (True, 24),                                  # baby mod-up: 8 moduli x 3 digits
+                    (False, 2), (True, 6),                                   # kcc = 1 mod-down: K x 1, 6 x 1
+                    (False, 6), (True, 24),                                  # giant mod-up
+                    (False, 6), (True, 10)]                                  # merged mod-down: (K + 1) x 2, 5 x 2
+
+
+def _bsgs_launches_below_2_60(n, level, K, alpha, bspec, gspec, present, rescale, fwd, inv):
+    """the count tests/test_gpu_bsgs.py derived on its own before the plan held BSGS: moduli below 2^60, so
+    ceil(D / 64) digit chunks per multiply-accumulate, and fwd / inv launches per transform"""
+    import hybrid_exact as hx
+
+    def targets(s):
+        return (480 - 4 * s) // (5 + s)
+
+    def up(macs):
+        groups, nb = hx.digits(level, alpha), level + K
+        ichunk = min(max(1, (256 << 20) // (len(groups) * n * 8)), nb, 64)
+        return inv * -(-level // 64) + sum(sum(-(-min(ichunk, nb - b0) // targets(len(S))) for S in groups)
+                                           + fwd + macs for b0 in range(0, nb, ichunk))
+
+    def down(lv, k):
+        return inv + sum(-(-min(64, lv - i0) // targets(k)) + fwd + 1 for i0 in range(0, lv, 64))
+
+    chunks, nb = -(-(-(-level // alpha)) // 64), level + K
+    stored = [i for i, (_, k) in enumerate(bspec)
+              if k is not None and any((j, i) in present for j in range(len(gspec)))]
+    total = up(len(stored) * chunks) if stored else 0
+    y_used = False
+    for j, (_, gk) in enumerate(gspec):
+        row = [i for i in range(len(bspec)) if (j, i) in present]
+        if not row:
+            continue
+        keyed_baby = any(bspec[i][1] is not None for i in row)
+        total += -(-(nb if keyed_baby else level) // 64) * -(-len(row) // 64)
+        y_used = y_used or keyed_baby or gk is not None
+        if gk is not None:
+            total += (down(level, K) if keyed_baby else 0) + up(chunks)
+    if rescale:
+        return total + down(level - 1, K + 1)
+    return total + (down(level, K) if y_used else 0)
+
+
+def test_bsgs_launches_agree_with_the_earlier_counts():
+    """below 2^60 the plan gives the counts tests/test_gpu_bsgs.py expected from its own formula, on the grids of its
+    test_launch_counts, with transforms of different launch counts in each direction"""
+    n = 1 << 12
+    bspec = [(1, None), (3, 0), (2 * n - 1, 1), (5, 2), (3, 1)]
+    gspec = [(1, None), (9, 0), (25, 1), (2 * n - 1, 2)]
+    sparse = {(0, 0), (0, 1), (0, 2), (0, 4), (1, 0), (2, 0), (2, 1), (2, 3), (2, 4)}
+    many = [(pow(5, i + 1, 2 * n), i % 3) for i in range(66)]
+    grids = [("sparse", bspec, gspec, sparse),
+             ("identity rows only", bspec, [(1, None), (1, None)], {(0, 0), (1, 0)}),
+             ("keyed giants over the identity baby", bspec, gspec, {(1, 0), (2, 0), (3, 0)}),
+             ("66 babies", many, gspec[:2], {(j, i) for j in range(2) for i in range(66)})]
+    for L, K, alpha, level in [(6, 2, 2, 6), (30, 10, 10, 30), (70, 2, 64, 70), (12, 1, 1, 12)]:
+        basis = [(1 << 45) + 1] * (level + K)
+        for name, bspec, gspec, present in grids:
+            for rescale in (False, True):
+                exp = _bsgs_launches_below_2_60(n, level, K, alpha, bspec, gspec, present, rescale, 2, 3)
+                got = plan.bsgs_launches(n, level, K, alpha, basis, lambda f, u: 2 if f else 3,
+                                         [k is not None for _, k in bspec], [k is not None for _, k in gspec],
+                                         present, rescale)
+                assert got == exp, (L, K, alpha, name, rescale)
+
+
+def test_bsgs_grids_have_the_plan_their_names_claim(port):
+    babies, giants, present = plan.BSGS_SPARSE
+    rows, stored = plan.bsgs_rows(babies, giants, present)
+    assert stored == [1, 3, 4, 5] and babies[2]                 # a keyed baby without a diagonal stores nothing
+    assert rows[0] == [0, 1, 5] and not giants[0]              # the identity giant over the identity and keyed babies
+    assert rows[1] == [0] and giants[1]                        # a keyed giant, no kcc = 1 mod-down
+    assert rows[2] == [0, 3, 4, 5] and giants[2]               # a keyed giant over keyed babies
+    assert rows[3] == [] and giants[3]                         # an absent last row: the fold goes to row 2
+    babies, giants, present = plan.BSGS_SWEEP
+    rows, stored = plan.bsgs_rows(babies, giants, present)
+    assert stored == [1, 2] and all(giants[j] and any(babies[i] for i in rows[j]) for j in (1, 2))
+    babies, giants, present = plan.BSGS_BENCH
+    rows, stored = plan.bsgs_rows(babies, giants, present)
+    assert stored == list(range(1, 8)) and all(row == list(range(8)) for row in rows)
+    # tools/bsgs_bench.py's shape: the seven kcc = 1 mod-downs and the final one convert into 29 + 1 targets, the
+    # merged rescale's into 27 + 2
+    logn, L, K, alpha, _, _, level = plan.BSGS_BENCH_SHAPE
+    assert (L, K, alpha, level) == (30, 10, 10, 30)
+    assert plan.hybrid_mod_down_blocks(level, K) == [[29, 1]]
+    assert plan.hybrid_mod_down_blocks(level, K, True) == [[27, 2]]
+    # the giants' mod-ups take the 16 + 8 digit chunks of mixed_chunks' second round as the stored babies' do: one
+    # launch more per stored baby and per keyed giant with a pair than with the moduli below 2^60
+    n, L, K, alpha, mods, levels = _hybrid_mods(port, "mixed_chunks")
+    level = levels[0]
+    basis = mods[:level] + mods[L:]
+    low = [(1 << 50) + 1] * len(basis)
+    for rescale in (False, True):
+        diff = (plan.bsgs_launches(n, level, K, alpha, basis, _one, *plan.BSGS_SPARSE, rescale)
+                - plan.bsgs_launches(n, level, K, alpha, low, _one, *plan.BSGS_SPARSE, rescale))
+        assert diff == 4 + 2
+
+
+def test_bsgs_every_level_sweep_crosses_the_one_component_mod_down_block():
+    """(30, 10, 10): the kcc = 1 mod-down of BSGS_SWEEP's keyed giants converts into one block of 29 targets at level 29
+    and two at level 30, like the final mod-down"""
+    ntt_calls = []
+
+    def ntt(forward, units):
+        ntt_calls.append((forward, units))
+        return 1
+
+    n = 1 << 8
+    for level in (29, 30):
+        ntt_calls.clear()
+        plan.bsgs_launches(n, level, 10, 10, [(1 << 50) + 1] * (level + 10), ntt, *plan.BSGS_SWEEP)
+        assert ntt_calls.count((False, 10)) == 2               # the two keyed giants' kcc = 1 mod-downs
+        assert len(plan.hybrid_mod_down_blocks(level, 10)[0]) == level - 28

@@ -8,7 +8,13 @@ against the existing GPU calls: one identity giant is LinearTransformHybrid over
 with diagonals of ones is LinearTransformHybrid over the giants (with one giant, ApplyGaloisKeySwitchHybridHoisted),
 at N = 2^12 and at N = 2^16, L = 30, alpha = K = 10, and at N = 2^16, L = 30, alpha = 1, where the mod-up takes
 several rounds and eight babies' products are stored.  Device, pageable, pinned, managed and split-host buffers; graph
-replay with new data; launch counts; the refusals; and a C++ caller."""
+replay with new data; launch counts against the plan of tests/composite_plan.py (bsgs_launches); the refusals; and a
+C++ caller.
+
+tests/test_gpu_bsgs_rounds.py holds the production coverage: every HYBRID_SHAPES entry at each of its levels with both
+rescale modes, tools/bsgs_bench.py's full 8 x 8 grid at N = 2^16, every level of two shapes, host batches that wrap
+the staging slots, host calls of different slot sizes in sequence, threads, offset views and the aliasing the API
+allows."""
 import os
 import shutil
 import subprocess
@@ -17,8 +23,10 @@ import numpy as np
 import pytest
 
 import bsgs_exact as bx
-from test_gpu_hybrid_key_switch import SENTINEL, _check, _levels, _ntt_launches, dev, host
-from test_gpu_hybrid_rotation import Case, _mod_down_launches, _mod_up_launches
+import composite_plan as plan
+from test_gpu_hybrid_key_switch import SENTINEL, _check, _levels, dev, host
+from test_gpu_hybrid_rotation import Case
+from test_gpu_hybrid_rounds import _ntt
 
 pytestmark = pytest.mark.gpu
 
@@ -263,43 +271,13 @@ def test_graph_replay(hb, port, buffers_case, rescale):
 
 
 # ------------------------------------------------------------------------------------------------ launch counts
-def bsgs_launches(n, level, K, alpha, bspec, gspec, present, rescale, fwd, inv):
-    """per ciphertext, moduli below 2^60 (ceil(D / 64) digit chunks per multiply-accumulate):
-    - when some keyed baby has a pair, the mod-up of c1 with one multiply-accumulate per stored baby and digit chunk
-      per round;
-    - per row with a pair, one sum launch per block of 64 moduli (of B, or of the data moduli without a keyed baby)
-      and chunk of 64 present babies;
-    - per keyed giant with a pair, the one-component mod-down of y_1 (with a keyed baby only) and a mod-up whose
-      rounds take one multiply-accumulate per digit chunk;
-    - the final mod-down (none while Y is empty), by q_{l-1} P with the rescale."""
-    D = -(-level // alpha)
-    chunks = -(-D // 64)
-    nb = level + K
-    stored = [i for i, (_, k) in enumerate(bspec) if k is not None and any((j, i) in present for j in range(len(gspec)))]
-    total = _mod_up_launches(n, level, K, alpha, fwd, inv, len(stored) * chunks) if stored else 0
-    y_used = False
-    for j, (_, gk) in enumerate(gspec):
-        row = [i for i in range(len(bspec)) if (j, i) in present]
-        if not row:
-            continue
-        keyed_baby = any(bspec[i][1] is not None for i in row)
-        total += -(-(nb if keyed_baby else level) // 64) * -(-len(row) // 64)
-        y_used = y_used or keyed_baby or gk is not None
-        if gk is not None:
-            total += (_mod_down_launches(level, K, fwd, inv) if keyed_baby else 0)
-            total += _mod_up_launches(n, level, K, alpha, fwd, inv, chunks)
-    if rescale:
-        return total + _mod_down_launches(level - 1, K + 1, fwd, inv)
-    return total + (_mod_down_launches(level, K, fwd, inv) if y_used else 0)
-
-
 @pytest.mark.parametrize("L, K, alpha, level", [(6, 2, 2, 6), (30, 10, 10, 30), (70, 2, 64, 70), (12, 1, 1, 12)])
 def test_launch_counts(hb, port, L, K, alpha, level):
     n = 1 << 12
     case = Case(hb, port, L, K, alpha, n, data_bits=(45,), special_bits=(45,), sets=3)
     bspec, gspec = _specs(n)
     ct = dev(case.ciphertexts(level, 2, 1))
-    fwd, inv = _ntt_launches(hb, n, True), _ntt_launches(hb, n, False)
+    ntt = _ntt(hb, n)
     many = [(pow(5, i + 1, 2 * n), i % 3) for i in range(66)]
     cases = [("sparse", bspec, gspec, PRESENT),
              ("identity rows only", bspec, [(1, None), (1, None)], {(0, 0), (1, 0)}),
@@ -316,8 +294,9 @@ def test_launch_counts(hb, port, L, K, alpha, level):
             bsgs(hb, case, out, ct, g, level, bs, gs, rescale, 2)
             torch.cuda.synchronize()
             got = hb.launch_count() - before
-            exp = bsgs_launches(n, level, K, alpha, bs, gs, present, rescale, fwd, inv)
-            assert got == 2 * exp, (name, rescale, got, 2 * exp, fwd, inv)
+            exp = plan.bsgs_launches(n, level, K, alpha, case.basis(level), ntt, [k is not None for _, k in bs],
+                                     [k is not None for _, k in gs], present, rescale)
+            assert got == 2 * exp, (name, rescale, got, 2 * exp)
 
 
 # ------------------------------------------------------------------------------------------------ refusals
