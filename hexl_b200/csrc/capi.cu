@@ -117,33 +117,52 @@ int sync_stage(int dev) {
 }
 
 // ---------------------------------------------------------------- debug checks
-int check_bounds(const u64* p, u64 n, u64 bound, const PtrInfo& pi, const char* what) {
+int check_bounds(const u64* p, u64 n, u64 bound, const PtrInfo& pi, const char* what, void* stream) {
   if (!g_debug.load() || !p) return 0;
   if (pi.where == Where::Host) {
     for (u64 i = 0; i < n; ++i)
       if (p[i] >= bound) return fail(HEXL_B200_ERR_INVALID_ARG, "%s: element %llu exceeds bound", what, (unsigned long long)i);
     return 0;
   }
+  // The check reads the operand in the order of the call's stream, so it sees what the caller queued there before the
+  // call, and the host waits for that stream alone.  A capture cannot be waited for, so it is refused before anything
+  // is queued on it.  (The legacy default stream cannot be captured, and querying it during another thread's capture
+  // would invalidate that capture.)
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (s) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    CU(cudaStreamIsCapturing(s, &cap));
+    if (cap != cudaStreamCaptureStatusNone)
+      return fail(HEXL_B200_ERR_INVALID_ARG,
+                  "%s: the range checks of hexl_b200_set_debug(1) wait for the stream, which is being captured into a "
+                  "CUDA graph: turn debug checks off to capture",
+                  what);
+  }
   DeviceGuard g;
   if (int rc = g.enter(pi.device)) return rc;
   int* flag = nullptr;
-  CU(cudaMalloc(&flag, sizeof(int)));
-  CU(cudaMemset(flag, 0, sizeof(int)));
-  bounds_kernel<<<296, 256>>>(p, n, bound, flag);
-  count_launch();
+  CU(scratch_alloc_async(reinterpret_cast<void**>(&flag), sizeof(int), s));
   int h = 0;
-  cudaError_t e = cudaMemcpy(&h, flag, sizeof(int), cudaMemcpyDeviceToHost);
-  cudaFree(flag);
+  cudaError_t e = cudaMemsetAsync(flag, 0, sizeof(int), s);
+  if (e == cudaSuccess) {
+    bounds_kernel<<<296, 256, 0, s>>>(p, n, bound, flag);
+    count_launch();
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, s);
+  scratch_free_async(flag, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return cuda_fail(e, "bounds check");
   if (h) return fail(HEXL_B200_ERR_INVALID_ARG, "%s: an element exceeds its bound", what);
   return 0;
 }
 
-int debug_bounds(const u64* p, u64 n, u64 bound, const char* what, std::initializer_list<const void*> all) {
+int debug_bounds(const u64* p, u64 n, u64 bound, const char* what, std::initializer_list<const void*> all,
+                 void* stream) {
   if (!g_debug.load()) return 0;
   PtrInfo pi;
   if (int rc = classify_all(all, &pi)) return rc;
-  return check_bounds(p, n, bound, pi, what);
+  return check_bounds(p, n, bound, pi, what, stream);
 }
 
 // ---------------------------------------------------------------- scratch pool

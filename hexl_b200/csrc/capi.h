@@ -296,18 +296,21 @@ int run_host(u64* result, const u64* a, const u64* b, u64 total, u64 unit, MakeL
 }
 
 // ---------------------------------------------------------------- debug checks
-// HEXL_CHECK_BOUNDS analogue (check.hpp:33-36): every element < bound
-int check_bounds(const u64* p, u64 n, u64 bound, const PtrInfo& pi, const char* what);
+// HEXL_CHECK_BOUNDS analogue (check.hpp:33-36): every element < bound.  Device data is checked on the call's
+// `stream`, after what the caller queued there before the call, and the check waits for that stream only; a stream
+// being captured into a CUDA graph is refused (HEXL_B200_ERR_INVALID_ARG) before anything is queued on it.
+int check_bounds(const u64* p, u64 n, u64 bound, const PtrInfo& pi, const char* what, void* stream);
 // check_bounds of p against bound when debug checks are on, classifying the call's pointers `all` first
-int debug_bounds(const u64* p, u64 n, u64 bound, const char* what, std::initializer_list<const void*> all);
+int debug_bounds(const u64* p, u64 n, u64 bound, const char* what, std::initializer_list<const void*> all,
+                 void* stream);
 // check_bounds of `polys` polynomials of `limbs` blocks of `words` words each, back to back: block i < bound(i)
 template <class Bound>
 int check_limb_bounds(const u64* p, u64 polys, u64 limbs, u64 words, Bound&& bound, const PtrInfo& pi,
-                      const char* what) {
+                      const char* what, void* stream) {
   if (!g_debug.load()) return 0;
   for (u64 c = 0; c < polys; ++c)
     for (u64 i = 0; i < limbs; ++i)
-      if (int rc = check_bounds(p + (c * limbs + i) * words, words, bound(i), pi, what)) return rc;
+      if (int rc = check_bounds(p + (c * limbs + i) * words, words, bound(i), pi, what, stream)) return rc;
   return 0;
 }
 

@@ -138,8 +138,8 @@ int hexl_b200_eltwise_add_mod(uint64_t* result, const uint64_t* op1, const uint6
   REQUIRE(n != 0, "Require n != 0");
   REQUIRE(q > 1, "Require modulus > 1");
   REQUIRE(q < (1ull << 63), "Require modulus < 2**63");
-  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1, op2})) return rc;
-  if (int rc = debug_bounds(op2, n, q, "operand2", {result, op1, op2})) return rc;
+  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1, op2}, stream)) return rc;
+  if (int rc = debug_bounds(op2, n, q, "operand2", {result, op1, op2}, stream)) return rc;
   EltParams p{};
   p.result = result; p.a = op1; p.b = op2; p.n = n; p.q = q;
   return eltwise_dispatch(EltOp::AddVV, p, stream);
@@ -153,7 +153,7 @@ int hexl_b200_eltwise_add_mod_scalar(uint64_t* result, const uint64_t* op1, uint
   REQUIRE(q > 1, "Require modulus > 1");
   REQUIRE(q < (1ull << 63), "Require modulus < 2**63");
   REQUIRE(op2 < q, "Require operand2 < modulus");
-  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1})) return rc;
+  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1}, stream)) return rc;
   EltParams p{};
   p.result = result; p.a = op1; p.n = n; p.q = q; p.scalar = op2;
   return eltwise_dispatch(EltOp::AddVS, p, stream);
@@ -166,8 +166,8 @@ int hexl_b200_eltwise_sub_mod(uint64_t* result, const uint64_t* op1, const uint6
   REQUIRE(n != 0, "Require n != 0");
   REQUIRE(q > 1, "Require modulus > 1");
   REQUIRE(q < (1ull << 63), "Require modulus < 2**63");
-  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1, op2})) return rc;
-  if (int rc = debug_bounds(op2, n, q, "operand2", {result, op1, op2})) return rc;
+  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1, op2}, stream)) return rc;
+  if (int rc = debug_bounds(op2, n, q, "operand2", {result, op1, op2}, stream)) return rc;
   EltParams p{};
   p.result = result; p.a = op1; p.b = op2; p.n = n; p.q = q;
   return eltwise_dispatch(EltOp::SubVV, p, stream);
@@ -181,7 +181,7 @@ int hexl_b200_eltwise_sub_mod_scalar(uint64_t* result, const uint64_t* op1, uint
   REQUIRE(q > 1, "Require modulus > 1");
   REQUIRE(q < (1ull << 63), "Require modulus < 2**63");
   REQUIRE(op2 < q, "Require operand2 < modulus");
-  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1})) return rc;
+  if (int rc = debug_bounds(op1, n, q, "operand1", {result, op1}, stream)) return rc;
   EltParams p{};
   p.result = result; p.a = op1; p.n = n; p.q = q; p.scalar = op2;
   return eltwise_dispatch(EltOp::SubVS, p, stream);
@@ -196,8 +196,8 @@ int hexl_b200_eltwise_mult_mod(uint64_t* result, const uint64_t* op1, const uint
   REQUIRE(in_mf == 1 || in_mf == 2 || in_mf == 4, "input_mod_factor must be 1, 2 or 4; got %llu", (unsigned long long)in_mf);
   REQUIRE(q < (1ull << 62), "Require modulus < (1ULL << 62)");
   REQUIRE(in_mf * q < (1ull << 63), "Require input_mod_factor * modulus < (1ULL << 63)");
-  if (int rc = debug_bounds(op1, n, in_mf * q, "operand1", {result, op1, op2})) return rc;
-  if (int rc = debug_bounds(op2, n, in_mf * q, "operand2", {result, op1, op2})) return rc;
+  if (int rc = debug_bounds(op1, n, in_mf * q, "operand1", {result, op1, op2}, stream)) return rc;
+  if (int rc = debug_bounds(op2, n, in_mf * q, "operand2", {result, op1, op2}, stream)) return rc;
   EltParams p = mult_params(q, (int)in_mf);
   p.result = result; p.a = op1; p.b = op2; p.n = n;
   return eltwise_dispatch(EltOp::MultVV, p, stream);
@@ -213,8 +213,8 @@ int hexl_b200_eltwise_fma_mod(uint64_t* result, const uint64_t* arg1, uint64_t a
   REQUIRE(in_mf == 1 || in_mf == 2 || in_mf == 4 || in_mf == 8,
           "input_mod_factor must be 1, 2, 4, or 8. Got %llu", (unsigned long long)in_mf);
   REQUIRE(arg2 < in_mf * q, "arg2 exceeds bound input_mod_factor * modulus");
-  if (int rc = debug_bounds(arg1, n, in_mf * q, "arg1", {result, arg1, arg3})) return rc;
-  if (int rc = debug_bounds(arg3, n, in_mf * q, "arg3", {result, arg1, arg3})) return rc;
+  if (int rc = debug_bounds(arg1, n, in_mf * q, "arg1", {result, arg1, arg3}, stream)) return rc;
+  if (int rc = debug_bounds(arg3, n, in_mf * q, "arg3", {result, arg1, arg3}, stream)) return rc;
   EltParams p{};
   p.result = result; p.a = arg1; p.b = arg3; p.n = n; p.q = q; p.in_mf = (int)in_mf;
   uint64_t s = arg2;  // ReduceMod<in_mf>(arg2), eltwise-fma-mod-internal.hpp:16-17
@@ -295,9 +295,9 @@ static int mont_dispatch(EltOp op, uint64_t* result, const uint64_t* a, const ui
   REQUIRE(r >= 1 && r <= 62, "With r > 62 internal ops might overflow");
   REQUIRE((1ull << r) > q, "Needs R bigger than q.");
   REQUIRE(((q * neg_inv_mod + 1) & ((1ull << r) - 1)) == 0, "neg_inv_mod is not -1/q mod R");
-  if (int rc = debug_bounds(a, n, q, "operand a", {result, a, b})) return rc;
+  if (int rc = debug_bounds(a, n, q, "operand a", {result, a, b}, stream)) return rc;
   if (op == EltOp::MontMult)
-    if (int rc = debug_bounds(b, n, q, "operand b", {result, a, b})) return rc;
+    if (int rc = debug_bounds(b, n, q, "operand b", {result, a, b}, stream)) return rc;
   EltParams p{};
   p.result = result; p.a = a; p.b = b; p.n = n; p.q = q; p.mu = neg_inv_mod & ((1ull << r) - 1); p.shift = r; p.scalar = scalar;
   return eltwise_dispatch(op, p, stream);
@@ -344,8 +344,8 @@ static int rns_eltwise_entry(int op, uint64_t* result, const uint64_t* operand1,
   if (pi.where == Where::Device)
     return run_on_device(pi, stream, [&] {
       auto bound = [&](u64 i) { return moduli[i] * in_mf; };
-      if (int rc = check_limb_bounds(operand1, 1, num_moduli, n_per_modulus, bound, pi, "operand1")) return rc;
-      if (int rc = check_limb_bounds(operand2, 1, num_moduli, n_per_modulus, bound, pi, "operand2")) return rc;
+      if (int rc = check_limb_bounds(operand1, 1, num_moduli, n_per_modulus, bound, pi, "operand1", stream)) return rc;
+      if (int rc = check_limb_bounds(operand2, 1, num_moduli, n_per_modulus, bound, pi, "operand2", stream)) return rc;
       return rns_eltwise_on_device(op, result, operand1, operand2, n_per_modulus, moduli, num_moduli, (int)in_mf,
                                    (cudaStream_t)stream);
     });
@@ -403,8 +403,8 @@ int hexl_b200_poly_multiply_multi(hexl_b200_ntt* const* handles, uint64_t count,
   if (int rc = classify_all({result, a, b}, &pi)) return rc;
   const uint64_t n = handles[0]->n;
   auto bound = [&](u64 i) { return handles[i]->q; };
-  if (int rc = check_limb_bounds(a, 1, count, group * n, bound, pi, "a")) return rc;
-  if (int rc = check_limb_bounds(b, 1, count, group * n, bound, pi, "b")) return rc;
+  if (int rc = check_limb_bounds(a, 1, count, group * n, bound, pi, "a", stream)) return rc;
+  if (int rc = check_limb_bounds(b, 1, count, group * n, bound, pi, "b", stream)) return rc;
   if (pi.where == Where::Device)
     return run_on_device(pi, stream, [&] {
       return poly_multiply_on_device(pi.device, handles, count, result, a, b, group, (cudaStream_t)stream);

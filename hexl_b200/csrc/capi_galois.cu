@@ -110,7 +110,7 @@ int hexl_b200_apply_galois(uint64_t* result, const uint64_t* operand, uint64_t n
           "result and operand must be the same buffer or not overlap");
   PtrInfo pi;
   if (int rc = classify_all({result, operand}, &pi)) return rc;
-  if (int rc = check_limb_bounds(operand, count, rns, n, [&](u64 i) { return moduli[i]; }, pi, "operand")) return rc;
+  if (int rc = check_limb_bounds(operand, count, rns, n, [&](u64 i) { return moduli[i]; }, pi, "operand", stream)) return rc;
   const bool ntt = ntt_form != 0;
   if (pi.where == Where::Device)
     return run_on_device(pi, stream, [&] {
@@ -146,7 +146,7 @@ int hexl_b200_apply_galois_key_switch(uint64_t* ciphertexts, uint64_t n, uint64_
   if (int rc = classify_all({ciphertexts}, &pi)) return rc;
   const uint64_t comp = decomp * n;
   if (int rc = check_limb_bounds(ciphertexts, 2 * batch, decomp, n, [&](u64 i) { return moduli[i]; }, pi,
-                                 "ciphertexts"))
+                                 "ciphertexts", stream))
     return rc;
   // host pointers: only the ciphertext crosses PCIe, and the slot's second buffer holds both permuted components
   if (pi.where == Where::Host)
@@ -202,7 +202,7 @@ int hexl_b200_apply_galois_key_switch_hoisted(uint64_t* results, const uint64_t*
   PtrInfo pi;
   if (int rc = classify_all({results, ciphertexts}, &pi)) return rc;
   if (int rc = check_limb_bounds(ciphertexts, 2 * batch, decomp, n, [&](u64 i) { return moduli[i]; }, pi,
-                                 "ciphertexts"))
+                                 "ciphertexts", stream))
     return rc;
   // host pointers: each input ciphertext crosses PCIe in once and its num_elts rotations come back from the same slot
   if (pi.where == Where::Host)

@@ -523,7 +523,7 @@ int hexl_b200_fast_base_convert(uint64_t* result, const uint64_t* operand, uint6
   REQUIRE(result + out_total <= operand || operand + in_total <= result, "result and operand must not overlap");
   PtrInfo pi;
   if (int rc = classify_all({result, operand}, &pi)) return rc;
-  if (int rc = check_limb_bounds(operand, count, from_count, n, [&](u64 i) { return from_moduli[i]; }, pi, "operand"))
+  if (int rc = check_limb_bounds(operand, count, from_count, n, [&](u64 i) { return from_moduli[i]; }, pi, "operand", stream))
     return rc;
   if (pi.where == Where::Device)
     return run_on_device(pi, stream, [&] {
@@ -546,7 +546,7 @@ int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64
           "result and target must not overlap");
   PtrInfo pi;
   if (int rc = classify_all({result, target}, &pi)) return rc;
-  if (int rc = check_limb_bounds(target, batch, level, n, [&](u64 i) { return moduli[i]; }, pi, "target")) return rc;
+  if (int rc = check_limb_bounds(target, batch, level, n, [&](u64 i) { return moduli[i]; }, pi, "target", stream)) return rc;
   std::vector<uint64_t> bmods;
   CachedNtts h(level + p_size);
   if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
@@ -625,7 +625,7 @@ int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const ui
   PtrInfo pi;
   if (int rc = classify_all({results, ciphertexts}, &pi)) return rc;
   if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
-                                 "ciphertexts"))
+                                 "ciphertexts", stream))
     return rc;
   std::vector<uint64_t> bmods;
   CachedNtts h(level + p_size);
@@ -672,12 +672,12 @@ int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* cipherte
   PtrInfo pi;
   if (int rc = classify_all({result, ciphertexts, diagonals}, &pi)) return rc;
   if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
-                                 "ciphertexts"))
+                                 "ciphertexts", stream))
     return rc;
   std::vector<uint64_t> bmods;
   CachedNtts h(nb);
   if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
-  if (int rc = check_limb_bounds(diagonals, num_elts, nb, n, [&](u64 i) { return bmods[i]; }, pi, "diagonals"))
+  if (int rc = check_limb_bounds(diagonals, num_elts, nb, n, [&](u64 i) { return bmods[i]; }, pi, "diagonals", stream))
     return rc;
   std::vector<const hexl_b200_keys*> keyed;  // the handles of the elements that switch keys
   for (uint64_t r = 0; r < num_elts; ++r)
@@ -762,13 +762,13 @@ int hexl_b200_linear_transform_hybrid_bsgs(uint64_t* result, const uint64_t* cip
     if (int rc = classify_all({result, diagonals[r]}, &pd)) return rc;
   }
   if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
-                                 "ciphertexts"))
+                                 "ciphertexts", stream))
     return rc;
   std::vector<uint64_t> bmods;
   CachedNtts h(nb);
   if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
   for (uint64_t r : present)
-    if (int rc = check_limb_bounds(diagonals[r], 1, nb, n, [&](u64 i) { return bmods[i]; }, pi, "diagonals")) return rc;
+    if (int rc = check_limb_bounds(diagonals[r], 1, nb, n, [&](u64 i) { return bmods[i]; }, pi, "diagonals", stream)) return rc;
   // the handles that switch keys: the keyed babies', then the keyed giants'
   std::vector<const hexl_b200_keys*> keyed;
   for (uint64_t i = 0; i < n1; ++i)
@@ -849,9 +849,9 @@ int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1,
   PtrInfo pi;
   if (int rc = classify_all({result, ct1, ct2}, &pi)) return rc;
   auto bound = [&](u64 i) { return moduli[i]; };
-  if (int rc = check_limb_bounds(ct1, 2 * batch, level, n, bound, pi, "ct1")) return rc;
+  if (int rc = check_limb_bounds(ct1, 2 * batch, level, n, bound, pi, "ct1", stream)) return rc;
   if (ct2 != ct1)
-    if (int rc = check_limb_bounds(ct2, 2 * batch, level, n, bound, pi, "ct2")) return rc;
+    if (int rc = check_limb_bounds(ct2, 2 * batch, level, n, bound, pi, "ct2", stream)) return rc;
   std::vector<uint64_t> bmods;
   CachedNtts h(level + p_size);
   if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;

@@ -431,6 +431,25 @@ static int divide_and_round_on_device(int dev, uint64_t* result, const uint64_t*
   return 0;  // ~Scratch returns the buffers to the pool in stream order
 }
 
+// The caller may have written device (or managed) key sources on any stream of their device, and the upload's copies
+// run on the legacy default stream, which does not wait for non-blocking streams: wait for every device that owns a
+// source before copying from it.
+static int wait_for_key_sources(const uint64_t* const* k_switch_keys, uint64_t decomp) {
+  std::vector<int> owners;
+  for (uint64_t j = 0; j < decomp; ++j) {
+    PtrInfo pi;
+    if (int rc = classify(k_switch_keys[j], &pi)) return rc;
+    if (pi.where == Where::Device && std::find(owners.begin(), owners.end(), pi.device) == owners.end())
+      owners.push_back(pi.device);
+  }
+  for (int dev : owners) {
+    DeviceGuard g;
+    if (int rc = g.enter(dev)) return rc;
+    CU(cudaDeviceSynchronize());
+  }
+  return 0;
+}
+
 }  // namespace hexl_b200
 
 // =============================================================== extern "C"
@@ -442,6 +461,7 @@ int hexl_b200_keys_upload(hexl_b200_keys** out, const uint64_t* const* k_switch_
   *out = nullptr;
   REQUIRE(n >= 1 && decomp >= 1 && kcc >= 1 && key_modulus_size >= 1, "Require non-zero sizes");
   for (uint64_t j = 0; j < decomp; ++j) REQUIRE(k_switch_keys[j] != nullptr, "Require k_switch_keys[j] != nullptr");
+  if (int rc = wait_for_key_sources(k_switch_keys, decomp)) return rc;
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
   std::sort(devs.begin(), devs.end());
@@ -495,6 +515,7 @@ int hexl_b200_keys_upload_sharded(hexl_b200_keys** out, const uint64_t* const* k
   REQUIRE(n >= 2 && !(n & (n - 1)), "Require n a power of two");
   REQUIRE(decomp >= 1 && kcc >= 1 && key_modulus_size >= decomp + 1, "Require decomp, kcc >= 1 and key_modulus_size > decomp");
   for (uint64_t j = 0; j < decomp; ++j) REQUIRE(k_switch_keys[j] != nullptr, "Require k_switch_keys[j] != nullptr");
+  if (int rc = wait_for_key_sources(k_switch_keys, decomp)) return rc;
   std::vector<int> devs;
   if (int rc = host_devices(&devs)) return rc;
   const uint64_t rns = decomp + 1;
@@ -662,7 +683,7 @@ int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand,
   CachedNtts h(ntt_form ? rns : 0);
   for (uint64_t i = 0; i < h.h.size(); ++i)
     if (int rc = h.load(i, n, moduli[i])) return rc;
-  if (int rc = check_limb_bounds(operand, count, rns, n, [&](u64 i) { return moduli[i]; }, pi, "operand")) return rc;
+  if (int rc = check_limb_bounds(operand, count, rns, n, [&](u64 i) { return moduli[i]; }, pi, "operand", stream)) return rc;
   const bool ntt = ntt_form != 0;
   if (pi.where == Where::Device)
     return run_on_device(pi, stream, [&] {

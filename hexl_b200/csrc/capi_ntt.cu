@@ -231,7 +231,7 @@ static int ntt_compute(bool forward, hexl_b200_ntt* h, uint64_t* result, const u
   if (batch == 0) return 0;
   PtrInfo pi;
   if (int rc = classify_all({result, operand}, &pi)) return rc;
-  if (int rc = check_bounds(operand, batch * h->n, h->q * in_mf, pi, "operand")) return rc;
+  if (int rc = check_bounds(operand, batch * h->n, h->q * in_mf, pi, "operand", stream)) return rc;
   const uint64_t n = h->n;
   auto launch = [&](const NttDeviceTables& t, u64* r, const u64* a, u64 polys, cudaStream_t s) {
     return forward ? launch_ntt_forward(t, r, a, (int)in_mf, (int)out_mf, polys, s)
@@ -273,7 +273,7 @@ static int ntt_compute_multi(bool forward, hexl_b200_ntt* const* handles, uint64
   if (int rc = classify_all({result, operand}, &pi)) return rc;
   const uint64_t n = handles[0]->n;
   if (int rc = check_limb_bounds(operand, 1, count, group * n, [&](u64 i) { return handles[i]->q * in_mf; }, pi,
-                                 "operand"))
+                                 "operand", stream))
     return rc;
   if (pi.where == Where::Host)  // staged, chunked and (with host devices set) split across GPUs like a single-modulus call
     return run_host_rns(forward ? RnsJob::NttFwd : RnsJob::NttInv, handles, nullptr, count, group * n, n, (int)in_mf,

@@ -32,6 +32,14 @@
  *    Cheap checks (null, n == 0, mod factors, modulus range) are always on;
  *    the O(n) input-range checks only when hexl_b200_set_debug(1) was called
  *    (the reference does them only in HEXL_DEBUG builds, check.hpp:12-44).
+ *    On device pointers the range checks run on `stream`, after the work the
+ *    caller queued there, and the host waits for the checks (that stream
+ *    only) before the call goes on or refuses: the work queued before a debug
+ *    call is complete when it returns.  The result itself is still computed
+ *    asynchronously on `stream`, as without the checks.  A debug call on a
+ *    stream that is being captured into a CUDA graph is refused with
+ *    HEXL_B200_ERR_INVALID_ARG before anything is queued, and the capture
+ *    stays valid; turn the checks off to capture.
  */
 #ifndef HEXL_B200_H
 #define HEXL_B200_H
@@ -294,7 +302,10 @@ int hexl_b200_apply_galois(uint64_t* result, const uint64_t* operand, uint64_t n
  * against them: ciphertext c uses result + c * key_component_count * decomp * n and t_target + c * decomp * n.
  * Host buffers are pipelined (copies of one ciphertext under the kernels of its neighbours) and split across the
  * devices holding the keys; device buffers run on `stream` on their own device.  Moduli, exactness and the difference
- * from the reference are as for hexl_b200_key_switch, sharded handles included. */
+ * from the reference are as for hexl_b200_key_switch, sharded handles included.
+ * The upload (sharded or not) is synchronous: it first waits for every device that owns a device or managed key
+ * buffer (cudaDeviceSynchronize there), so keys the caller has just written on any stream of that device, blocking or
+ * not, are the ones copied; the handle is complete when the call returns. */
 typedef struct hexl_b200_keys hexl_b200_keys;
 int hexl_b200_keys_upload(hexl_b200_keys** out, const uint64_t* const* k_switch_keys, uint64_t n,
                           uint64_t decomp_modulus_size, uint64_t key_modulus_size, uint64_t key_component_count);
