@@ -137,6 +137,8 @@ _sig("hexl_b200_linear_transform_hybrid_bsgs", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _int, _u64, _vp])
 _sig("hexl_b200_multiply_relinearize_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
+_sig("hexl_b200_multiply_relinearize_sum_hybrid", _int,
+     [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -739,4 +741,43 @@ def MultiplyRelinearizeHybrid(result, ct1, ct2, n, level_size, q_size, p_size, d
                                                       mods.ctypes.data,
                                                       relin_keys._h if relin_keys is not None else None,
                                                       int(bool(rescale)), batch, _stream(stream, rc or ac or bc)))
+    return result
+
+
+def MultiplyRelinearizeSumHybrid(result, ct1, ct2, n, level_size, q_size, p_size, digit_size, moduli,
+                                 relin_keys: KeySwitchKeys, rescale=False, batch=1, stream=None):
+    """sum_r ct1_r x ct2_r relinearized once with hybrid keys (hexl_b200_multiply_relinearize_sum_hybrid): ct1 and ct2
+    list batch x num_pairs ciphertexts (flat, entry c * num_pairs + r = pair r of output c, or one list per output),
+    each 2*level_size*n words; output c is stored at result[c * 2*l'*n:], l' = level_size - rescale.  relin_keys
+    switches s^2 to s.  num_pairs = 1 is MultiplyRelinearizeHybrid bit for bit; rescale=False is DyadicMultiply of every
+    pair, the sums and KeySwitchHybrid bit for bit.  Entries may repeat, and ct1[x] may be ct2[x]."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result)
+
+    def flat(cts):
+        return [x for row in cts for x in row] if cts and isinstance(cts[0], (list, tuple)) else list(cts)
+
+    a, b = flat(ct1), flat(ct2)
+    if len(a) != len(b):
+        raise HexlB200Error(-1, f"ct1 lists {len(a)} ciphertexts and ct2 {len(b)}")
+    if batch and len(a) % batch:
+        raise HexlB200Error(-1, f"{len(a)} pairs do not split into {batch} outputs")
+    pairs = len(a) // batch if batch else 0
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size)
+    _need("result", rn, batch * 2 * (level_size - int(bool(rescale))) * n)
+    ptrs, any_cuda = [[], []], bool(rc)
+    for side, cts in enumerate((a, b)):
+        for x, ct in enumerate(cts):
+            p, cn, cc = _buf(ct)
+            if p is not None:
+                _need(f"ct{side + 1}[{x}]", cn, per)
+            ptrs[side].append(p)
+            any_cuda = any_cuda or bool(cc)
+    t1 = (_vp * max(1, len(a)))(*ptrs[0])
+    t2 = (_vp * max(1, len(b)))(*ptrs[1])
+    _check(_lib.hexl_b200_multiply_relinearize_sum_hybrid(rp, t1, t2, pairs, n, level_size, q_size, p_size,
+                                                          digit_size, mods.ctypes.data,
+                                                          relin_keys._h if relin_keys is not None else None,
+                                                          int(bool(rescale)), batch, _stream(stream, any_cuda)))
     return result

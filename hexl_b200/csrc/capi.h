@@ -406,7 +406,8 @@ int key_switch_elts_on_device(int dev, uint64_t* const* results, const uint64_t*
                               uint64_t key_modulus_size, uint64_t rns, uint64_t kcc, const uint64_t* moduli,
                               const uint64_t* const* const* d_key_ptrs, const uint64_t* galois_elts, uint64_t elts,
                               const uint64_t* modswitch, cudaStream_t s);
-// run(dev, device result block, device input block, the key handles' copies on dev, stream): one ciphertext's switch.
+// run(dev, device result block, device input block, the key handles' copies on dev, stream): one ciphertext's switch,
+// called for the ciphertexts in order, 0 to batch - 1.
 // prepare(dev) (optional) runs once on each device of the split, with it current, before its first ciphertext.
 // in2 (optional): a second input of in_words words per ciphertext, copied into the input block after the first.
 using HostSwitch = std::function<int(int, uint64_t*, uint64_t*, const uint64_t* const* const*, cudaStream_t)>;

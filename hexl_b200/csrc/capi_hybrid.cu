@@ -1,8 +1,8 @@
 // Hybrid key switching (OpenFHE's KeySwitchHYBRID): digits of up to 64 data moduli and up to 64 special primes, the
 // mod-up and the mod-down by fast base conversion (rns.cu); the base conversion on its own; and the rotations with
 // hybrid keys: hoisted, the diagonal-weighted sum of rotations under one mod-down (the linear transform) and its
-// double-hoisted baby-step giant-step form; and the ciphertext product relinearized with hybrid keys, its rescale
-// optionally merged into the mod-down.
+// double-hoisted baby-step giant-step form; and the ciphertext product, or a sum of such products, relinearized with
+// hybrid keys, its rescale optionally merged into the mod-down.
 #include <cstdio>
 #include <numeric>
 
@@ -389,11 +389,14 @@ static int bsgs_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct, 
 // limbs): the mod-up of a1 (.) b1, multiplied in the mod-up's first inverse transform; per round, the relinearization
 // multiply-accumulate, whose storing launch adds [P] (a0 b0, a0 b1 + a1 b0) on the data moduli; and one mod-down,
 // by P or, with rescale, by q_{level-1} P (q_{level-1} is the limb of B right before the special limbs).  Scratch: one
-// round of transformed digits plus (level + K) x 2 x n words of products.
+// round of transformed digits plus (level + K) x 2 x n words of products.  sum (nullptr: none) holds the tensor
+// (d0, d1, t) already formed ([3][level][n], canonical): the mod-up then reads t, the storing launches read d0 and d1,
+// and ct1 and ct2 are not read.
 static int multiply_relinearize_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct1, const uint64_t* ct2,
                                                  uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size,
                                                  uint64_t alpha, bool rescale, const CachedNtts& h,
-                                                 const uint64_t* bmods, const uint64_t* const* keys, cudaStream_t s) {
+                                                 const uint64_t* bmods, const uint64_t* const* keys, cudaStream_t s,
+                                                 const uint64_t* sum = nullptr) {
   const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, comp = level * n;
   Scratch ws(s);
   uint64_t *prod = nullptr, *tmp = nullptr;
@@ -402,8 +405,12 @@ static int multiply_relinearize_hybrid_on_device(int dev, uint64_t* result, cons
   auto mac = [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) -> int {
     const KsModuli mods = ks_mac_moduli(bmods + b0, slots, cnt);
     RelinTensor tensor{};
-    tensor.ct1 = ct1 + b0 * n;
-    tensor.ct2 = ct2 + b0 * n;
+    if (sum) {
+      tensor.sum = sum + b0 * n;
+    } else {
+      tensor.ct1 = ct1 + b0 * n;
+      tensor.ct2 = ct2 + b0 * n;
+    }
     tensor.comp = comp;
     tensor.data = b0 < level ? std::min(cnt, level - b0) : 0;
     for (uint64_t e = 0; e < tensor.data; ++e) {
@@ -423,10 +430,45 @@ static int multiply_relinearize_hybrid_on_device(int dev, uint64_t* result, cons
     }
     return 0;
   };
-  if (int rc = hybrid_mod_up(dev, ct1 + comp, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s, ct2 + comp))
-    return rc;
+  const int up = sum ? hybrid_mod_up(dev, sum + 2 * comp, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s)
+                     : hybrid_mod_up(dev, ct1 + comp, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s, ct2 + comp);
+  if (up) return up;
   if (rescale) return hybrid_mod_down(dev, result, prod, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);
   return hybrid_mod_down(dev, result, prod, tmp, n, level, p_size, 2, h, bmods, false, s);
+}
+
+// The sum over `pairs` pairs of ciphertexts (ct1[r], ct2[r], laid out as above) of their products, relinearized once
+// into result.  One pair is multiply_relinearize_hybrid_on_device.  Otherwise the tensor terms of every pair are summed
+// into scratch (d0, d1, t) ([3][level][n]) by one launch per block of 64 data limbs and chunk of kRelinSumPairs pairs,
+// and the single relinearization reads the sums: the mod-up of t, the multiply-accumulate adding [P] (d0, d1) and one
+// mod-down.  Scratch: 3 x level x n words, plus what the single product takes.
+static int multiply_relinearize_sum_hybrid_on_device(int dev, uint64_t* result, const uint64_t* const* ct1,
+                                                     const uint64_t* const* ct2, uint64_t pairs, uint64_t n,
+                                                     uint64_t level, uint64_t q_size, uint64_t p_size, uint64_t alpha,
+                                                     bool rescale, const CachedNtts& h, const uint64_t* bmods,
+                                                     const uint64_t* const* keys, cudaStream_t s) {
+  if (pairs == 1)
+    return multiply_relinearize_hybrid_on_device(dev, result, ct1[0], ct2[0], n, level, q_size, p_size, alpha, rescale,
+                                                 h, bmods, keys, s);
+  Scratch ws(s);
+  uint64_t* sum = nullptr;
+  if (int rc = ws.get(&sum, 3 * level * n)) return rc;  // [d0, d1, t][i][n]
+  for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
+    const uint64_t cnt = std::min<uint64_t>(kParamBlock, level - i0);
+    const KsModuli mods = ks_mac_moduli(bmods + i0, nullptr, cnt);
+    for (uint64_t r0 = 0; r0 < pairs; r0 += kRelinSumPairs) {
+      const uint64_t rcnt = std::min<uint64_t>(kRelinSumPairs, pairs - r0);
+      RelinSumPairs chunk{};
+      for (uint64_t r = 0; r < rcnt; ++r) {
+        chunk.ct1[r] = ct1[r0 + r];
+        chunk.ct2[r] = ct2[r0 + r];
+      }
+      const cudaError_t e = launch_relin_tensor_sum(sum, n, level, i0, cnt, chunk, rcnt, mods, r0 != 0, s);
+      if (e != cudaSuccess) return cuda_fail(e, "MultiplyRelinearizeSumHybrid: tensor sum launch");
+    }
+  }
+  return multiply_relinearize_hybrid_on_device(dev, result, nullptr, nullptr, n, level, q_size, p_size, alpha, rescale,
+                                               h, bmods, keys, s, sum);
 }
 
 // The shape rules of hexl_b200_key_switch_hybrid, without the key handle
@@ -878,6 +920,100 @@ int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1,
       if (int rc = multiply_relinearize_hybrid_on_device(pi.device, result + c * out_words, ct1 + c * in_words,
                                                          ct2 + c * in_words, n, level, q_size, p_size, alpha, rs, h,
                                                          bmods.data(), dk[0], (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+int hexl_b200_multiply_relinearize_sum_hybrid(uint64_t* result, const uint64_t* const* ct1, const uint64_t* const* ct2,
+                                              uint64_t num_pairs, uint64_t n, uint64_t level_size, uint64_t q_size,
+                                              uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                              const hexl_b200_keys* relin_keys, int rescale, uint64_t batch,
+                                              void* stream) {
+  const uint64_t level = level_size, alpha = digit_size, k = num_pairs, total = batch * num_pairs;
+  REQUIRE(result && moduli && relin_keys, "Require non-null arguments");
+  REQUIRE(total == 0 || (ct1 && ct2), "Require ct1, ct2 != nullptr");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (int rc = hybrid_handle_check(relin_keys, n, q_size, p_size, alpha, 2, "relin_keys")) return rc;
+  REQUIRE(rescale == 0 || rescale == 1, "Require rescale = 0 or 1");
+  REQUIRE(!rescale || level >= 2, "rescale = 1 requires level_size >= 2");
+  REQUIRE(!rescale || p_size < (uint64_t)kParamBlock, "rescale = 1 requires p_size <= %d", kParamBlock - 1);
+  if (total == 0) return 0;
+  const uint64_t in_words = 2 * level * n, out_words = 2 * (level - rescale) * n, out_total = batch * out_words;
+  // the distinct input ciphertexts, each read (and checked, and on host buffers uploaded) once
+  std::vector<const uint64_t*> inputs;
+  for (uint64_t x = 0; x < total; ++x) {
+    REQUIRE(ct1[x] && ct2[x], "Require ct1[%llu], ct2[%llu] != nullptr", (unsigned long long)x, (unsigned long long)x);
+    inputs.push_back(ct1[x]);
+    inputs.push_back(ct2[x]);
+  }
+  std::sort(inputs.begin(), inputs.end());
+  inputs.erase(std::unique(inputs.begin(), inputs.end()), inputs.end());
+  for (const uint64_t* p : inputs)
+    REQUIRE(result + out_total <= p || p + in_words <= result, "result must not overlap an input ciphertext");
+  PtrInfo pi;
+  if (int rc = classify_all({result, inputs[0]}, &pi)) return rc;
+  for (const uint64_t* p : inputs) {
+    PtrInfo pp;
+    if (int rc = classify_all({result, p}, &pp)) return rc;
+    pi.managed = pi.managed || pp.managed;
+  }
+  for (const uint64_t* p : inputs)
+    if (int rc = check_limb_bounds(p, 2, level, n, [&](u64 i) { return moduli[i]; }, pi, "an input ciphertext", stream))
+      return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(level + p_size);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  const bool rs = rescale != 0;
+  if (pi.where == Where::Host) {
+    // host pointers: the distinct inputs go to each device of the split once, before its first output; each output is
+    // computed in a staging slot and comes back from it.  key_switch_host_batch runs the outputs in order, so the
+    // calls of `run` count them.
+    std::vector<uint64_t> slot1(total), slot2(total);  // entry x's index among the distinct inputs
+    for (uint64_t x = 0; x < total; ++x) {
+      slot1[x] = std::lower_bound(inputs.begin(), inputs.end(), ct1[x]) - inputs.begin();
+      slot2[x] = std::lower_bound(inputs.begin(), inputs.end(), ct2[x]) - inputs.begin();
+    }
+    std::vector<std::pair<int, uint64_t*>> uploaded;
+    uint64_t c = 0;
+    const int rc = key_switch_host_batch(
+        result, out_words, false, nullptr, 0, 0, &relin_keys, 1, batch,
+        [&](int dev, uint64_t* d_res, uint64_t*, const uint64_t* const* const* dk, cudaStream_t s) {
+          const uint64_t* base = nullptr;
+          for (auto& u : uploaded)
+            if (u.first == dev) base = u.second;
+          std::vector<const uint64_t*> a(k), b(k);
+          for (uint64_t r = 0; r < k; ++r) {
+            a[r] = base + slot1[c * k + r] * in_words;
+            b[r] = base + slot2[c * k + r] * in_words;
+          }
+          ++c;
+          return multiply_relinearize_sum_hybrid_on_device(dev, d_res, a.data(), b.data(), k, n, level, q_size, p_size,
+                                                           alpha, rs, h, bmods.data(), dk[0], s);
+        },
+        [&](int dev) -> int {
+          uint64_t* p = nullptr;
+          CU(cudaMalloc(&p, inputs.size() * in_words * sizeof(uint64_t)));
+          uploaded.emplace_back(dev, p);
+          for (size_t i = 0; i < inputs.size(); ++i)
+            CU(cudaMemcpy(p + i * in_words, inputs[i], in_words * sizeof(uint64_t), cudaMemcpyHostToDevice));
+          CU(cudaStreamSynchronize(nullptr));  // the staging streams do not wait for the legacy stream's copies
+          return 0;
+        });
+    for (auto& u : uploaded) {
+      DeviceGuard g;
+      if (g.enter(u.first) == 0) cudaFree(u.second);
+    }
+    return rc;
+  }
+  std::vector<const uint64_t* const*> dk;
+  if (keys_on_device(&relin_keys, 1, pi.device, &dk) < 1)
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "relin_keys holds no copy on the device of the ciphertexts");
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = multiply_relinearize_sum_hybrid_on_device(pi.device, result + c * out_words, ct1 + c * k,
+                                                             ct2 + c * k, k, n, level, q_size, p_size, alpha, rs, h,
+                                                             bmods.data(), dk[0], (cudaStream_t)stream))
         return rc;
     return 0;
   });

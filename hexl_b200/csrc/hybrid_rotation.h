@@ -1,7 +1,7 @@
 // Launchers of the two kernels of the hybrid linear transform (seal.cu): the weighted multi-element
 // multiply-accumulate and the weighted permuted sum of the ciphertext's limbs; of the giant-step sums of the
-// baby-step giant-step transform; and of the multiply-accumulate of the multiply-relinearize call, which adds the
-// tensor terms.  All take two-component ciphertexts (key component count 2)
+// baby-step giant-step transform; of the multiply-accumulate of the multiply-relinearize call, which adds the
+// tensor terms; and of the tensor sums of a sum of products.  All take two-component ciphertexts (key component count 2)
 // in NTT form, every word canonical, every modulus below 2^61.
 #pragma once
 #include "internal.h"
@@ -67,21 +67,39 @@ cudaError_t launch_ks_bsgs_sum(u64* x, u64* y, u64* x1, u64* y1, const u64* ct, 
 
 // The tensor terms of the multiply-relinearize call for the first `data` moduli of a mod-up round (the data moduli
 // q_i, i = b0 + e): ct1 and ct2 point at limb b0 of component 0 of the two ciphertexts, component 1 is comp words
-// further, and p[e] = [P]_{q_i} for P the product of the special primes.
+// further, and p[e] = [P]_{q_i} for P the product of the special primes.  sum (nullptr: none) holds (d0, d1) already
+// formed, canonical, laid out like ct1 (d1 comp words after d0); ct1 and ct2 are then not read.
 struct RelinTensor {
   const u64* ct1;
   const u64* ct2;
   u64 comp;
   u64 data;
   u64 p[kParamBlock];
+  const u64* sum;
 };
 // For the `count` moduli of a mod-up round (mods as for launch_ks_mac), every slot l and both key components k:
 //   prod[e][k][l] (+)= sum_{j < jcount} ops[e][j][l] keys.p[j][k][c_e][l]  (+ [P]_{q_i} d_k[i][l] when storing and
 //                      e < tensor.data)   mod q_e,
-// d_0 = a0 b0 and d_1 = a0 b1 + a1 b0 at limb i = b0 + e, (a0, a1) = ct1, (b0, b1) = ct2.  The digit sum stays
-// unreduced in 128 bits (the bound of ks_mac_digits_per_launch); the tensor term is reduced on its own and added mod q.
+// d_0 = a0 b0 and d_1 = a0 b1 + a1 b0 at limb i = b0 + e, (a0, a1) = ct1, (b0, b1) = ct2, or d_k read from tensor.sum.
+// The digit sum stays unreduced in 128 bits (the bound of ks_mac_digits_per_launch); the tensor term is reduced on its
+// own and added mod q.
 cudaError_t launch_ks_relin_mac(u64* prod, const u64* ops, u64 ops_stride, const KeyPointers& keys, u64 n, u64 jcount,
                                 u64 key_modulus_size, u64 count, const KsModuli& mods, const RelinTensor& tensor,
                                 bool accumulate, cudaStream_t stream);
+
+// Up to kRelinSumPairs pairs of ciphertexts of one sum of products: ct1[r] and ct2[r] point at pair r's ciphertexts
+// (two components of `level` limbs each).  d1 takes two products per pair, so a launch's 128-bit sums hold at most 64
+// products of canonical words, which cannot wrap below 2^61.
+constexpr int kRelinSumPairs = 32;
+struct RelinSumPairs {
+  const u64* ct1[kRelinSumPairs];
+  const u64* ct2[kRelinSumPairs];
+};
+// For the data limbs [i0, i0 + count) (mods.m[e] describing limb i0 + e with a, b = 2^64 mod q and its Shoup factor),
+// every slot l, over the num_pairs pairs r, (a0, a1) = ct1[r], (b0, b1) = ct2[r]:
+//   out[0][i][l] (+)= sum_r a0 b0,  out[1][i][l] (+)= sum_r (a0 b1 + a1 b0),  out[2][i][l] (+)= sum_r a1 b1   mod q_i
+// canonical; out is [3][level][n]; accumulate adds into out (later chunks of pairs), else stores.
+cudaError_t launch_relin_tensor_sum(u64* out, u64 n, u64 level, u64 i0, u64 count, const RelinSumPairs& pairs,
+                                    u64 num_pairs, const KsModuli& mods, bool accumulate, cudaStream_t stream);
 
 }  // namespace hexl_b200

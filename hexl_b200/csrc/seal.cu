@@ -336,15 +336,20 @@ __global__ void __launch_bounds__(kThreads)
     v1 = csub(v1 + out[n], md.q);
   } else if (e < tensor.data) {
     const u64 s = e * n + l;
-    const u64 a0 = tensor.ct1[s], a1 = tensor.ct1[s + tensor.comp];
-    const u64 b0 = tensor.ct2[s], b1 = tensor.ct2[s + tensor.comp];
-    u64 lo = 0, hi = 0;
-    mac128(a0, b0, lo, hi);
-    const u64 d0 = reduce128(hi, lo, md);
-    lo = hi = 0;
-    mac128(a0, b1, lo, hi);
-    mac128(a1, b0, lo, hi);
-    const u64 d1 = reduce128(hi, lo, md);
+    u64 d0, d1, lo = 0, hi = 0;
+    if (tensor.sum) {
+      d0 = tensor.sum[s];
+      d1 = tensor.sum[s + tensor.comp];
+    } else {
+      const u64 a0 = tensor.ct1[s], a1 = tensor.ct1[s + tensor.comp];
+      const u64 b0 = tensor.ct2[s], b1 = tensor.ct2[s + tensor.comp];
+      mac128(a0, b0, lo, hi);
+      d0 = reduce128(hi, lo, md);
+      lo = hi = 0;
+      mac128(a0, b1, lo, hi);
+      mac128(a1, b0, lo, hi);
+      d1 = reduce128(hi, lo, md);
+    }
     const u64 P = tensor.p[e];
     lo = hi = 0;
     mac128(P, d0, lo, hi);
@@ -355,6 +360,39 @@ __global__ void __launch_bounds__(kThreads)
   }
   out[0] = v0;
   out[n] = v1;
+}
+
+// ---- A sum of ciphertext products: the tensor terms of a chunk of pairs, summed before one relinearization.
+// A thread owns one slot l of one data limb i = i0 + e and reads the four words of every pair there.  d0 and t take one
+// product per pair, d1 two: at most kRelinSumPairs pairs keep each 128-bit sum within 64 products of canonical words,
+// exact below 2^61.  Each sum is reduced once; a later chunk adds mod q into what the first stored.
+__global__ void __launch_bounds__(kThreads)
+    relin_tensor_sum_kernel(u64* out, u64 n, u64 level, u64 i0, u64 count, const __grid_constant__ RelinSumPairs pairs,
+                            u64 num_pairs, const __grid_constant__ KsModuli mods, int accumulate) {
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= n * count) return;
+  const u64 e = g / n, l = g - e * n;
+  const KsModulus& md = mods.m[e];
+  const u64 comp = level * n, s = (i0 + e) * n + l;
+  u64 lo0 = 0, hi0 = 0, lo1 = 0, hi1 = 0, lo2 = 0, hi2 = 0;
+  for (unsigned r = 0; r < (unsigned)num_pairs; ++r) {  // at most kRelinSumPairs pairs per launch
+    const u64 a0 = pairs.ct1[r][s], a1 = pairs.ct1[r][s + comp];
+    const u64 b0 = pairs.ct2[r][s], b1 = pairs.ct2[r][s + comp];
+    mac128(a0, b0, lo0, hi0);
+    mac128(a0, b1, lo1, hi1);
+    mac128(a1, b0, lo1, hi1);
+    mac128(a1, b1, lo2, hi2);
+  }
+  u64 v0 = reduce128(hi0, lo0, md), v1 = reduce128(hi1, lo1, md), v2 = reduce128(hi2, lo2, md);
+  u64* o = out + s;
+  if (accumulate) {
+    v0 = csub(v0 + o[0], md.q);
+    v1 = csub(v1 + o[comp], md.q);
+    v2 = csub(v2 + o[2 * comp], md.q);
+  }
+  o[0] = v0;
+  o[comp] = v1;
+  o[2 * comp] = v2;
 }
 
 // The two halves of the mod-down by the last modulus, shared by the kernels below.
@@ -511,6 +549,14 @@ cudaError_t launch_ks_relin_mac(u64* prod, const u64* ops, u64 ops_stride, const
                                 bool accumulate, cudaStream_t stream) {
   ks_relin_mac_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(prod, ops, ops_stride, keys, n, jcount,
                                                                      key_modulus_size, count, mods, tensor, accumulate);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_relin_tensor_sum(u64* out, u64 n, u64 level, u64 i0, u64 count, const RelinSumPairs& pairs,
+                                    u64 num_pairs, const KsModuli& mods, bool accumulate, cudaStream_t stream) {
+  relin_tensor_sum_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(out, n, level, i0, count, pairs, num_pairs,
+                                                                         mods, accumulate);
   count_launch();
   return cudaGetLastError();
 }

@@ -820,6 +820,21 @@ inline void MultiplyRelinearizeHybrid(uint64_t* result, const uint64_t* ct1, con
                                                            moduli, relin_keys.Handle(), rescale ? 1 : 0, batch,
                                                            stream));
 }
+
+// extension: sum_r ct1_r x ct2_r relinearized once with hybrid keys that switch s^2 to s, for each of `batch` outputs.
+// ct1 and ct2 hold batch x num_pairs pointers (entry c * num_pairs + r: pair r of output c, 2 x level_size limbs);
+// output c is stored at result + c * 2 * (level_size - rescale) * n (hexl_b200_multiply_relinearize_sum_hybrid has the
+// formula).  num_pairs = 1 equals MultiplyRelinearizeHybrid bit for bit; rescale = 0 equals DyadicMultiply of every
+// pair, the sums, then KeySwitchHybrid bit for bit.  Inputs may repeat; ct1[x] == ct2[x] squares.
+inline void MultiplyRelinearizeSumHybrid(uint64_t* result, const uint64_t* const* ct1, const uint64_t* const* ct2,
+                                         uint64_t num_pairs, uint64_t n, uint64_t level_size, uint64_t q_size,
+                                         uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                         const KeySwitchKeys& relin_keys, bool rescale, uint64_t batch = 1,
+                                         void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_multiply_relinearize_sum_hybrid(result, ct1, ct2, num_pairs, n, level_size, q_size,
+                                                               p_size, digit_size, moduli, relin_keys.Handle(),
+                                                               rescale ? 1 : 0, batch, stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

@@ -575,6 +575,46 @@ int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1,
                                           const uint64_t* moduli, const hexl_b200_keys* relin_keys, int rescale,
                                           uint64_t batch, void* stream);
 
+/* A sum of ciphertext products relinearized once with hybrid keys (extension; lazy relinearization: Lattigo's MulThenAdd
+ * followed by one Relinearize, OpenFHE's EvalMultNoRelin + EvalAdd + Relinearize), optionally rescaled in the same
+ * mod-down, for each of `batch` outputs: the inner products, the k-sums of matrix products and the sums of products of
+ * polynomial evaluation.  Relinearization is linear in the tensor's last term, so one key switch serves the whole sum.
+ * ct1 and ct2 are host arrays of batch x num_pairs pointers: entry c * num_pairs + r is pair r of output c and points at
+ * one ciphertext (two components of l = level_size limbs, NTT form, canonical, in the memory kind of result).  Output c
+ * is STORED at result + c * 2 * l' * n, l' = l - rescale.  The moduli, digits, key handle (one relinearization key,
+ * s^2 -> s) and shape rules are those of hexl_b200_multiply_relinearize_hybrid.  With (a0_r, a1_r) = ct1[c * num_pairs
+ * + r] and (b0_r, b1_r) = ct2[c * num_pairs + r], per data limb i < l:
+ *   d0 = sum_r a0_r (.) b0_r,  d1 = sum_r (a0_r (.) b1_r + a1_r (.) b0_r),  t = sum_r a1_r (.) b1_r      mod q_i, canonical
+ * and from there the steps of hexl_b200_multiply_relinearize_hybrid from "prod = the mod-up of t times the keys" on,
+ * unchanged: ext = prod + [P] d on the data limbs, then the mod-down by P or by q_{l-1} P.  Hence, bit for bit:
+ * num_pairs = 1 is hexl_b200_multiply_relinearize_hybrid in both rescale modes; rescale = 0 is hexl_b200_dyadic_multiply
+ * of every pair, the three components summed with hexl_b200_eltwise_add_mod_multi, then hexl_b200_key_switch_hybrid of
+ * the summed d2 into the summed (d0, d1).  It is NOT the sum of the num_pairs products of
+ * hexl_b200_multiply_relinearize_hybrid bit for bit: that sum rounds num_pairs times and carries num_pairs key-switch
+ * errors.  It decrypts to sum_r phase(ct1_r) phase(ct2_r), divided by q_{l-1} and rounded with rescale = 1, within the
+ * bound of ONE relinearization.  Inputs are only read: they may repeat and overlap freely (a ciphertext may appear in
+ * several pairs and outputs, and ct1[x] == ct2[x] squares it); result must not overlap any of them.
+ * HEXL_B200_ERR_INVALID_ARG on every refusal of hexl_b200_multiply_relinearize_hybrid (shape, handle, rescale other than
+ * 0 or 1, rescale = 1 with level_size < 2 or p_size > 63), a null array when batch x num_pairs > 0, a null entry in
+ * either array, and result overlapping an input; HEXL_B200_ERR_MIXED_POINTERS when result and the entries are not all
+ * of one memory kind (and device).  num_pairs = 0 or batch = 0 does nothing.  Every distinct input is checked below its
+ * modulus under hexl_b200_set_debug(1).  On the device, per output: num_pairs = 1 runs the launches of
+ * hexl_b200_multiply_relinearize_hybrid.  Otherwise one tensor-sum launch per block of 64 data limbs and chunk of 32
+ * pairs (d1's 128-bit sum takes two products per pair: 64 x (2^61 - 1)^2 < 2^128, so the sums are exact for every
+ * modulus below 2^61 and every num_pairs) stores (d0, d1, t), then the launches of hexl_b200_multiply_relinearize_hybrid,
+ * whose mod-up reads t (its first inverse transform launches as with the multiply on load) and whose storing
+ * multiply-accumulate reads d0 and d1: ceil(l / 64) x ceil(num_pairs / 32) launches more than one product.  Library
+ * scratch: 3 x l x n words plus that of hexl_b200_multiply_relinearize_hybrid.  Device calls capture into a CUDA graph
+ * once the transforms are warm.  Host buffers: every distinct input goes to each device of the
+ * hexl_b200_set_host_devices split once per call, before its first output; the outputs are split by output over the
+ * devices where the handle holds a copy and each comes back from its staging slot.  Managed buffers take the device
+ * path.  Not covered: keys sharded by modulus (refused), plaintext-weighted sums, and an in-place variant. */
+int hexl_b200_multiply_relinearize_sum_hybrid(uint64_t* result, const uint64_t* const* ct1, const uint64_t* const* ct2,
+                                              uint64_t num_pairs, uint64_t n, uint64_t level_size, uint64_t q_size,
+                                              uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                                              const hexl_b200_keys* relin_keys, int rescale, uint64_t batch,
+                                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif
