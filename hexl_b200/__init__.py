@@ -139,6 +139,8 @@ _sig("hexl_b200_multiply_relinearize_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
 _sig("hexl_b200_multiply_relinearize_sum_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
+_sig("hexl_b200_inner_sum_hybrid", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _u64, _vp, _vp, _u64, _int, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -780,4 +782,25 @@ def MultiplyRelinearizeSumHybrid(result, ct1, ct2, n, level_size, q_size, p_size
                                                           digit_size, mods.ctypes.data,
                                                           relin_keys._h if relin_keys is not None else None,
                                                           int(bool(rescale)), batch, _stream(stream, any_cuda)))
+    return result
+
+
+def InnerSumHybrid(result, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, galois_elt, sum_count,
+                   galois_keys, key_elts, rescale=False, batch=1, stream=None):
+    """sum_{j < sum_count} sigma_{g^j}(ct) with hybrid keys, g = galois_elt (hexl_b200_inner_sum_hybrid): ciphertext c
+    of `ciphertexts` (2*level_size*n words each) is stored at result[c * 2*l'*n:], l' = level_size - rescale.
+    (key_elts[r], galois_keys[r]) is a table of available keys; the call looks up the powers of g it needs there.  The
+    log-step rotate-and-sum stays in the extended basis and is rounded once; rescale=True divides by the last limb in
+    that mod-down."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    ke = np.ascontiguousarray(key_elts, dtype=np.uint64)
+    rp, rn, rc = _buf(result); cp, cn, cc = _buf(ciphertexts)
+    _need("moduli", mods.size, q_size + p_size)
+    _need("galois_keys", len(galois_keys), ke.size)
+    _need("result", rn, batch * 2 * (level_size - int(bool(rescale))) * n)
+    _need("ciphertexts", cn, batch * 2 * level_size * n)
+    keys = (_vp * max(1, ke.size))(*[k._h if k is not None else None for k in list(galois_keys)[:ke.size]])
+    _check(_lib.hexl_b200_inner_sum_hybrid(rp, cp, n, level_size, q_size, p_size, digit_size, mods.ctypes.data,
+                                           galois_elt, sum_count, keys, ke.ctypes.data, ke.size,
+                                           int(bool(rescale)), batch, _stream(stream, rc or cc)))
     return result

@@ -1,8 +1,9 @@
 // Hybrid key switching (OpenFHE's KeySwitchHYBRID): digits of up to 64 data moduli and up to 64 special primes, the
 // mod-up and the mod-down by fast base conversion (rns.cu); the base conversion on its own; and the rotations with
 // hybrid keys: hoisted, the diagonal-weighted sum of rotations under one mod-down (the linear transform) and its
-// double-hoisted baby-step giant-step form; and the ciphertext product, or a sum of such products, relinearized with
-// hybrid keys, its rescale optionally merged into the mod-down.
+// double-hoisted baby-step giant-step form; the ciphertext product, or a sum of such products, relinearized with
+// hybrid keys, its rescale optionally merged into the mod-down; and the inner sum of k rotations, a rotate-and-sum kept
+// in the extended basis.
 #include <cstdio>
 #include <numeric>
 
@@ -469,6 +470,141 @@ static int multiply_relinearize_sum_hybrid_on_device(int dev, uint64_t* result, 
   }
   return multiply_relinearize_hybrid_on_device(dev, result, nullptr, nullptr, n, level, q_size, p_size, alpha, rescale,
                                                h, bmods, keys, s, sum);
+}
+
+// The inner sum's recurrence, per bit i of k from 0 to floor(log2 k): the doubling element g^(2^i) when 2^(i+1) <= k
+// (0: no doubling) and the shift element g^s when bit i is set (0: R is not updated), s the sum of the set bits below
+// i.  Elements are reduced mod 2n; 1 is an identity.
+struct InnerSumBit {
+  uint64_t dbl, shift;
+};
+static std::vector<InnerSumBit> inner_sum_bits(uint64_t g, uint64_t k, uint64_t n) {
+  std::vector<InnerSumBit> bits;
+  const uint64_t two_n = 2 * n;
+  uint64_t power = g % two_n, shift = 1;  // g^(2^i), g^s
+  for (uint64_t i = 0; (k >> i) != 0; ++i) {
+    InnerSumBit bit{0, 0};
+    if ((k >> i) & 1) {
+      bit.shift = shift;
+      shift = shift * power % two_n;
+    }
+    if ((k >> (i + 1)) != 0) bit.dbl = power;
+    power = power * power % two_n;
+    bits.push_back(bit);
+  }
+  return bits;
+}
+
+// The inner sum of one ciphertext ct (two components of level limbs, NTT form, device memory) into result
+// (2 x (level - rescale) x n words): per bit of k, with dbl_keys[i] / shift_keys[i] the keys of the bit's doubling and
+// shift elements (nullptr for an identity or an absent rotation):
+//   1. the step launches (per block of 64 moduli of B, only the data moduli while no Y is read or written): A' and R
+//      from A's component 0 at l, pi_d(l) and pi_s(l);
+//   2. with a keyed element: c1' = X_A1 + ModDown_P(Y_A1) (one component, into X_A1, which is not read again; none
+//      while Y_A is empty), then one mod-up of c1' whose multiply-accumulates read pi_d and pi_s and add into Y_A' and
+//      Y_R, laid out one stride apart;
+//   3. after the last bit, the mod-down of Y_R adding into result, which holds X_R (none while Y_R is empty), or with
+//      the rescale, [P] X_R folded into Y_R by the last step launch and the mod-down by q_{level-1} P that stores.
+// A ping-pongs between two scratch pairs; at bit 0 it is ct itself, whose Y is empty.
+static int inner_sum_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct, uint64_t n, uint64_t level,
+                                      uint64_t q_size, uint64_t p_size, uint64_t alpha, bool rescale,
+                                      const CachedNtts& h, const uint64_t* bmods, const std::vector<InnerSumBit>& bits,
+                                      const uint64_t* const* const* dbl_keys, const uint64_t* const* const* shift_keys,
+                                      cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, comp = level * n;
+  const uint64_t stride = nb * 2 * n;  // one Y
+  Scratch ws(s);
+  uint64_t *xs = nullptr, *ys = nullptr, *xr = result, *y1 = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&xs, 2 * 2 * comp)) return rc;  // X of the two A buffers, [2][k][i][n]
+  if (int rc = ws.get(&ys, 3 * stride)) return rc;    // Y of the two A buffers, then Y_R, [3][b][k][n]
+  if (rescale)
+    if (int rc = ws.get(&xr, 2 * comp)) return rc;  // [k][i][n]
+  if (int rc = ws.get(&y1, nb * n)) return rc;      // [b][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * 2 * n)) return rc;  // [i][k][n], one block
+  uint64_t* const yr = ys + 2 * stride;
+  const uint64_t* xa = ct;
+  uint64_t *xa_own = nullptr, *ya = nullptr;  // A in scratch (nullptr while A is ct)
+  bool y_a = false, y_r = false, r_set = false;
+  int next = 0;
+  for (size_t i = 0; i < bits.size(); ++i) {
+    const InnerSumBit& bit = bits[i];
+    const bool dbl = bit.dbl != 0, upd = bit.shift != 0, fold = rescale && i + 1 == bits.size();
+    const bool d_keyed = dbl && bit.dbl != 1, s_keyed = upd && bit.shift != 1;
+    uint64_t *xn = xs + next * 2 * comp, *yn = ys + next * stride;
+    int mode = y_a ? kSumYA : 0;
+    if (dbl) {
+      mode |= kSumNext;
+      if (y_a || d_keyed) mode |= kSumNextY;
+      if (bit.dbl == 1) mode |= kSumDoubleId;
+    }
+    if (upd) {
+      mode |= kSumR;
+      if (!r_set) mode |= kSumRStore;
+      if (y_r) mode |= kSumRY;
+      if (y_a || s_keyed || fold) mode |= kSumRYWrite;
+      if (bit.shift == 1) mode |= kSumShiftId;
+      if (fold) mode |= kSumFold;
+    }
+    if (y_a && (d_keyed || s_keyed)) mode |= kSumCopy1;
+    // 1. the step; Y only where it is read or written
+    const uint64_t span = (mode & (kSumNextY | kSumRYWrite | kSumCopy1)) ? nb : level;
+    for (uint64_t b0 = 0; b0 < span; b0 += kParamBlock) {
+      const uint64_t cnt = std::min<uint64_t>(kParamBlock, span - b0);
+      KsModuli mods = ks_mac_moduli(bmods + b0, nullptr, cnt);
+      if (fold)
+        for (uint64_t e = 0; e < cnt && b0 + e < level; ++e) {
+          const uint64_t q = bmods[b0 + e];
+          uint64_t P = 1 % q;
+          for (uint64_t j = 0; j < p_size; ++j) P = mul_mod128(P, bmods[level + j] % q, q);
+          mods.m[e].c = P;
+        }
+      const cudaError_t e = launch_inner_sum_step(xa, ya, xn, yn, xr, yr, y1, n, level, b0, cnt, dbl ? bit.dbl : 1,
+                                                  upd ? bit.shift : 1, mods, mode, s);
+      if (e != cudaSuccess) return cuda_fail(e, "InnerSumHybrid: step launch");
+    }
+    // 2. the bit's keyed rotations, hoisted: one c1', one mod-up, the products of both elements
+    if (d_keyed || s_keyed) {
+      const uint64_t* c1 = xa + comp;
+      if (y_a) {
+        if (int rc = hybrid_mod_down(dev, xa_own + comp, y1, tmp, n, level, p_size, 1, h, bmods, true, s)) return rc;
+        c1 = xa_own + comp;
+      }
+      const uint64_t* const* keys[2];
+      uint64_t elts[2], count = 0;
+      if (d_keyed) {
+        keys[count] = dbl_keys[i];
+        elts[count++] = bit.dbl;
+      }
+      if (s_keyed) {
+        keys[count] = shift_keys[i];
+        elts[count++] = bit.shift;
+      }
+      uint64_t* prod = d_keyed ? yn : yr;  // Y_A' below Y_R: the second element's products land one stride further
+      const uint64_t pstride = (uint64_t)(yr - yn);
+      Scratch wu(s);
+      if (int rc = hybrid_mod_up(dev, c1, n, level, q_size, p_size, alpha, h, bmods, wu,
+                                 [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) {
+                                   return ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, 2,
+                                                          prod + b0 * 2 * n, pstride, keys, elts, count, s, true);
+                                 },
+                                 s))
+        return rc;
+    }
+    if (dbl) {
+      xa = xa_own = xn;
+      ya = yn;
+      y_a = (mode & kSumNextY) != 0;
+      next ^= 1;
+    }
+    if (upd) {
+      r_set = true;
+      y_r = y_r || (mode & kSumRYWrite);
+    }
+  }
+  // 3. the final mod-down
+  if (rescale) return hybrid_mod_down(dev, result, yr, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);
+  if (!y_r) return 0;
+  return hybrid_mod_down(dev, result, yr, tmp, n, level, p_size, 2, h, bmods, true, s);
 }
 
 // The shape rules of hexl_b200_key_switch_hybrid, without the key handle
@@ -1014,6 +1150,84 @@ int hexl_b200_multiply_relinearize_sum_hybrid(uint64_t* result, const uint64_t* 
       if (int rc = multiply_relinearize_sum_hybrid_on_device(pi.device, result + c * out_words, ct1 + c * k,
                                                              ct2 + c * k, k, n, level, q_size, p_size, alpha, rs, h,
                                                              bmods.data(), dk[0], (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+int hexl_b200_inner_sum_hybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                               uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                               uint64_t galois_elt, uint64_t sum_count, const hexl_b200_keys* const* galois_keys,
+                               const uint64_t* key_elts, uint64_t num_keys, int rescale, uint64_t batch,
+                               void* stream) {
+  const uint64_t level = level_size, alpha = digit_size, g = galois_elt;
+  REQUIRE(result && ciphertexts && moduli, "Require non-null arguments");
+  REQUIRE(num_keys == 0 || (galois_keys && key_elts), "Require galois_keys, key_elts != nullptr");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  REQUIRE(g % 2 == 1 && g < 2 * n, "Require galois_elt odd and in [1, 2n)");
+  REQUIRE(rescale == 0 || rescale == 1, "Require rescale = 0 or 1");
+  REQUIRE(!rescale || level >= 2, "rescale = 1 requires level_size >= 2");
+  REQUIRE(!rescale || p_size < (uint64_t)kParamBlock, "rescale = 1 requires p_size <= %d", kParamBlock - 1);
+  // the keys of every element the recurrence rotates by, looked up in the table: used[] the distinct handles, and per
+  // bit the index of its doubling's and its shift's handle among them (-1: identity or none)
+  const std::vector<InnerSumBit> bits = inner_sum_bits(g, sum_count, n);
+  std::vector<const hexl_b200_keys*> used;
+  std::vector<int64_t> dbl_slot(bits.size(), -1), shift_slot(bits.size(), -1);
+  auto lookup = [&](uint64_t elt, int64_t* slot) -> int {
+    if (elt <= 1) return 0;
+    uint64_t r = 0;
+    while (r < num_keys && key_elts[r] != elt) ++r;
+    REQUIRE(r < num_keys, "no key for the Galois element %llu, which the sum of %llu rotations by %llu needs",
+            (unsigned long long)elt, (unsigned long long)sum_count, (unsigned long long)g);
+    REQUIRE(galois_keys[r], "Require galois_keys[%llu] != nullptr (the key of element %llu)", (unsigned long long)r,
+            (unsigned long long)elt);
+    char what[40];
+    std::snprintf(what, sizeof what, "galois_keys[%llu]", (unsigned long long)r);
+    if (int rc = hybrid_handle_check(galois_keys[r], n, q_size, p_size, alpha, 2, what)) return rc;
+    const auto it = std::find(used.begin(), used.end(), galois_keys[r]);
+    *slot = it - used.begin();
+    if (it == used.end()) used.push_back(galois_keys[r]);
+    return 0;
+  };
+  for (size_t i = 0; i < bits.size(); ++i) {
+    if (int rc = lookup(bits[i].dbl, &dbl_slot[i])) return rc;
+    if (int rc = lookup(bits[i].shift, &shift_slot[i])) return rc;
+  }
+  if (sum_count == 0 || batch == 0) return 0;
+  const uint64_t in_words = 2 * level * n, out_words = 2 * (level - rescale) * n;
+  REQUIRE(result + batch * out_words <= ciphertexts || ciphertexts + batch * in_words <= result,
+          "result and ciphertexts must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, ciphertexts}, &pi)) return rc;
+  if (int rc = check_limb_bounds(ciphertexts, 2 * batch, level, n, [&](u64 i) { return moduli[i]; }, pi,
+                                 "ciphertexts", stream))
+    return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(level + p_size);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  const bool rs = rescale != 0;
+  // one ciphertext on one device: dk[u] is used[u]'s copy there
+  auto run = [&](int dev, uint64_t* res, const uint64_t* ct, const uint64_t* const* const* dk, cudaStream_t s) {
+    std::vector<const uint64_t* const*> dbl_keys(bits.size(), nullptr), shift_keys(bits.size(), nullptr);
+    for (size_t i = 0; i < bits.size(); ++i) {
+      if (dbl_slot[i] >= 0) dbl_keys[i] = dk[dbl_slot[i]];
+      if (shift_slot[i] >= 0) shift_keys[i] = dk[shift_slot[i]];
+    }
+    return inner_sum_hybrid_on_device(dev, res, ct, n, level, q_size, p_size, alpha, rs, h, bmods.data(), bits,
+                                      dbl_keys.data(), shift_keys.data(), s);
+  };
+  // host pointers: each ciphertext crosses PCIe in once and its sum comes back from the same slot
+  if (pi.where == Where::Host)
+    return key_switch_host_batch(result, out_words, false, ciphertexts, in_words, in_words, used.data(), used.size(),
+                                 batch,
+                                 [&](int dev, uint64_t* d_res, uint64_t* d_ct, const uint64_t* const* const* dk,
+                                     cudaStream_t s) { return run(dev, d_res, d_ct, dk, s); });
+  std::vector<const uint64_t* const*> dk;
+  if (keys_on_device(used.data(), used.size(), pi.device, &dk) < used.size())
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "a key handle holds no copy on the device of the ciphertexts");
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = run(pi.device, result + c * out_words, ciphertexts + c * in_words, dk.data(), (cudaStream_t)stream))
         return rc;
     return 0;
   });

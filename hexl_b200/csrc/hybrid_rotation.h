@@ -1,7 +1,8 @@
 // Launchers of the two kernels of the hybrid linear transform (seal.cu): the weighted multi-element
 // multiply-accumulate and the weighted permuted sum of the ciphertext's limbs; of the giant-step sums of the
 // baby-step giant-step transform; of the multiply-accumulate of the multiply-relinearize call, which adds the
-// tensor terms; and of the tensor sums of a sum of products.  All take two-component ciphertexts (key component count 2)
+// tensor terms; of the tensor sums of a sum of products; and of the per-bit step of the inner sum (a rotate-and-sum
+// kept in the extended basis).  All take two-component ciphertexts (key component count 2)
 // in NTT form, every word canonical, every modulus below 2^61.
 #pragma once
 #include "internal.h"
@@ -101,5 +102,28 @@ struct RelinSumPairs {
 // canonical; out is [3][level][n]; accumulate adds into out (later chunks of pairs), else stores.
 cudaError_t launch_relin_tensor_sum(u64* out, u64 n, u64 level, u64 i0, u64 count, const RelinSumPairs& pairs,
                                     u64 num_pairs, const KsModuli& mods, bool accumulate, cudaStream_t stream);
+
+// One bit of the inner sum's rotate-and-sum recurrence.  The pairs A (the current partial sum, read), A' (A + Rot_d(A),
+// written) and R (the result so far, R += Rot_s(A)) each hold X, two components on the data limbs ([k][i][n], level
+// limbs), and Y, two components over B ([b][k][n]).  mode bits:
+//   kSumYA         A has Y (else Y_A reads as zero)
+//   kSumNext       write A'; kSumNextY: A' has Y (writes it over B); kSumDoubleId: d = 1, so component 1 doubles
+//   kSumR          update R; kSumRStore: X_R is stored (the first set bit); kSumRY: R had Y before (else Y_R is stored);
+//                  kSumRYWrite: write Y_R over B; kSumShiftId: s = 1, so component 1 of A adds into R too
+//   kSumCopy1      store Y_A's component 1 into y1 ([b][n]), the input of the one-component mod-down of c1'
+//   kSumFold       R's last update under the merged rescale: Y_R's data limbs take [P]_{q_i} X_R (mods.m[e].c),
+//                  X_R is not stored
+enum : int {
+  kSumYA = 1, kSumNext = 2, kSumNextY = 4, kSumDoubleId = 8, kSumR = 16, kSumRStore = 32, kSumRY = 64,
+  kSumRYWrite = 128, kSumShiftId = 256, kSumCopy1 = 512, kSumFold = 1024
+};
+// Over the moduli [b0, b0 + count) of B (l = level; mods.m[e] describes modulus b0 + e with a, b = 2^64 mod q and its
+// Shoup factor), every slot l, with d and s the doubling and shift elements (1 when absent):
+//   A'0[l] = A0[l] + A0[pi_d(l)],  A'1[l] = A1[l] (2 A1[l] under kSumDoubleId)
+//   R0[l] (+)= A0[pi_s(l)],        R1[l] (+)= A1[l] under kSumShiftId
+// on X for the data moduli and on Y where Y is written; everything canonical.  xa, ya (A) are only read.
+cudaError_t launch_inner_sum_step(const u64* xa, const u64* ya, u64* xn, u64* yn, u64* xr, u64* yr, u64* y1, u64 n,
+                                  u64 level, u64 b0, u64 count, u64 dbl, u64 shift, const KsModuli& mods, int mode,
+                                  cudaStream_t stream);
 
 }  // namespace hexl_b200

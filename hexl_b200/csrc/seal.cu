@@ -395,6 +395,79 @@ __global__ void __launch_bounds__(kThreads)
   o[2 * comp] = v2;
 }
 
+// ---- The inner sum: one bit of the rotate-and-sum recurrence, A' = A + Rot_d(A) and R += Rot_s(A).
+// A thread owns one slot l of one modulus b = b0 + e of B and handles X (data moduli) and Y there.  It reads A's
+// component 0 at l, pi_d(l) and pi_s(l) and component 1 at l, once each; component 1 moves to A' unchanged, or doubled
+// when d = 1.  Only additions of canonical words, except the fold's [P] X_R, one 128-bit product reduced once.
+struct SumPart {
+  u64 a0, ad, as, a1;  // A0 at l, pi_d(l), pi_s(l); A1 at l
+};
+__device__ __forceinline__ SumPart sum_read(const u64* a0, const u64* a1, u64 l, u64 pd, u64 ps) {
+  return SumPart{a0[l], a0[pd], a0[ps], a1[l]};
+}
+__global__ void __launch_bounds__(kThreads)
+    inner_sum_step_kernel(const u64* xa, const u64* ya, u64* xn, u64* yn, u64* xr, u64* yr, u64* y1, u64 n, u64 level,
+                          u64 b0, u64 count, unsigned dbl, unsigned shift, const __grid_constant__ KsModuli mods,
+                          int mode) {
+  const u64 g = (u64)blockIdx.x * kThreads + threadIdx.x;
+  if (g >= n * count) return;
+  const u64 e = g / n, l = g - e * n, b = b0 + e;
+  const KsModulus& md = mods.m[e];
+  const u64 q = md.q;
+  const int log_n = __ffsll((long long)n) - 1;
+  const unsigned mask = (unsigned)(2 * n - 1);
+  const u64 pd = ntt_source((unsigned)l, dbl, mask, log_n), ps = ntt_source((unsigned)l, shift, mask, log_n);
+  const bool twice = mode & kSumDoubleId, shift_id = mode & kSumShiftId;
+  u64 xr0 = 0, xr1 = 0;  // X_R after this bit, for the fold
+  if (b < level) {
+    const u64 comp = level * n;
+    const SumPart x = sum_read(xa + b * n, xa + comp + b * n, l, pd, ps);
+    if (mode & kSumNext) {
+      xn[b * n + l] = csub(x.a0 + x.ad, q);
+      xn[comp + b * n + l] = twice ? csub(x.a1 + x.a1, q) : x.a1;
+    }
+    if (mode & kSumR) {
+      u64* r = xr + b * n + l;
+      xr0 = x.as;
+      xr1 = shift_id ? x.a1 : 0;
+      if (!(mode & kSumRStore)) {
+        xr0 = csub(xr0 + r[0], q);
+        xr1 = csub(xr1 + r[comp], q);
+      }
+      if (!(mode & kSumFold)) {
+        r[0] = xr0;
+        r[comp] = xr1;
+      }
+    }
+  }
+  const bool y_next = (mode & kSumNext) && (mode & kSumNextY), y_r = (mode & kSumR) && (mode & kSumRYWrite);
+  if (!y_next && !y_r && !(mode & kSumCopy1)) return;
+  const SumPart y = (mode & kSumYA) ? sum_read(ya + b * 2 * n, ya + b * 2 * n + n, l, pd, ps) : SumPart{0, 0, 0, 0};
+  if (y_next) {
+    yn[b * 2 * n + l] = csub(y.a0 + y.ad, q);
+    yn[b * 2 * n + n + l] = twice ? csub(y.a1 + y.a1, q) : y.a1;
+  }
+  if (y_r) {
+    u64* r = yr + b * 2 * n + l;
+    u64 v0 = y.as, v1 = shift_id ? y.a1 : 0;
+    if (mode & kSumRY) {
+      v0 = csub(v0 + r[0], q);
+      v1 = csub(v1 + r[n], q);
+    }
+    if ((mode & kSumFold) && b < level) {  // y_{q_i} += [P]_{q_i} X_R, md.c = [P]_{q_i}
+      u64 lo = 0, hi = 0;
+      mac128(md.c, xr0, lo, hi);
+      v0 = csub(v0 + reduce128(hi, lo, md), q);
+      lo = hi = 0;
+      mac128(md.c, xr1, lo, hi);
+      v1 = csub(v1 + reduce128(hi, lo, md), q);
+    }
+    r[0] = v0;
+    r[n] = v1;
+  }
+  if (mode & kSumCopy1) y1[b * n + l] = y.a1;
+}
+
 // The two halves of the mod-down by the last modulus, shared by the kernels below.
 // round: a coefficient of the last modulus's part (coefficient form, [0, 2 q_last)) rounded and moved into modulus q:
 //   t = (x + q_last/2) mod q_last;  out = (t mod q) + add,  add = q - (q_last/2 mod q);  out < 2q
@@ -557,6 +630,15 @@ cudaError_t launch_relin_tensor_sum(u64* out, u64 n, u64 level, u64 i0, u64 coun
                                     u64 num_pairs, const KsModuli& mods, bool accumulate, cudaStream_t stream) {
   relin_tensor_sum_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(out, n, level, i0, count, pairs, num_pairs,
                                                                          mods, accumulate);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_inner_sum_step(const u64* xa, const u64* ya, u64* xn, u64* yn, u64* xr, u64* yr, u64* y1, u64 n,
+                                  u64 level, u64 b0, u64 count, u64 dbl, u64 shift, const KsModuli& mods, int mode,
+                                  cudaStream_t stream) {
+  inner_sum_step_kernel<<<blocks_for(n * count), kThreads, 0, stream>>>(xa, ya, xn, yn, xr, yr, y1, n, level, b0, count,
+                                                                       (unsigned)dbl, (unsigned)shift, mods, mode);
   count_launch();
   return cudaGetLastError();
 }

@@ -835,6 +835,23 @@ inline void MultiplyRelinearizeSumHybrid(uint64_t* result, const uint64_t* const
                                                                p_size, digit_size, moduli, relin_keys.Handle(),
                                                                rescale ? 1 : 0, batch, stream));
 }
+
+// extension: sum_{j < sum_count} sigma_{g^j}(ct) with hybrid keys, g = galois_elt, for each of `batch` ciphertexts
+// (2 x level_size limbs each), stored at result + c * 2 * (level_size - rescale) * n: the log-step rotate-and-sum kept in
+// the extended basis and rounded once (hexl_b200_inner_sum_hybrid has the recurrence).  (key_elts[r], galois_keys[r]) is
+// a table of available keys; the call looks up the powers of g it needs there, and a missing one throws.  sum_count = 2
+// equals ApplyGaloisKeySwitchHybridHoisted by g plus EltwiseAddModMulti with ct bit for bit.
+inline void InnerSumHybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                           uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                           uint64_t galois_elt, uint64_t sum_count, const KeySwitchKeys* const* galois_keys,
+                           const uint64_t* key_elts, uint64_t num_keys, bool rescale, uint64_t batch = 1,
+                           void* stream = nullptr) {
+  std::vector<const hexl_b200_keys*> keys(num_keys);
+  for (uint64_t r = 0; r < num_keys; ++r) keys[r] = galois_keys[r] ? galois_keys[r]->Handle() : nullptr;
+  b200_detail::Throw(hexl_b200_inner_sum_hybrid(result, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli,
+                                                galois_elt, sum_count, keys.data(), key_elts, num_keys,
+                                                rescale ? 1 : 0, batch, stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

@@ -615,6 +615,62 @@ int hexl_b200_multiply_relinearize_sum_hybrid(uint64_t* result, const uint64_t* 
                                               const hexl_b200_keys* relin_keys, int rescale, uint64_t batch,
                                               void* stream);
 
+/* The inner sum of k = sum_count rotations with hybrid keys (extension; Lattigo's InnerSum, OpenFHE's EvalSum, the last
+ * step of EvalInnerProduct): sum_{j<k} sigma_{g^j}(ct) for g = galois_elt, for each of `batch` ciphertexts, by the
+ * log-step recurrence A <- A + Rot(A) kept in the extended basis B = {q_0..q_{l-1}, p_0..p_{K-1}} and rounded once at
+ * the end, the rescale optionally merged into that mod-down.  The moduli, digits, shape rules, handle rules (non-null,
+ * the right shape, not sharded), layouts, rescale (l' = l - rescale), memory kinds, batch splitting and debug checks are
+ * those of hexl_b200_linear_transform_hybrid_bsgs: ciphertext c (two components of l = level_size limbs, NTT form,
+ * canonical) is read at ciphertexts + c * 2 * l * n and its sum STORED at result + c * 2 * l' * n.
+ * (key_elts[r], galois_keys[r]) for r < num_keys is a table of available keys (galois_keys[r] switches s(X^e) to s for
+ * e = key_elts[r]); the call looks up the elements it needs there (the first match), so one set of keys for the powers
+ * g^(2^i) serves every sum_count.  With pi_e / sigma_e the NTT-form automorphism of hexl_b200_apply_galois, elements
+ * reduced mod 2n, the mod-up D_{d,m} and keys K of hexl_b200_key_switch_hybrid, and a pair (X, Y) as in the BSGS call
+ * (X two components on the data limbs, Y two components over B or empty, val = X + ModDown_P(Y)):
+ *   Rot_1(X, Y)  = (X, Y)                                                       (no key)
+ *   Rot_e(X, Y)  = ((sigma_e X0, 0), (pi_e Y0 + M_e,0, M_e,1)),  c1' = X1 + ModDown_P(Y1) (X1 while Y is empty),
+ *                  M_e,k = sum_d pi_e(D_{d,m}(c1')) (.) K_e[d][k][slot(m)]                         every m in B
+ *   A = (ct, empty);  R = none;  s = 0
+ *   for i = 0 .. floor(log2 k):
+ *     if bit i of k is set:  R = Rot_{g^s}(A) (R none) or R + Rot_{g^s}(A);  s += 2^i
+ *     if 2^(i+1) <= k:       A = A + Rot_{g^(2^i)}(A)
+ *   rescale = 0:  result = X_R + ModDown_P(Y_R)      (X_R while Y_R is empty)
+ *   rescale = 1:  [P] X_R folded into Y_R's data limbs and the mod-down by q_{l-1} P, as in the BSGS call
+ * Pairs add component-wise, an empty Y as zero.  Both rotations of one bit read the same A, so they share one c1' and
+ * one mod-up (hoisted).  The needed elements are g^(2^i) for 2^(i+1) <= k and g^s at every set bit but the lowest; one
+ * equal to 1 (mod 2n) is an identity and needs no key (the conjugation 2n - 1 squared is 1).  It decrypts to
+ * sum_{j<k} sigma_{g^j}(phase(ct)), divided by q_{l-1} and rounded with rescale = 1, within one key switch and one
+ * rounding of c1' times s per keyed rotation, carried through the sum.  Canonical modular sums do not depend on their
+ * order, so bit for bit: k = 1 is hexl_b200_linear_transform_hybrid_bsgs with one identity baby, one identity giant and
+ * a unit diagonal (a copy of ct with rescale = 0); k = 2 is hexl_b200_apply_galois_key_switch_hybrid_hoisted by g plus
+ * hexl_b200_eltwise_add_mod_multi with ct, and hexl_b200_linear_transform_hybrid over {1, g} with unit diagonals;
+ * k = 3 is the BSGS call with babies {1, g}, giants {1, g}, unit diagonals and the (giant 1, baby g) pair absent, and
+ * k = 4 the BSGS call with babies {1, g}, giants {1, g^2} and four unit diagonals, both in both rescale modes.  For
+ * k >= 5 it is a nested chain of such steps, not one BSGS call.  It is NOT the chain of separately rounded hoisted
+ * rotations and additions bit for bit: that rounds once per rotation.
+ * HEXL_B200_ERR_INVALID_ARG on the shape refusals of hexl_b200_key_switch_hybrid, galois_elt even or outside [1, 2n),
+ * a needed element other than 1 missing from key_elts (the message names it), a null or misshapen handle for a needed
+ * element, rescale other than 0 or 1, rescale = 1 with level_size < 2 or p_size > 63, null galois_keys or key_elts with
+ * num_keys > 0, and result overlapping the ciphertexts.  sum_count = 0 or batch = 0 does nothing.
+ * On the device, per ciphertext and bit i of k: one step launch per block of 64 moduli of B (of the data moduli only
+ * while no Y is read or written), which writes A' = A + pi_d(A0) into the other buffer of a ping-pong pair and adds
+ * pi_s(A0) into R; then, when the bit has a keyed element, the one-component mod-down of Y_A1 (none while Y_A is empty)
+ * and one mod-up of c1' whose multiply-accumulates add the products of the bit's one or two keyed elements into Y_A'
+ * and Y_R; after the last bit, the mod-down of Y_R (none while it is empty), or the merged one with rescale = 1.  So a
+ * ciphertext takes sum_i (ceil(span_i / 64) + [keyed_i] (down_1 [Y_A non-empty] + up(e_i))) + down_2 launches, span_i
+ * = l or l + K, e_i <= 2 its keyed elements, up(e) the launches of the mod-up of hexl_b200_key_switch_hybrid with e
+ * multiply-accumulate sets (ceil(l / alpha) digits) and down_c those of its mod-down of c components (0 while Y_R is
+ * empty without the rescale).  Library scratch: two pairs for A and R (5 x (l + K) x 2 x n words and less), one round of
+ * converted digits and a few l x n buffers.  Device calls capture into a CUDA graph once the transforms are warm.  Host
+ * buffers: each ciphertext crosses PCIe in once and its sum comes back on the same staging stream, split by ciphertext
+ * over the devices of hexl_b200_set_host_devices where every needed handle holds a copy.  Managed buffers take the
+ * device path.  Not covered: keys sharded by modulus (refused), mapping rotation steps to elements, sums over other
+ * than the powers of one element, and an in-place variant. */
+int hexl_b200_inner_sum_hybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                               uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                               uint64_t galois_elt, uint64_t sum_count, const hexl_b200_keys* const* galois_keys,
+                               const uint64_t* key_elts, uint64_t num_keys, int rescale, uint64_t batch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
