@@ -141,6 +141,9 @@ _sig("hexl_b200_multiply_relinearize_sum_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _int, _u64, _vp])
 _sig("hexl_b200_inner_sum_hybrid", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _u64, _vp, _vp, _u64, _int, _u64, _vp])
+_sig("hexl_b200_bfv_multiply", _int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp, _u64, _u64, _u64, _u64, _vp])
+_sig("hexl_b200_bfv_multiply_relinearize_hybrid", _int,
+     [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _u64, _u64, _u64, _vp, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -803,4 +806,41 @@ def InnerSumHybrid(result, ciphertexts, n, level_size, q_size, p_size, digit_siz
     _check(_lib.hexl_b200_inner_sum_hybrid(rp, cp, n, level_size, q_size, p_size, digit_size, mods.ctypes.data,
                                            galois_elt, sum_count, keys, ke.ctypes.data, ke.size,
                                            int(bool(rescale)), batch, _stream(stream, rc or cc)))
+    return result
+
+
+def BfvMultiply(result, ct1, ct2, n, moduli, level_size, base_b, m_sk, plain_modulus, batch=1, stream=None):
+    """BFV ct1 x ct2 by BEHZ (hexl_b200_bfv_multiply): pair c reads ct1[c * 2*level_size*n:] and ct2[c * 2*level_size*n:]
+    (coefficient form) and its tensor scaled by t/Q, (d0, d1, d2), is stored at result[c * 3*level_size*n:].  Q is the
+    first level_size entries of moduli; base_b (B) and m_sk are the BEHZ bases, plain_modulus is t.  ct1 may be ct2."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    bb = np.ascontiguousarray(base_b, dtype=np.uint64)
+    rp, rn, rc = _buf(result); ap, an, ac = _buf(ct1); bp, bn, bc = _buf(ct2)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, level_size)
+    _need("result", rn, batch * 3 * level_size * n)
+    _need("ct1", an, batch * per); _need("ct2", bn, batch * per)
+    _check(_lib.hexl_b200_bfv_multiply(rp, ap, bp, n, mods.ctypes.data, level_size, bb.ctypes.data, bb.size, m_sk,
+                                       plain_modulus, batch, _stream(stream, rc or ac or bc)))
+    return result
+
+
+def BfvMultiplyRelinearizeHybrid(result, ct1, ct2, n, level_size, q_size, p_size, digit_size, moduli, base_b, m_sk,
+                                 plain_modulus, relin_keys: KeySwitchKeys, batch=1, stream=None):
+    """BFV ct1 x ct2 by BEHZ relinearized with hybrid keys (hexl_b200_bfv_multiply_relinearize_hybrid): pair c's
+    (d0, d1) + KS(d2) is stored at result[c * 2*level_size*n:], coefficient form.  moduli holds q_size data moduli then
+    p_size special primes, as for MultiplyRelinearizeHybrid; base_b, m_sk and plain_modulus as for BfvMultiply.  Bit for
+    bit BfvMultiply, the forward transform of d2, KeySwitchHybrid, the inverse transform and the addition of (d0, d1)."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    bb = np.ascontiguousarray(base_b, dtype=np.uint64)
+    rp, rn, rc = _buf(result); ap, an, ac = _buf(ct1); bp, bn, bc = _buf(ct2)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size)
+    _need("result", rn, batch * per)
+    _need("ct1", an, batch * per); _need("ct2", bn, batch * per)
+    _check(_lib.hexl_b200_bfv_multiply_relinearize_hybrid(rp, ap, bp, n, level_size, q_size, p_size, digit_size,
+                                                          mods.ctypes.data, bb.ctypes.data, bb.size, m_sk,
+                                                          plain_modulus,
+                                                          relin_keys._h if relin_keys is not None else None, batch,
+                                                          _stream(stream, rc or ac or bc)))
     return result

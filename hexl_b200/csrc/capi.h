@@ -416,4 +416,27 @@ int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, 
                           const HostSwitch& run, const std::function<int(int)>& prepare = nullptr,
                           const uint64_t* in2 = nullptr);
 
+// BFV multiplication by BEHZ (capi_bfv.cu).  The refusals of hexl_b200_bfv_multiply that do not depend on the
+// buffers' memory: null pointers, shapes, moduli, plain modulus and the bound on Bsk.
+bool behz_bound_holds(uint64_t n, uint64_t t, const uint64_t* q, uint64_t l, const uint64_t* b, uint64_t k,
+                      uint64_t m_sk);
+int bfv_check(const void* result, const void* ct1, const void* ct2, uint64_t n, const uint64_t* moduli, uint64_t l,
+              const uint64_t* base_b, uint64_t k, uint64_t m_sk, uint64_t t);
+// What one call needs: the transforms of Q u Bsk (l + k + 1 moduli, Q first, then b_0..b_{k-1}, m_sk) and the
+// constant tables of the two kernels (internal.h), uploaded to each device on first use
+struct BfvPlan {
+  uint64_t n = 0, l = 0, k = 0;
+  std::vector<uint64_t> mods, ext_tab, scale_tab;
+  CachedNtts h;
+  explicit BfvPlan(size_t count) : h(count) {}
+};
+int bfv_plan(BfvPlan* plan, uint64_t n, const uint64_t* moduli, uint64_t l, const uint64_t* base_b, uint64_t k,
+             uint64_t m_sk, uint64_t t);
+// One pair (ct1, ct2: two components of l limbs, coefficient form, device memory; ct1 == ct2 squares) into d0, d1, d2
+// at out.p[0..2] (l limbs each), asynchronous on s: the extension launches, one forward transform of the lifted
+// inputs, the tensor, one inverse transform and the scaling launch.  Scratch: 7 (or 5 when squaring) x (l + k + 1) x n
+// words.
+int bfv_product_on_device(int dev, const BfvPlan& plan, const BfvOutputs& out, const uint64_t* ct1,
+                          const uint64_t* ct2, cudaStream_t s);
+
 }  // namespace hexl_b200

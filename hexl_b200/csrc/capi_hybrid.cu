@@ -2,8 +2,8 @@
 // mod-up and the mod-down by fast base conversion (rns.cu); the base conversion on its own; and the rotations with
 // hybrid keys: hoisted, the diagonal-weighted sum of rotations under one mod-down (the linear transform) and its
 // double-hoisted baby-step giant-step form; the ciphertext product, or a sum of such products, relinearized with
-// hybrid keys, its rescale optionally merged into the mod-down; and the inner sum of k rotations, a rotate-and-sum kept
-// in the extended basis.
+// hybrid keys, its rescale optionally merged into the mod-down; the inner sum of k rotations, a rotate-and-sum kept
+// in the extended basis; and the BFV product relinearized with hybrid keys in coefficient form.
 #include <cstdio>
 #include <numeric>
 
@@ -77,29 +77,33 @@ static int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t 
 // transformed into ops ([e][d][n], D x n words between moduli), and mac(b0, cnt, ops, slots) multiplies them with the
 // keys: moduli [b0, b0 + cnt) of B, slots[e] the key slot of modulus b0 + e.  Scratch comes from ws.  mul (nullptr:
 // none; laid out like target) makes the target the point-wise product target (.) mul, multiplied in the first inverse
-// transform's load, so the product is never written.
+// transform's load, so the product is never written.  coef: the target is already in coefficient form (canonical);
+// its limbs are read directly and step 1 is skipped.
 template <class Mac>
 static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t level, uint64_t q_size,
                          uint64_t p_size, uint64_t alpha, const CachedNtts& h, const uint64_t* bmods, Scratch& ws,
-                         Mac&& mac, cudaStream_t s, const uint64_t* mul = nullptr) {
+                         Mac&& mac, cudaStream_t s, const uint64_t* mul = nullptr, bool coef = false) {
   const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size;
   // moduli handled per round of the mod-up: bounded by the parameter block and by ~256 MiB of scratch
   const uint64_t per_mod = D * n;
   uint64_t ichunk = std::max<uint64_t>(1, (256ull << 20) / (per_mod * 8));
   ichunk = std::min<uint64_t>({ichunk, nb, (uint64_t)kParamBlock});
   uint64_t *t_coef = nullptr, *ops = nullptr;
-  if (int rc = ws.get(&t_coef, level * n)) return rc;
+  if (!coef)
+    if (int rc = ws.get(&t_coef, level * n)) return rc;
   if (int rc = ws.get(&ops, ichunk * per_mod)) return rc;  // [e][d][n]
   // 1. the target's limbs back to coefficients, canonical
-  if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s, nullptr, false, mul))
-    return rc;
+  if (!coef)
+    if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s, nullptr, false, mul))
+      return rc;
+  const uint64_t* a = coef ? target : t_coef;
   // 2. mod-up: every digit converted into each modulus of the round, lazily transformed, multiplied with the keys.
   //    (A digit's own limbs are converted and transformed again like the others: NTT(INTT(t)) = t.)
   for (uint64_t b0 = 0; b0 < nb; b0 += ichunk) {
     const uint64_t cnt = std::min(ichunk, nb - b0);
     for (uint64_t d = 0; d < D; ++d) {
       const uint64_t lo = d * alpha, width = std::min(alpha, level - lo);
-      if (int rc = base_convert_on_device(ops + d * n, per_mod, 0, t_coef + lo * n, n, 0, n, 1, bmods + lo, width,
+      if (int rc = base_convert_on_device(ops + d * n, per_mod, 0, a + lo * n, n, 0, n, 1, bmods + lo, width,
                                           bmods + b0, cnt, false, s))
         return rc;
     }
@@ -115,10 +119,12 @@ static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t l
 // special limbs back to coefficients in place, rounded and converted into each data modulus, transformed, and
 // (prod - that) * P^-1 accumulated into result (kcc x level x n), or stored when !accumulate.  tmp holds
 // min(level, 64) x kcc x n words.  P is the product of the p_size moduli of B after the first `level`: called with
-// level - 1 and p_size + 1 it divides by q_{level-1} P as well, the mod-down merged with the rescale.
+// level - 1 and p_size + 1 it divides by q_{level-1} P as well, the mod-down merged with the rescale.  coef: result is
+// in coefficient form; the products' data limbs go back to coefficients in place instead of the rounded correction
+// being transformed forward, and the finish, point-wise, is the same: INTT((prod - NTT(c)) P^-1) = (INTT(prod) - c) P^-1.
 static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* tmp, uint64_t n, uint64_t level,
                            uint64_t p_size, uint64_t kcc, const CachedNtts& h, const uint64_t* bmods, bool accumulate,
-                           cudaStream_t s) {
+                           cudaStream_t s, bool coef = false) {
   uint64_t* special = prod + level * kcc * n;  // [j][k][n]
   if (int rc = ntt_multi_on_device(false, dev, h.data() + level, p_size, special, special, 1, kcc, s)) return rc;
   for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
@@ -126,7 +132,12 @@ static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* 
     if (int rc = base_convert_on_device(tmp, kcc * n, n, special, kcc * n, n, n, kcc, bmods + level, p_size,
                                         bmods + i0, cnt, true, s))
       return rc;
-    if (int rc = ntt_multi_on_device(true, dev, h.data() + i0, cnt, tmp, tmp, 4, kcc, s)) return rc;
+    if (coef) {
+      uint64_t* data = prod + i0 * kcc * n;
+      if (int rc = ntt_multi_on_device(false, dev, h.data() + i0, cnt, data, data, 1, kcc, s)) return rc;
+    } else if (int rc = ntt_multi_on_device(true, dev, h.data() + i0, cnt, tmp, tmp, 4, kcc, s)) {
+      return rc;
+    }
     KsModuli fin;
     for (uint64_t e = 0; e < cnt; ++e) {
       const uint64_t q = bmods[i0 + e];
@@ -470,6 +481,33 @@ static int multiply_relinearize_sum_hybrid_on_device(int dev, uint64_t* result, 
   }
   return multiply_relinearize_hybrid_on_device(dev, result, nullptr, nullptr, n, level, q_size, p_size, alpha, rescale,
                                                h, bmods, keys, s, sum);
+}
+
+// The BFV product of one pair (ct1, ct2: two components of level limbs, coefficient form, device memory), relinearized
+// with keys (digit d's key buffer keys[d]) and stored into result (2 x level x n words, coefficient form): the BEHZ chain
+// of hexl_b200_bfv_multiply stores d0 and d1 into result and d2 into scratch; the mod-up reads d2's limbs as they are;
+// per round, the multiply-accumulate stores the products; the mod-down brings the products' data limbs back to
+// coefficients and adds (prod - c) P^-1 into (d0, d1).  Scratch: that of hexl_b200_bfv_multiply, l x n words of d2, one
+// round of converted digits and (level + K) x 2 x n words of products.
+static int bfv_multiply_relinearize_on_device(int dev, uint64_t* result, const uint64_t* ct1, const uint64_t* ct2,
+                                              const BfvPlan& plan, uint64_t n, uint64_t level, uint64_t q_size,
+                                              uint64_t p_size, uint64_t alpha, const CachedNtts& h,
+                                              const uint64_t* bmods, const uint64_t* const* keys, cudaStream_t s) {
+  const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, comp = level * n;
+  Scratch ws(s);
+  uint64_t *d2 = nullptr, *prod = nullptr, *tmp = nullptr;
+  if (int rc = ws.get(&d2, comp)) return rc;
+  if (int rc = ws.get(&prod, nb * 2 * n)) return rc;                                       // [b][k][n]
+  if (int rc = ws.get(&tmp, std::min<uint64_t>(level, kParamBlock) * 2 * n)) return rc;  // [i][k][n], one block
+  if (int rc = bfv_product_on_device(dev, plan, BfvOutputs{{result, result + comp, d2}}, ct1, ct2, s)) return rc;
+  if (int rc = hybrid_mod_up(dev, d2, n, level, q_size, p_size, alpha, h, bmods, ws,
+                             [&](uint64_t b0, uint64_t cnt, const uint64_t* ops, const uint64_t* slots) {
+                               return ks_mac_products(h.data() + b0, slots, cnt, kms, ops, D, n, 2,
+                                                      prod + b0 * 2 * n, nb * 2 * n, &keys, nullptr, 1, s);
+                             },
+                             s, nullptr, true))
+    return rc;
+  return hybrid_mod_down(dev, result, prod, tmp, n, level, p_size, 2, h, bmods, true, s, true);
 }
 
 // The inner sum's recurrence, per bit i of k from 0 to floor(log2 k): the doubling element g^(2^i) when 2^(i+1) <= k
@@ -1228,6 +1266,57 @@ int hexl_b200_inner_sum_hybrid(uint64_t* result, const uint64_t* ciphertexts, ui
   return run_on_device(pi, stream, [&] {
     for (uint64_t c = 0; c < batch; ++c)
       if (int rc = run(pi.device, result + c * out_words, ciphertexts + c * in_words, dk.data(), (cudaStream_t)stream))
+        return rc;
+    return 0;
+  });
+}
+
+int hexl_b200_bfv_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                              uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                              uint64_t digit_size, const uint64_t* moduli, const uint64_t* base_b,
+                                              uint64_t base_b_size, uint64_t m_sk, uint64_t plain_modulus,
+                                              const hexl_b200_keys* relin_keys, uint64_t batch, void* stream) {
+  const uint64_t level = level_size, alpha = digit_size, k = base_b_size;
+  REQUIRE(result && ct1 && ct2 && moduli && base_b && relin_keys, "Require non-null arguments");
+  if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (int rc = hybrid_handle_check(relin_keys, n, q_size, p_size, alpha, 2, "relin_keys")) return rc;
+  if (int rc = bfv_check(result, ct1, ct2, n, moduli, level, base_b, k, m_sk, plain_modulus)) return rc;
+  if (batch == 0) return 0;
+  const uint64_t comp = level * n, words = 2 * comp, total = batch * words;
+  REQUIRE(result + total <= ct1 || ct1 + total <= result, "result and ct1 must not overlap");
+  REQUIRE(result + total <= ct2 || ct2 + total <= result, "result and ct2 must not overlap");
+  PtrInfo pi;
+  if (int rc = classify_all({result, ct1, ct2}, &pi)) return rc;
+  auto bound = [&](u64 i) { return moduli[i]; };
+  if (int rc = check_limb_bounds(ct1, 2 * batch, level, n, bound, pi, "ct1", stream)) return rc;
+  if (ct2 != ct1)
+    if (int rc = check_limb_bounds(ct2, 2 * batch, level, n, bound, pi, "ct2", stream)) return rc;
+  BfvPlan plan(level + k + 1);
+  if (int rc = bfv_plan(&plan, n, moduli, level, base_b, k, m_sk, plain_modulus)) return rc;
+  std::vector<uint64_t> bmods;
+  CachedNtts h(level + p_size);
+  if (int rc = hybrid_basis(n, level, q_size, p_size, moduli, &bmods, &h)) return rc;
+  // host pointers: both ciphertexts of a pair cross PCIe in once (one copy when squaring) and the product comes back
+  // from the same slot
+  if (pi.where == Where::Host) {
+    const bool square = ct1 == ct2;
+    return key_switch_host_batch(result, words, false, ct1, words, square ? words : 2 * words, &relin_keys, 1, batch,
+                                 [&](int dev, uint64_t* d_res, uint64_t* d_in, const uint64_t* const* const* dk,
+                                     cudaStream_t s) {
+                                   return bfv_multiply_relinearize_on_device(
+                                       dev, d_res, d_in, square ? d_in : d_in + words, plan, n, level, q_size, p_size,
+                                       alpha, h, bmods.data(), dk[0], s);
+                                 },
+                                 nullptr, square ? nullptr : ct2);
+  }
+  std::vector<const uint64_t* const*> dk;
+  if (keys_on_device(&relin_keys, 1, pi.device, &dk) < 1)
+    return fail(HEXL_B200_ERR_MIXED_POINTERS, "relin_keys holds no copy on the device of the ciphertexts");
+  return run_on_device(pi, stream, [&] {
+    for (uint64_t c = 0; c < batch; ++c)
+      if (int rc = bfv_multiply_relinearize_on_device(pi.device, result + c * words, ct1 + c * words,
+                                                      ct2 + c * words, plan, n, level, q_size, p_size, alpha, h,
+                                                      bmods.data(), dk[0], (cudaStream_t)stream))
         return rc;
     return 0;
   });

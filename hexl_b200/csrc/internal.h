@@ -189,6 +189,34 @@ inline u64 base_conv_targets(u64 from) { return (kBaseConvWords - 4 * from) / (5
 cudaError_t launch_base_conv(u64* result, u64 res_limb, u64 res_poly, const u64* operand, u64 op_limb, u64 op_poly,
                              u64 n, u64 polys, u64 from, u64 to, const BaseConvTable& tab, cudaStream_t stream);
 
+// BFV multiplication by BEHZ (bfv.cu), coefficient form, every modulus below 2^61, l = |Q| and k = |B| in [1, 64].
+// The constants are too many for the kernel parameters (l = k = 64 takes ~9000 words), so they live in a device table
+// (capi_bfv.cu caches one per parameter set and device).  Extension table, in words:
+//   per q_i (3):        q_i, [m~ (Q/q_i)^-1]_{q_i}, its Shoup factor
+//   per q_i (1):        [Q/q_i] mod 2^32;  then 1 word: [-Q^-1] mod 2^32
+//   per m of Bsk (8):   m, floor(2^64 / m), 2^64 mod m, its Shoup factor, [Q]_m, [-Q 2^32]_m, [2^-32]_m, its Shoup factor
+//   per m of Bsk (l):   [Q/q_i]_m for every i
+// Scaling table, in words:
+//   per q_i (3):        q_i, [t (Q/q_i)^-1]_{q_i}, its Shoup factor
+//   per m of Bsk (10):  m, floor(2^64 / m), 2^64 mod m, its Shoup factor, [t Q^-1]_m, Shoup, [-Q^-1]_m, Shoup,
+//                       [(B/b_j)^-1]_{b_j} and its Shoup factor (m = b_j; zeros for m_sk)
+//   per m of Bsk (l):   [Q/q_i]_m for every i
+//   per q_i, then m_sk (5): q, floor(2^64 / q), 2^64 mod q, its Shoup factor, [B]_q
+//   per q_i, then m_sk (k): [B/b_j]_q for every j
+//   2 words:            [B^-1]_{m_sk}, its Shoup factor
+// Bsk is ordered b_0..b_{k-1}, m_sk, and a lifted polynomial is l + k + 1 limbs: Q, then Bsk.
+constexpr unsigned kBehzTile = 32;
+// `polys` polynomials: polynomial p reads l limbs at operand + p op_poly and writes l + k + 1 limbs at
+// result + p res_poly (limb stride n both), its Q limbs copied
+cudaError_t launch_bfv_extend(u64* result, u64 res_poly, const u64* operand, u64 op_poly, u64 n, u64 polys, u64 l,
+                              u64 k, const u64* tab, cudaStream_t stream);
+// `polys` <= 3 tensor polynomials of l + k + 1 limbs, d_poly words apart, scaled by t/Q into l limbs at out.p[p]
+struct BfvOutputs {
+  u64* p[3];
+};
+cudaError_t launch_bfv_scale(const BfvOutputs& out, const u64* tensor, u64 d_poly, u64 n, u64 polys, u64 l, u64 k,
+                             const u64* tab, cudaStream_t stream);
+
 // Galois automorphism sigma_g (galois.cu).  NTT form: `polys` polynomials of 2^log_n words, one launch, words move
 // unchanged (result[j] = operand[pi_g(j)]).  Coefficient form: limbs [i0, i0 + cnt) of `polys` polynomials of rns
 // limbs each, limb i0 + e under mods.q[e]; galois_inv = g^-1 mod 2n.  result and operand must not overlap.

@@ -852,6 +852,31 @@ inline void InnerSumHybrid(uint64_t* result, const uint64_t* ciphertexts, uint64
                                                 galois_elt, sum_count, keys.data(), key_elts, num_keys,
                                                 rescale ? 1 : 0, batch, stream));
 }
+
+// extension: BFV ct1 x ct2 by BEHZ for each of `batch` pairs (2 x level_size limbs each, coefficient form), the tensor
+// scaled by t/Q stored at result + c * 3 * level_size * n as (d0, d1, d2) (hexl_b200_bfv_multiply has the definition
+// and the bound on B u {m_sk}).  moduli holds Q; base_b and m_sk are SEAL's base_B and m_sk; plain_modulus is t.
+// ct1 == ct2 squares.
+inline void BfvMultiply(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n, const uint64_t* moduli,
+                        uint64_t level_size, const uint64_t* base_b, uint64_t base_b_size, uint64_t m_sk,
+                        uint64_t plain_modulus, uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bfv_multiply(result, ct1, ct2, n, moduli, level_size, base_b, base_b_size, m_sk,
+                                            plain_modulus, batch, stream));
+}
+
+// extension: BfvMultiply followed by the relinearization of d2 with hybrid keys that switch s^2 to s, in coefficient
+// form: (d0, d1) + KS(d2) stored at result + c * 2 * level_size * n.  Moduli, digits and keys as for
+// MultiplyRelinearizeHybrid; bit for bit BfvMultiply, the forward transform of d2, KeySwitchHybrid, the inverse
+// transform and the addition of (d0, d1).
+inline void BfvMultiplyRelinearizeHybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                         uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                         const uint64_t* moduli, const uint64_t* base_b, uint64_t base_b_size,
+                                         uint64_t m_sk, uint64_t plain_modulus, const KeySwitchKeys& relin_keys,
+                                         uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bfv_multiply_relinearize_hybrid(result, ct1, ct2, n, level_size, q_size, p_size,
+                                                               digit_size, moduli, base_b, base_b_size, m_sk,
+                                                               plain_modulus, relin_keys.Handle(), batch, stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

@@ -671,6 +671,79 @@ int hexl_b200_inner_sum_hybrid(uint64_t* result, const uint64_t* ciphertexts, ui
                                uint64_t galois_elt, uint64_t sum_count, const hexl_b200_keys* const* galois_keys,
                                const uint64_t* key_elts, uint64_t num_keys, int rescale, uint64_t batch, void* stream);
 
+/* BFV ciphertext multiplication by BEHZ (extension; Bajard, Eynard, Hasan, Zucca 2016; SEAL's Evaluator::multiply for
+ * BFV with its RNSTool): the tensor of two ciphertexts scaled by t/Q, integer arithmetic only, for each of `batch`
+ * pairs.  Q = q_0..q_{l-1} (moduli, l = level_size), B = b_0..b_{k-1} (base_b, k = base_b_size), Bsk = B u {m_sk},
+ * m~ = 2^32 and t = plain_modulus.  Pair c reads ct1 + c*2*l*n and ct2 + c*2*l*n, two components of l limbs each in
+ * COEFFICIENT form (SEAL's BFV form), canonical; its product is STORED at result + c*3*l*n as (d0, d1, d2), l limbs
+ * each, coefficient form, canonical.  With FBC the conversion of hexl_b200_fast_base_convert, per input polynomial x:
+ *   y_i  = [x_i m~]_{q_i},  z_m = FBC(y; Q -> m) for m in Bsk u {m~}
+ *   r    = [-z_m~ Q^-1]_m~,  r_c = r - m~ if r >= m~/2 else r
+ *   x'_m = [(z_m + [Q]_m r_c) m~^-1]_m for m in Bsk,  x'_{q_i} = x_i                       (SEAL's sm_mrq)
+ * per modulus m of Q u Bsk, (a0, a1) and (b0, b1) the lifted inputs, negacyclic products mod m (forward NTT, dyadic,
+ * inverse NTT):
+ *   D0 = a0 b0,  D1 = a0 b1 + a1 b0,  D2 = a1 b1
+ * and per output polynomial D over Q u Bsk:
+ *   u_i   = [t D_{q_i}]_{q_i},  w_m = [(t D_m - FBC(u; Q -> m)) [Q^-1]_m]_m for m in Bsk    (fast_floor)
+ *   c_i   = FBC(w_B; B -> q_i),  gamma = FBC(w_B; B -> m_sk),  alpha = [(gamma - w_{m_sk}) [B^-1]_{m_sk}]_{m_sk}
+ *   out_i = [c_i + [B]_{q_i} (m_sk - alpha)]_{q_i} if alpha > floor(m_sk/2), else [c_i - [B]_{q_i} alpha]_{q_i}
+ *                                                                                                (fastbconv_sk)
+ * Each out coefficient is floor(t D / Q) - v mod Q with 0 <= v < l, D the integer tensor of the lifts, exactly when
+ * Bsk passes this bound, which the call checks with exact integers:
+ *   n t Q (m~ + 2l)^2 + 2 (l + 1) m~^2 <= B (m_sk - 1 - 2k) m~^2.
+ * Why: the lift is x' = x mod Q with -Q/2 <= x' < lambda Q, lambda = 1/2 + l/m~; so |D| < 2 n lambda^2 Q^2 (D1 sums 2n
+ * products); the fast floor gives w = floor(t D / Q) - v, |w| < 2 n t lambda^2 Q + l + 1; Shenoy-Kumaresan returns w
+ * exactly when |w| <= B ((m_sk - 1)/2 - k).  Multiplied through by 2 m~^2 that is the test.  Every B of SEAL's rule
+ * (|B| = l, or l + 1 when 32 + bits(t) + bits(Q) >= 61 (l + 1), 61-bit primes, and a 61-bit m_sk) passes it.
+ * ct1 == ct2 (squaring) is allowed; the inputs are only read.  batch = 0 does nothing.  HEXL_B200_ERR_INVALID_ARG for a
+ * null pointer, n not a power of two in [2, 2^20], l or k outside [1, 64], plain_modulus outside [2, 2^61), a modulus of
+ * Q u Bsk that is >= 2^61, not NTT-friendly for n or not coprime to the others, result overlapping an input, and Bsk
+ * failing the bound.  Inputs are checked below their modulus under hexl_b200_set_debug(1).  On the device, per pair: one
+ * extension launch per input ciphertext (one when squaring) that reads the l limbs and writes all l + k + 1; one
+ * forward transform of the four (two) lifted polynomials (ceil(4 (l + k + 1) / 64) launches); one DyadicMultiply
+ * launch per block of 64 moduli; one inverse transform of the tensor (ceil(3 (l + k + 1) / 64) launches); and one
+ * scaling launch that reads l + k + 1 limbs and writes l.  The kernels' constants live in a device table built and
+ * uploaded on first use per (Q, B, m_sk, t) and device, so device calls capture into a CUDA graph once the call has
+ * run once on that device and the transforms are warm.  Library scratch: 7 x (l + k + 1) x n words (5 when squaring).
+ * Host buffers: both ciphertexts of a pair cross PCIe in once (one copy when squaring) and the product comes back on
+ * the same staging stream, split by pair over the devices of hexl_b200_set_host_devices.  Managed buffers take the
+ * device path.  Not covered: HPS or other floating-point scaling, BGV, inputs of more than two components, choosing B
+ * or m_sk (the caller's context does), and an in-place variant. */
+int hexl_b200_bfv_multiply(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                           const uint64_t* moduli, uint64_t level_size, const uint64_t* base_b, uint64_t base_b_size,
+                           uint64_t m_sk, uint64_t plain_modulus, uint64_t batch, void* stream);
+
+/* BFV ciphertext multiplication relinearized with hybrid keys (extension; SEAL's multiply + relinearize for BFV): the
+ * product of hexl_b200_bfv_multiply followed by the key switch of its d2.  The moduli, digits, key handle (one
+ * relinearization key, s^2 -> s, key_component_count 2) and shape rules are those of
+ * hexl_b200_multiply_relinearize_hybrid; Q is the first l = level_size data moduli and base_b, m_sk, plain_modulus are
+ * the BEHZ bases and plain modulus of hexl_b200_bfv_multiply for that level.  Pair c reads ct1 + c*2*l*n and
+ * ct2 + c*2*l*n (coefficient form, canonical) and its result is STORED at result + c*2*l*n, coefficient form,
+ * canonical:
+ *   (d0, d1, d2) = hexl_b200_bfv_multiply(ct1, ct2)
+ *   result       = (d0, d1) + KS(d2)
+ * with KS the switch of hexl_b200_key_switch_hybrid taken in coefficient form: the mod-up reads d2's limbs directly,
+ * and the mod-down brings the data limbs of the products back to coefficients and adds (INTT(prod) - c) P^-1, c the
+ * rounded conversion of the special limbs.  Every step is canonical and the NTT a bijection, so this is bit for bit the
+ * chain hexl_b200_bfv_multiply; hexl_b200_ntt_forward_multi of d2; hexl_b200_key_switch_hybrid into a zeroed
+ * two-component result; hexl_b200_ntt_inverse_multi; hexl_b200_eltwise_add_mod_multi with (d0, d1).  At digit_size = 1
+ * with one special prime it is therefore SEAL's multiply + relinearize with hexl_b200_key_switch_resident.  It decrypts
+ * under (1, s) to the product's message within the product's noise plus one key switch's.  HEXL_B200_ERR_INVALID_ARG
+ * on the refusals of hexl_b200_multiply_relinearize_hybrid (rescale aside) and of hexl_b200_bfv_multiply.  ct1 == ct2
+ * squares; batch = 0 does nothing.  On the device, per pair: the launches of hexl_b200_bfv_multiply, then those of
+ * hexl_b200_key_switch_hybrid with kcc = 2 less its first inverse transform, and in the mod-down an inverse transform
+ * of the products' data limbs in place of the forward transform of the correction.  Library scratch: that of
+ * hexl_b200_bfv_multiply plus l x n words of d2, one round of converted digits and (l + p_size) x 2 x n words of
+ * products.  Device calls capture into a CUDA graph once the call has run once on that device.  Host buffers: as for
+ * hexl_b200_bfv_multiply, split by pair over the devices where the handle holds a copy.  Not covered: keys sharded by
+ * modulus (refused), a relinearize-only call for three-component coefficient-form ciphertexts, BFV rotations, and an
+ * in-place variant. */
+int hexl_b200_bfv_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                              uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                              uint64_t digit_size, const uint64_t* moduli, const uint64_t* base_b,
+                                              uint64_t base_b_size, uint64_t m_sk, uint64_t plain_modulus,
+                                              const hexl_b200_keys* relin_keys, uint64_t batch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
