@@ -144,6 +144,13 @@ _sig("hexl_b200_inner_sum_hybrid", _int,
 _sig("hexl_b200_bfv_multiply", _int, [_vp, _vp, _vp, _u64, _vp, _u64, _vp, _u64, _u64, _u64, _u64, _vp])
 _sig("hexl_b200_bfv_multiply_relinearize_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _vp, _u64, _u64, _u64, _vp, _u64, _vp])
+_sig("hexl_b200_bgv_mod_switch", _int, [_vp, _vp, _u64, _vp, _u64, _u64, _u64, _int, _vp])
+_sig("hexl_b200_bgv_key_switch_hybrid", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _vp, _u64, _vp])
+_sig("hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted", _int,
+     [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _vp, _vp, _u64, _u64, _vp])
+_sig("hexl_b200_bgv_multiply_relinearize_hybrid", _int,
+     [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _vp, _int, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -842,5 +849,72 @@ def BfvMultiplyRelinearizeHybrid(result, ct1, ct2, n, level_size, q_size, p_size
                                                           mods.ctypes.data, bb.ctypes.data, bb.size, m_sk,
                                                           plain_modulus,
                                                           relin_keys._h if relin_keys is not None else None, batch,
+                                                          _stream(stream, rc or ac or bc)))
+    return result
+
+
+# ------------------------------------------------------------------ BGV
+def BgvModSwitch(result, operand, n, moduli, rns_modulus_size, plain_modulus, count=1, ntt_form=True, stream=None):
+    """BGV modulus switch of `count` polynomials of rns_modulus_size limbs (n words each) by their last modulus
+    (hexl_b200_bgv_mod_switch; SEAL's mod_t_and_divide_q_last(_ntt)_inplace): DivideAndRoundQLast's layout with the
+    rounding replaced by a correction that is 0 mod plain_modulus.  Limb L of result is not written; result may be
+    operand.  The message picks up [q_L^-1]_t."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); op, on, oc = _buf(operand)
+    _need("moduli", mods.size, rns_modulus_size)
+    _need("result", rn, count * rns_modulus_size * n); _need("operand", on, count * rns_modulus_size * n)
+    _check(_lib.hexl_b200_bgv_mod_switch(rp, op, n, mods.ctypes.data, rns_modulus_size, plain_modulus, count,
+                                         int(bool(ntt_form)), _stream(stream, rc or oc)))
+    return result
+
+
+def BgvKeySwitchHybrid(result, target, n, level_size, q_size, p_size, digit_size, key_component_count, moduli,
+                       plain_modulus, keys: KeySwitchKeys, batch=1, stream=None):
+    """KeySwitchHybrid for BGV (hexl_b200_bgv_key_switch_hybrid): the same layouts, with the mod-down by P subtracting
+    a correction that is 0 mod plain_modulus.  Accumulates into result."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); tp, tn, tc = _buf(target)
+    _need("moduli", mods.size, q_size + p_size)
+    _need("result", rn, batch * key_component_count * level_size * n); _need("target", tn, batch * level_size * n)
+    _check(_lib.hexl_b200_bgv_key_switch_hybrid(rp, tp, n, level_size, q_size, p_size, digit_size,
+                                                key_component_count, mods.ctypes.data, plain_modulus,
+                                                keys._h if keys is not None else None, batch,
+                                                _stream(stream, rc or tc)))
+    return result
+
+
+def BgvApplyGaloisKeySwitchHybridHoisted(results, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli,
+                                         plain_modulus, galois_keys, galois_elts, batch=1, stream=None):
+    """ApplyGaloisKeySwitchHybridHoisted for BGV (hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted): SEAL's
+    rotate_rows / rotate_columns for every element of galois_elts with one mod-up, the same layouts."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    elts = np.ascontiguousarray(galois_elts, dtype=np.uint64)
+    rp, rn, rc = _buf(results); cp, cn, cc = _buf(ciphertexts)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size); _need("galois_keys", len(galois_keys), elts.size)
+    _need("results", rn, batch * elts.size * per); _need("ciphertexts", cn, batch * per)
+    keys = (_vp * max(1, len(galois_keys)))(*[k._h if k is not None else None for k in galois_keys])
+    _check(_lib.hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted(rp, cp, n, level_size, q_size, p_size,
+                                                                     digit_size, mods.ctypes.data, plain_modulus,
+                                                                     keys, elts.ctypes.data, elts.size, batch,
+                                                                     _stream(stream, rc or cc)))
+    return results
+
+
+def BgvMultiplyRelinearizeHybrid(result, ct1, ct2, n, level_size, q_size, p_size, digit_size, moduli, plain_modulus,
+                                 relin_keys: KeySwitchKeys, mod_switch=False, batch=1, stream=None):
+    """MultiplyRelinearizeHybrid for BGV (hexl_b200_bgv_multiply_relinearize_hybrid): the same layouts, the mod-down
+    t-corrected; mod_switch=True drops the last limb in the same mod-down (the message picks up [q_{l-1}^-1]_t).
+    mod_switch=False equals DyadicMultiply followed by BgvKeySwitchHybrid bit for bit.  ct1 may be ct2."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); ap, an, ac = _buf(ct1); bp, bn, bc = _buf(ct2)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, q_size + p_size)
+    _need("result", rn, batch * 2 * (level_size - int(bool(mod_switch))) * n)
+    _need("ct1", an, batch * per); _need("ct2", bn, batch * per)
+    _check(_lib.hexl_b200_bgv_multiply_relinearize_hybrid(rp, ap, bp, n, level_size, q_size, p_size, digit_size,
+                                                          mods.ctypes.data, plain_modulus,
+                                                          relin_keys._h if relin_keys is not None else None,
+                                                          int(bool(mod_switch)), batch,
                                                           _stream(stream, rc or ac or bc)))
     return result

@@ -1,6 +1,6 @@
 // What the host sources of the C ABI (include/hexl_b200.h) share: capi.cu (library state, staging, scratch pool),
 // capi_ntt.cu, capi_eltwise.cu, capi_keyswitch.cu (key switch, key handles, rescale), capi_galois.cu and
-// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations and multiplication with hybrid keys).
+// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations and multiplication with hybrid keys, CKKS and BGV).
 // Host-side responsibilities, all one-off or O(1) per call:
 //   * argument validation mirroring the reference's HEXL_CHECKs,
 //   * NTT handle = (N, q, root) -> twiddle tables, built on the host exactly as
@@ -415,6 +415,16 @@ int key_switch_host_batch(uint64_t* result, uint64_t res_words, bool result_in, 
                           uint64_t buf_words, const hexl_b200_keys* const* keys, uint64_t num_keys, uint64_t batch,
                           const HostSwitch& run, const std::function<int(int)>& prepare = nullptr,
                           const uint64_t* in2 = nullptr);
+
+// Fast base conversion of `polys` polynomials from the moduli `from` into the moduli `to` (capi_hybrid.cu): plain
+// (round = false), rounded (the CKKS mod-down) or, with plain_modulus = tau != 0, t-corrected (the BGV mod-down and
+// modulus switch); strides as launch_base_conv, device pointers on the current device, asynchronous on s.
+int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t res_poly, const uint64_t* operand,
+                           uint64_t op_limb, uint64_t op_poly, uint64_t n, uint64_t polys, const uint64_t* from,
+                           uint64_t from_count, const uint64_t* to, uint64_t to_count, bool round, cudaStream_t s,
+                           uint64_t plain_modulus = 0);
+// The BGV refusal of a plain modulus: outside [2, 2^61), or sharing a factor with one of moduli[0, count)
+int bgv_plain_modulus_check(uint64_t plain_modulus, const uint64_t* moduli, uint64_t count);
 
 // BFV multiplication by BEHZ (capi_bfv.cu).  The refusals of hexl_b200_bfv_multiply that do not depend on the
 // buffers' memory: null pointers, shapes, moduli, plain modulus and the bound on Bsk.

@@ -26,13 +26,72 @@ static uint64_t half_product_mod(const uint64_t* moduli, uint64_t count, uint64_
 // `to`, device pointers on the current device, asynchronous on s; strides as launch_base_conv.  One launch per block of
 // base_conv_targets(from_count) targets; the constants are computed here, per call.  round (the mod-down by
 // P = Q): x_i + [floor(P/2)]_{q_i} on input and - [floor(P/2)]_t on output, so that an input X in [0, P) comes out as
-// the centred lift of X + floor(P/2) minus floor(P/2), plus e P with 0 <= e < from_count.
-static int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t res_poly, const uint64_t* operand,
-                                  uint64_t op_limb, uint64_t op_poly, uint64_t n, uint64_t polys,
-                                  const uint64_t* from, uint64_t from_count, const uint64_t* to, uint64_t to_count,
-                                  bool round, cudaStream_t s) {
+// the centred lift of X + floor(P/2) minus floor(P/2), plus e P with 0 <= e < from_count.  plain_modulus = tau != 0
+// (BGV's mod-down, round ignored): the t-corrected conversion of launch_base_conv_t instead, one launch per block of
+// base_conv_t_targets(from_count) targets, which yields delta = X mod P with delta = 0 mod tau.
+int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t res_poly, const uint64_t* operand,
+                           uint64_t op_limb, uint64_t op_poly, uint64_t n, uint64_t polys, const uint64_t* from,
+                           uint64_t from_count, const uint64_t* to, uint64_t to_count, bool round, cudaStream_t s,
+                           uint64_t plain_modulus) {
   const uint64_t F = from_count, block = base_conv_targets(F);
+  std::vector<uint64_t> prefix(F + 1), suffix(F + 1);
   BaseConvTable tab;
+  // [Q/q_i]_t for every source i into row[0..F)
+  auto cofactors = [&](uint64_t t, uint64_t* row) {
+    prefix[0] = suffix[F] = 1 % t;
+    for (uint64_t i = 0; i < F; ++i) prefix[i + 1] = mul_mod128(prefix[i], from[i] % t, t);
+    for (uint64_t i = F; i-- > 0;) suffix[i] = mul_mod128(suffix[i + 1], from[i] % t, t);
+    for (uint64_t i = 0; i < F; ++i) row[i] = mul_mod128(prefix[i], suffix[i + 1], t);
+  };
+  // t, floor(2^64 / t), 2^64 mod t and its Shoup factor into row[0..4)
+  auto reducer = [](uint64_t t, uint64_t* row) {
+    const uint64_t mu = nt::multiply_factor(1, 64, t);
+    const Twiddle R = make_twiddle(mu * (0 - t) % t, t);
+    row[0] = t;
+    row[1] = mu;
+    row[2] = R.w;
+    row[3] = R.wp;
+  };
+  if (plain_modulus) {
+    const uint64_t tau = plain_modulus, tblock = base_conv_t_targets(F);
+    for (uint64_t i = 0; i < F; ++i) {
+      const uint64_t q = from[i];
+      uint64_t rest = 1 % q;
+      for (uint64_t j = 0; j < F; ++j)
+        if (j != i) rest = mul_mod128(rest, from[j] % q, q);
+      const Twiddle inv = make_twiddle(nt::inverse_mod(rest, q), q);
+      tab.w[3 * i] = q;
+      tab.w[3 * i + 1] = inv.w;
+      tab.w[3 * i + 2] = inv.wp;
+    }
+    uint64_t* trow = tab.w + 3 * F;
+    reducer(tau, trow);
+    uint64_t P_tau = 1 % tau;
+    for (uint64_t i = 0; i < F; ++i) P_tau = mul_mod128(P_tau, from[i] % tau, tau);
+    const Twiddle neg_inv = make_twiddle((tau - nt::inverse_mod(P_tau, tau)) % tau, tau);
+    trow[4] = neg_inv.w;
+    trow[5] = neg_inv.wp;
+    cofactors(tau, trow + 6);
+    for (uint64_t e0 = 0; e0 < to_count; e0 += tblock) {
+      const uint64_t cnt = std::min(tblock, to_count - e0);
+      uint64_t* targets = trow + 6 + F;
+      uint64_t* matrix = targets + 6 * cnt;
+      for (uint64_t e = 0; e < cnt; ++e) {
+        const uint64_t t = to[e0 + e];
+        reducer(t, targets + 6 * e);
+        uint64_t P = 1 % t;
+        for (uint64_t i = 0; i < F; ++i) P = mul_mod128(P, from[i] % t, t);
+        const Twiddle Pt = make_twiddle(P, t);
+        targets[6 * e + 4] = Pt.w;
+        targets[6 * e + 5] = Pt.wp;
+        cofactors(t, matrix + e * F);
+      }
+      const cudaError_t e = launch_base_conv_t(result + e0 * res_limb, res_limb, res_poly, operand, op_limb, op_poly,
+                                               n, polys, F, cnt, tab, s);
+      if (e != cudaSuccess) return cuda_fail(e, "t-corrected base conversion launch");
+    }
+    return 0;
+  }
   // (Q/q_i)^-1 mod q_i from prefix and suffix products under q_i
   for (uint64_t i = 0; i < F; ++i) {
     const uint64_t q = from[i];
@@ -45,23 +104,15 @@ static int base_convert_on_device(uint64_t* result, uint64_t res_limb, uint64_t 
     tab.w[4 * i + 2] = inv.wp;
     tab.w[4 * i + 3] = round ? half_product_mod(from, F, q) : 0;
   }
-  std::vector<uint64_t> prefix(F + 1), suffix(F + 1);
   for (uint64_t e0 = 0; e0 < to_count; e0 += block) {
     const uint64_t cnt = std::min(block, to_count - e0);
     uint64_t* targets = tab.w + 4 * F;
     uint64_t* matrix = targets + 5 * cnt;
     for (uint64_t e = 0; e < cnt; ++e) {
-      const uint64_t t = to[e0 + e], mu = nt::multiply_factor(1, 64, t);
-      const Twiddle R = make_twiddle(mu * (0 - t) % t, t);  // 2^64 mod t
-      targets[5 * e] = t;
-      targets[5 * e + 1] = mu;
-      targets[5 * e + 2] = R.w;
-      targets[5 * e + 3] = R.wp;
+      const uint64_t t = to[e0 + e];
+      reducer(t, targets + 5 * e);
       targets[5 * e + 4] = round ? half_product_mod(from, F, t) : 0;
-      prefix[0] = suffix[F] = 1 % t;
-      for (uint64_t i = 0; i < F; ++i) prefix[i + 1] = mul_mod128(prefix[i], from[i] % t, t);
-      for (uint64_t i = F; i-- > 0;) suffix[i] = mul_mod128(suffix[i + 1], from[i] % t, t);
-      for (uint64_t i = 0; i < F; ++i) matrix[e * F + i] = mul_mod128(prefix[i], suffix[i + 1], t);  // [Q/q_i]_t
+      cofactors(t, matrix + e * F);
     }
     const cudaError_t e = launch_base_conv(result + e0 * res_limb, res_limb, res_poly, operand, op_limb, op_poly, n,
                                            polys, F, cnt, tab, s);
@@ -122,15 +173,16 @@ static int hybrid_mod_up(int dev, const uint64_t* target, uint64_t n, uint64_t l
 // level - 1 and p_size + 1 it divides by q_{level-1} P as well, the mod-down merged with the rescale.  coef: result is
 // in coefficient form; the products' data limbs go back to coefficients in place instead of the rounded correction
 // being transformed forward, and the finish, point-wise, is the same: INTT((prod - NTT(c)) P^-1) = (INTT(prod) - c) P^-1.
+// plain_modulus = tau != 0 (BGV): the t-corrected conversion in place of the rounded one, so that c = 0 mod tau.
 static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* tmp, uint64_t n, uint64_t level,
                            uint64_t p_size, uint64_t kcc, const CachedNtts& h, const uint64_t* bmods, bool accumulate,
-                           cudaStream_t s, bool coef = false) {
+                           cudaStream_t s, bool coef = false, uint64_t plain_modulus = 0) {
   uint64_t* special = prod + level * kcc * n;  // [j][k][n]
   if (int rc = ntt_multi_on_device(false, dev, h.data() + level, p_size, special, special, 1, kcc, s)) return rc;
   for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {
     const uint64_t cnt = std::min<uint64_t>(kParamBlock, level - i0);
     if (int rc = base_convert_on_device(tmp, kcc * n, n, special, kcc * n, n, n, kcc, bmods + level, p_size,
-                                        bmods + i0, cnt, true, s))
+                                        bmods + i0, cnt, true, s, plain_modulus))
       return rc;
     if (coef) {
       uint64_t* data = prod + i0 * kcc * n;
@@ -158,11 +210,12 @@ static int hybrid_mod_down(int dev, uint64_t* result, uint64_t* prod, uint64_t* 
 // kcc x (q_size + K) x n words) and one mod-down accumulated into results[r].  galois_elts[r] (nullptr: none) makes
 // switch r read the transformed digits permuted by pi_g, as key_switch_elts_on_device does for the hoisted
 // rotations.  Scratch: one round of transformed digits plus elts x (level + K) x kcc x n words of products.
+// plain_modulus != 0: the mod-downs are BGV's t-corrected ones (hybrid_mod_down).
 static int key_switch_hybrid_elts_on_device(int dev, uint64_t* const* results, const uint64_t* target, uint64_t n,
                                             uint64_t level, uint64_t q_size, uint64_t p_size, uint64_t alpha,
                                             uint64_t kcc, const CachedNtts& h, const uint64_t* bmods,
                                             const uint64_t* const* const* keys, const uint64_t* galois_elts,
-                                            uint64_t elts, cudaStream_t s) {
+                                            uint64_t elts, cudaStream_t s, uint64_t plain_modulus = 0) {
   const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size;
   Scratch ws(s);
   uint64_t *prod = nullptr, *tmp = nullptr;
@@ -177,7 +230,8 @@ static int key_switch_hybrid_elts_on_device(int dev, uint64_t* const* results, c
     return rc;
   for (uint64_t r = 0; r < elts; ++r)
     if (int rc =
-            hybrid_mod_down(dev, results[r], prod + r * nb * kcc * n, tmp, n, level, p_size, kcc, h, bmods, true, s))
+            hybrid_mod_down(dev, results[r], prod + r * nb * kcc * n, tmp, n, level, p_size, kcc, h, bmods, true, s,
+                            false, plain_modulus))
       return rc;
   return 0;  // asynchronous on s; ~Scratch returns the buffers to the pool in stream order
 }
@@ -185,9 +239,9 @@ static int key_switch_hybrid_elts_on_device(int dev, uint64_t* const* results, c
 static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level,
                                        uint64_t q_size, uint64_t p_size, uint64_t alpha, uint64_t kcc,
                                        const CachedNtts& h, const uint64_t* bmods, const uint64_t* const* keys,
-                                       cudaStream_t s) {
+                                       cudaStream_t s, uint64_t plain_modulus) {
   return key_switch_hybrid_elts_on_device(dev, &result, target, n, level, q_size, p_size, alpha, kcc, h, bmods, &keys,
-                                          nullptr, 1, s);
+                                          nullptr, 1, s, plain_modulus);
 }
 
 // The hoisted hybrid rotations of one ciphertext ct (two components of level limbs, NTT form, device memory) by
@@ -196,7 +250,8 @@ static int key_switch_hybrid_on_device(int dev, uint64_t* result, const uint64_t
 static int hybrid_hoisted_on_device(int dev, uint64_t* out, const uint64_t* ct, uint64_t n, uint64_t level,
                                     uint64_t q_size, uint64_t p_size, uint64_t alpha, const CachedNtts& h,
                                     const uint64_t* bmods, const uint64_t* const* const* keys,
-                                    const uint64_t* galois_elts, uint64_t elts, cudaStream_t s) {
+                                    const uint64_t* galois_elts, uint64_t elts, cudaStream_t s,
+                                    uint64_t plain_modulus) {
   const uint64_t comp = level * n;
   std::vector<uint64_t*> results(elts);
   for (uint64_t r = 0; r < elts; ++r) {
@@ -206,7 +261,7 @@ static int hybrid_hoisted_on_device(int dev, uint64_t* out, const uint64_t* ct, 
     CU(cudaMemsetAsync(results[r] + comp, 0, comp * sizeof(uint64_t), s));
   }
   return key_switch_hybrid_elts_on_device(dev, results.data(), ct + comp, n, level, q_size, p_size, alpha, 2, h, bmods,
-                                          keys, galois_elts, elts, s);
+                                          keys, galois_elts, elts, s, plain_modulus);
 }
 
 // The hybrid linear transform of one ciphertext ct (as above) into result (2 x level x n words, device memory):
@@ -403,12 +458,13 @@ static int bsgs_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct, 
 // by P or, with rescale, by q_{level-1} P (q_{level-1} is the limb of B right before the special limbs).  Scratch: one
 // round of transformed digits plus (level + K) x 2 x n words of products.  sum (nullptr: none) holds the tensor
 // (d0, d1, t) already formed ([3][level][n], canonical): the mod-up then reads t, the storing launches read d0 and d1,
-// and ct1 and ct2 are not read.
+// and ct1 and ct2 are not read.  plain_modulus != 0 (BGV): the mod-down is t-corrected, and with rescale it is the
+// merged modulus switch by q_{level-1} P.
 static int multiply_relinearize_hybrid_on_device(int dev, uint64_t* result, const uint64_t* ct1, const uint64_t* ct2,
                                                  uint64_t n, uint64_t level, uint64_t q_size, uint64_t p_size,
                                                  uint64_t alpha, bool rescale, const CachedNtts& h,
                                                  const uint64_t* bmods, const uint64_t* const* keys, cudaStream_t s,
-                                                 const uint64_t* sum = nullptr) {
+                                                 const uint64_t* sum = nullptr, uint64_t plain_modulus = 0) {
   const uint64_t D = (level + alpha - 1) / alpha, nb = level + p_size, kms = q_size + p_size, comp = level * n;
   Scratch ws(s);
   uint64_t *prod = nullptr, *tmp = nullptr;
@@ -445,6 +501,9 @@ static int multiply_relinearize_hybrid_on_device(int dev, uint64_t* result, cons
   const int up = sum ? hybrid_mod_up(dev, sum + 2 * comp, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s)
                      : hybrid_mod_up(dev, ct1 + comp, n, level, q_size, p_size, alpha, h, bmods, ws, mac, s, ct2 + comp);
   if (up) return up;
+  if (plain_modulus)  // BGV: the t-corrected mod-down by P, or by q_{level-1} P (the merged modulus switch)
+    return hybrid_mod_down(dev, result, prod, tmp, n, level - rescale, p_size + rescale, 2, h, bmods, false, s, false,
+                           plain_modulus);
   if (rescale) return hybrid_mod_down(dev, result, prod, tmp, n, level - 1, p_size + 1, 2, h, bmods, false, s);
   return hybrid_mod_down(dev, result, prod, tmp, n, level, p_size, 2, h, bmods, false, s);
 }
@@ -666,6 +725,15 @@ static int hybrid_shape_check(uint64_t n, uint64_t level, uint64_t q_size, uint6
   return 0;
 }
 
+int bgv_plain_modulus_check(uint64_t plain_modulus, const uint64_t* moduli, uint64_t count) {
+  // the t-corrected conversion reduces its 128-bit sums mod tau with the lazy reductions of every other target
+  REQUIRE(plain_modulus >= 2 && plain_modulus < (1ull << 61), "Require 2 <= plain_modulus < 2^61");
+  for (uint64_t i = 0; i < count; ++i)
+    REQUIRE(std::gcd(plain_modulus, moduli[i]) == 1, "Require plain_modulus coprime to moduli[%llu]",
+            (unsigned long long)i);
+  return 0;
+}
+
 // A hybrid key handle of the shape: ceil(q_size / digit_size) digits, kcc x (q_size + p_size) words, not sharded
 static int hybrid_handle_check(const hexl_b200_keys* keys, uint64_t n, uint64_t q_size, uint64_t p_size,
                                uint64_t alpha, uint64_t kcc, const char* what) {
@@ -749,12 +817,20 @@ int hexl_b200_fast_base_convert(uint64_t* result, const uint64_t* operand, uint6
   return base_convert_host(result, operand, n, from_moduli, from_count, to_moduli, to_count, count);
 }
 
-int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
-                                uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
-                                const uint64_t* moduli, const hexl_b200_keys* keys, uint64_t batch, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// hexl_b200_key_switch_hybrid, and with bgv hexl_b200_bgv_key_switch_hybrid
+int key_switch_hybrid_call(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size, uint64_t q_size,
+                           uint64_t p_size, uint64_t digit_size, uint64_t key_component_count, const uint64_t* moduli,
+                           const hexl_b200_keys* keys, uint64_t batch, void* stream, bool bgv,
+                           uint64_t plain_modulus) {
   const uint64_t level = level_size, alpha = digit_size, kcc = key_component_count;
   REQUIRE(result && target && moduli && keys, "Require non-null arguments");
   if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, kcc, moduli)) return rc;
+  if (bgv)
+    if (int rc = bgv_plain_modulus_check(plain_modulus, moduli, q_size + p_size)) return rc;
   if (int rc = hybrid_handle_check(keys, n, q_size, p_size, alpha, kcc, "the key handle")) return rc;
   if (batch == 0) return 0;
   const uint64_t in_words = level * n, out_words = kcc * level * n;
@@ -771,7 +847,8 @@ int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64
                                  [&](int dev, uint64_t* d_res, uint64_t* d_t, const uint64_t* const* const* dk,
                                      cudaStream_t s) {
                                    return key_switch_hybrid_on_device(dev, d_res, d_t, n, level, q_size, p_size,
-                                                                      alpha, kcc, h, bmods.data(), dk[0], s);
+                                                                      alpha, kcc, h, bmods.data(), dk[0], s,
+                                                                      plain_modulus);
                                  });
   std::vector<const uint64_t* const*> dk;
   if (keys_on_device(&keys, 1, pi.device, &dk) < 1)
@@ -780,15 +857,11 @@ int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64
     for (uint64_t c = 0; c < batch; ++c)
       if (int rc = key_switch_hybrid_on_device(pi.device, result + c * out_words, target + c * in_words, n, level,
                                                q_size, p_size, alpha, kcc, h, bmods.data(), dk[0],
-                                               (cudaStream_t)stream))
+                                               (cudaStream_t)stream, plain_modulus))
         return rc;
     return 0;
   });
 }
-
-}  // extern "C"
-
-namespace {
 
 // The element and key-handle rules of the two hybrid rotation calls.  identity_ok: a null handle is an identity term,
 // allowed for the element 1 only; otherwise every handle must be there.
@@ -819,20 +892,17 @@ std::vector<const uint64_t* const*> per_element(const hexl_b200_keys* const* key
   return out;
 }
 
-}  // namespace
-
-extern "C" {
-
-int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
-                                                     uint64_t level_size, uint64_t q_size, uint64_t p_size,
-                                                     uint64_t digit_size, const uint64_t* moduli,
-                                                     const hexl_b200_keys* const* galois_keys,
-                                                     const uint64_t* galois_elts, uint64_t num_elts, uint64_t batch,
-                                                     void* stream) {
+// hexl_b200_apply_galois_key_switch_hybrid_hoisted, and with bgv its BGV form
+int hoisted_hybrid_call(uint64_t* results, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
+                        uint64_t q_size, uint64_t p_size, uint64_t digit_size, const uint64_t* moduli,
+                        const hexl_b200_keys* const* galois_keys, const uint64_t* galois_elts, uint64_t num_elts,
+                        uint64_t batch, void* stream, bool bgv, uint64_t plain_modulus) {
   const uint64_t level = level_size, alpha = digit_size;
   REQUIRE(results && ciphertexts && moduli, "Require non-null arguments");
   REQUIRE(num_elts == 0 || (galois_keys && galois_elts), "Require galois_keys, galois_elts != nullptr");
   if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (bgv)
+    if (int rc = bgv_plain_modulus_check(plain_modulus, moduli, q_size + p_size)) return rc;
   if (int rc = hybrid_elts_check(n, q_size, p_size, alpha, galois_keys, galois_elts, num_elts, false)) return rc;
   if (num_elts == 0 || batch == 0) return 0;
   const uint64_t comp = level * n, in_total = batch * 2 * comp, out_total = batch * num_elts * 2 * comp;
@@ -853,7 +923,8 @@ int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const ui
                                  [&](int dev, uint64_t* d_res, uint64_t* d_ct, const uint64_t* const* const* dk,
                                      cudaStream_t s) {
                                    return hybrid_hoisted_on_device(dev, d_res, d_ct, n, level, q_size, p_size, alpha,
-                                                                   h, bmods.data(), dk, galois_elts, num_elts, s);
+                                                                   h, bmods.data(), dk, galois_elts, num_elts, s,
+                                                                   plain_modulus);
                                  });
   std::vector<const uint64_t* const*> dk;
   const uint64_t missing = keys_on_device(galois_keys, num_elts, pi.device, &dk);
@@ -864,10 +935,50 @@ int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const ui
     for (uint64_t c = 0; c < batch; ++c)
       if (int rc = hybrid_hoisted_on_device(pi.device, results + c * num_elts * 2 * comp, ciphertexts + c * 2 * comp, n,
                                             level, q_size, p_size, alpha, h, bmods.data(), dk.data(), galois_elts,
-                                            num_elts, (cudaStream_t)stream))
+                                            num_elts, (cudaStream_t)stream, plain_modulus))
         return rc;
     return 0;
   });
+}
+
+}  // namespace
+
+extern "C" {
+
+int hexl_b200_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
+                                uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
+                                const uint64_t* moduli, const hexl_b200_keys* keys, uint64_t batch, void* stream) {
+  return key_switch_hybrid_call(result, target, n, level_size, q_size, p_size, digit_size, key_component_count, moduli,
+                                keys, batch, stream, false, 0);
+}
+
+int hexl_b200_bgv_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
+                                    uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                    uint64_t key_component_count, const uint64_t* moduli, uint64_t plain_modulus,
+                                    const hexl_b200_keys* keys, uint64_t batch, void* stream) {
+  return key_switch_hybrid_call(result, target, n, level_size, q_size, p_size, digit_size, key_component_count, moduli,
+                                keys, batch, stream, true, plain_modulus);
+}
+
+int hexl_b200_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                                     uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                                     uint64_t digit_size, const uint64_t* moduli,
+                                                     const hexl_b200_keys* const* galois_keys,
+                                                     const uint64_t* galois_elts, uint64_t num_elts, uint64_t batch,
+                                                     void* stream) {
+  return hoisted_hybrid_call(results, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, galois_keys,
+                             galois_elts, num_elts, batch, stream, false, 0);
+}
+
+int hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                                         uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                                         uint64_t digit_size, const uint64_t* moduli,
+                                                         uint64_t plain_modulus,
+                                                         const hexl_b200_keys* const* galois_keys,
+                                                         const uint64_t* galois_elts, uint64_t num_elts,
+                                                         uint64_t batch, void* stream) {
+  return hoisted_hybrid_call(results, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, galois_keys,
+                             galois_elts, num_elts, batch, stream, true, plain_modulus);
 }
 
 int hexl_b200_linear_transform_hybrid(uint64_t* result, const uint64_t* ciphertexts, uint64_t n, uint64_t level_size,
@@ -1043,18 +1154,27 @@ int hexl_b200_linear_transform_hybrid_bsgs(uint64_t* result, const uint64_t* cip
   });
 }
 
-int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
-                                          uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
-                                          const uint64_t* moduli, const hexl_b200_keys* relin_keys, int rescale,
-                                          uint64_t batch, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// hexl_b200_multiply_relinearize_hybrid, and with bgv hexl_b200_bgv_multiply_relinearize_hybrid, whose merged mod-down
+// is the modulus switch (the messages name rescale mod_switch there)
+int multiply_relinearize_hybrid_call(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                     uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                     const uint64_t* moduli, const hexl_b200_keys* relin_keys, int rescale,
+                                     uint64_t batch, void* stream, bool bgv, uint64_t plain_modulus) {
   const uint64_t level = level_size, alpha = digit_size;
+  const char* flag = bgv ? "mod_switch" : "rescale";
   REQUIRE(result && ct1 && ct2 && moduli && relin_keys, "Require non-null arguments");
   if (int rc = hybrid_shape_check(n, level, q_size, p_size, alpha, 2, moduli)) return rc;
+  if (bgv)
+    if (int rc = bgv_plain_modulus_check(plain_modulus, moduli, q_size + p_size)) return rc;
   if (int rc = hybrid_handle_check(relin_keys, n, q_size, p_size, alpha, 2, "relin_keys")) return rc;
-  REQUIRE(rescale == 0 || rescale == 1, "Require rescale = 0 or 1");
+  REQUIRE(rescale == 0 || rescale == 1, "Require %s = 0 or 1", flag);
   // the merged rescale divides by q_{l-1} too: a level to drop, and K + 1 sources of one base conversion
-  REQUIRE(!rescale || level >= 2, "rescale = 1 requires level_size >= 2");
-  REQUIRE(!rescale || p_size < (uint64_t)kParamBlock, "rescale = 1 requires p_size <= %d", kParamBlock - 1);
+  REQUIRE(!rescale || level >= 2, "%s = 1 requires level_size >= 2", flag);
+  REQUIRE(!rescale || p_size < (uint64_t)kParamBlock, "%s = 1 requires p_size <= %d", flag, kParamBlock - 1);
   if (batch == 0) return 0;
   const uint64_t in_words = 2 * level * n, out_words = 2 * (level - rescale) * n;
   const uint64_t in_total = batch * in_words, out_total = batch * out_words;
@@ -1082,7 +1202,7 @@ int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1,
                                      cudaStream_t s) {
                                    return multiply_relinearize_hybrid_on_device(
                                        dev, d_res, d_in, square ? d_in : d_in + in_words, n, level, q_size, p_size,
-                                       alpha, rs, h, bmods.data(), dk[0], s);
+                                       alpha, rs, h, bmods.data(), dk[0], s, nullptr, plain_modulus);
                                  },
                                  nullptr, square ? nullptr : ct2);
   }
@@ -1093,10 +1213,32 @@ int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1,
     for (uint64_t c = 0; c < batch; ++c)
       if (int rc = multiply_relinearize_hybrid_on_device(pi.device, result + c * out_words, ct1 + c * in_words,
                                                          ct2 + c * in_words, n, level, q_size, p_size, alpha, rs, h,
-                                                         bmods.data(), dk[0], (cudaStream_t)stream))
+                                                         bmods.data(), dk[0], (cudaStream_t)stream, nullptr,
+                                                         plain_modulus))
         return rc;
     return 0;
   });
+}
+
+}  // namespace
+
+extern "C" {
+
+int hexl_b200_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                          uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                          const uint64_t* moduli, const hexl_b200_keys* relin_keys, int rescale,
+                                          uint64_t batch, void* stream) {
+  return multiply_relinearize_hybrid_call(result, ct1, ct2, n, level_size, q_size, p_size, digit_size, moduli,
+                                          relin_keys, rescale, batch, stream, false, 0);
+}
+
+int hexl_b200_bgv_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                              uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                              uint64_t digit_size, const uint64_t* moduli, uint64_t plain_modulus,
+                                              const hexl_b200_keys* relin_keys, int mod_switch, uint64_t batch,
+                                              void* stream) {
+  return multiply_relinearize_hybrid_call(result, ct1, ct2, n, level_size, q_size, p_size, digit_size, moduli,
+                                          relin_keys, mod_switch, batch, stream, true, plain_modulus);
 }
 
 int hexl_b200_multiply_relinearize_sum_hybrid(uint64_t* result, const uint64_t* const* ct1, const uint64_t* const* ct2,

@@ -431,6 +431,56 @@ static int divide_and_round_on_device(int dev, uint64_t* result, const uint64_t*
   return 0;  // ~Scratch returns the buffers to the pool in stream order
 }
 
+// BGV's modulus switch by the last modulus, same layout: limbs [0, rns - 1) of result get (x_i - delta) q_L^-1 mod q_i,
+// with delta = x_L + q_L [-x_L q_L^-1]_tau the t-corrected conversion of the last limb (T = {q_L}, one source).  Per
+// chunk of polynomials: in NTT form the last limbs are gathered and transformed back to coefficients (canonical); per
+// block of 64 moduli, one conversion launch reads every polynomial's last limb through its strides, delta is
+// transformed forward (NTT form only) and the finish stores, reading the operand laid out like the result (in place
+// works: limb rns - 1 is neither written nor read after the conversions of the chunk).
+static int bgv_mod_switch_on_device(int dev, uint64_t* result, const uint64_t* operand, uint64_t n,
+                                    const uint64_t* moduli, uint64_t rns, uint64_t count, bool ntt_form,
+                                    uint64_t plain_modulus, hexl_b200_ntt* const* h, cudaStream_t s) {
+  const uint64_t L = rns - 1, q_last = moduli[L];
+  const uint64_t block = std::min<uint64_t>(L, kParamBlock);
+  uint64_t chunk = std::max<uint64_t>(1, (256ull << 20) / ((block + 1) * n * 8));
+  chunk = std::min(chunk, count);
+  Scratch ws(s);
+  uint64_t *t_last = nullptr, *tmp = nullptr;
+  if (ntt_form)
+    if (int rc = ws.get(&t_last, chunk * n)) return rc;    // [p][n]
+  if (int rc = ws.get(&tmp, block * chunk * n)) return rc;  // [e][p][n]
+  for (uint64_t p0 = 0; p0 < count; p0 += chunk) {
+    const uint64_t cnt = std::min(chunk, count - p0);
+    const uint64_t* op = operand + p0 * rns * n;
+    const uint64_t* last = op + L * n;
+    uint64_t last_poly = rns * n;
+    if (ntt_form) {
+      CU(cudaMemcpy2DAsync(t_last, n * 8, last, rns * n * 8, n * 8, cnt, cudaMemcpyDeviceToDevice, s));
+      if (int rc = ntt_multi_on_device(false, dev, h + L, 1, t_last, t_last, 1, cnt, s)) return rc;
+      last = t_last;
+      last_poly = n;
+    }
+    for (uint64_t i0 = 0; i0 < L; i0 += kParamBlock) {
+      const uint64_t cm = std::min<uint64_t>(kParamBlock, L - i0);
+      if (int rc = base_convert_on_device(tmp, cnt * n, n, last, n, last_poly, n, cnt, &q_last, 1, moduli + i0, cm,
+                                          false, s, plain_modulus))
+        return rc;
+      if (ntt_form)
+        if (int rc = ntt_multi_on_device(true, dev, h + i0, cm, tmp, tmp, 4, cnt, s)) return rc;
+      KsModuli fin;
+      for (uint64_t e = 0; e < cm; ++e) {
+        const uint64_t qi = moduli[i0 + e];
+        const Twiddle f = make_twiddle(nt::inverse_mod(q_last % qi, qi), qi);
+        fin.m[e] = KsModulus{qi, nt::multiply_factor(1, 64, qi), f.w, f.wp, 0};
+      }
+      const cudaError_t e =
+          launch_ks_finish(result + p0 * rns * n, op, tmp, n, cnt, rns, i0, cm, fin, true, false, s);
+      if (e != cudaSuccess) return cuda_fail(e, "BgvModSwitch: finish launch");
+    }
+  }
+  return 0;  // ~Scratch returns the buffers to the pool in stream order
+}
+
 // The caller may have written device (or managed) key sources on any stream of their device, and the upload's copies
 // run on the legacy default stream, which does not wait for non-blocking streams: wait for every device that owns a
 // source before copying from it.
@@ -653,8 +703,13 @@ int hexl_b200_key_switch(uint64_t* result, const uint64_t* t_target_iter_ptr, ui
   return rc;
 }
 
-int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
-                                      uint64_t rns_modulus_size, uint64_t count, int ntt_form, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// hexl_b200_divide_and_round_q_last (plain_modulus = 0) and hexl_b200_bgv_mod_switch (plain_modulus checked)
+int last_modulus_call(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                      uint64_t rns_modulus_size, uint64_t count, int ntt_form, void* stream, uint64_t plain_modulus) {
   REQUIRE(result && operand && moduli, "Require result, operand, moduli != nullptr");
   REQUIRE(rns_modulus_size >= 2, "Require rns_modulus_size >= 2");
   REQUIRE(ntt_form == 0 || ntt_form == 1, "Require ntt_form = 0 or 1");
@@ -685,18 +740,36 @@ int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand,
     if (int rc = h.load(i, n, moduli[i])) return rc;
   if (int rc = check_limb_bounds(operand, count, rns, n, [&](u64 i) { return moduli[i]; }, pi, "operand", stream)) return rc;
   const bool ntt = ntt_form != 0;
+  auto on_device = [&](int dev, uint64_t* r, const uint64_t* a, uint64_t polys, cudaStream_t s) {
+    return plain_modulus ? bgv_mod_switch_on_device(dev, r, a, n, moduli, rns, polys, ntt, plain_modulus, h.data(), s)
+                         : divide_and_round_on_device(dev, r, a, n, moduli, rns, polys, ntt, h.data(), s);
+  };
   if (pi.where == Where::Device)
-    return run_on_device(pi, stream, [&] {
-      return divide_and_round_on_device(pi.device, result, operand, n, moduli, rns, count, ntt, h.data(),
-                                        (cudaStream_t)stream);
-    });
+    return run_on_device(pi, stream, [&] { return on_device(pi.device, result, operand, count, (cudaStream_t)stream); });
   // host pointers: whole polynomials through the staging slots (split over the host devices when set); only limbs
   // [0, L) of each polynomial are copied back, so limb L of result is left as it was
   return run_host(result, operand, nullptr, total, unit, [&](int dev, u64, u64, auto&& run) {
     return run([&, dev](u64* r, const u64* a, const u64*, u64, u64 elems, cudaStream_t s) {
-      return divide_and_round_on_device(dev, r, a, n, moduli, rns, elems / unit, ntt, h.data(), s);
+      return on_device(dev, r, a, elems / unit, s);
     });
   }, L * n);
+}
+
+}  // namespace
+
+extern "C" {
+
+int hexl_b200_divide_and_round_q_last(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                                      uint64_t rns_modulus_size, uint64_t count, int ntt_form, void* stream) {
+  return last_modulus_call(result, operand, n, moduli, rns_modulus_size, count, ntt_form, stream, 0);
+}
+
+int hexl_b200_bgv_mod_switch(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                             uint64_t rns_modulus_size, uint64_t plain_modulus, uint64_t count, int ntt_form,
+                             void* stream) {
+  REQUIRE(moduli, "Require result, operand, moduli != nullptr");
+  if (int rc = bgv_plain_modulus_check(plain_modulus, moduli, rns_modulus_size)) return rc;
+  return last_modulus_call(result, operand, n, moduli, rns_modulus_size, count, ntt_form, stream, plain_modulus);
 }
 
 }  // extern "C"

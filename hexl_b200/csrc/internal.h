@@ -188,6 +188,19 @@ struct BaseConvTable {
 inline u64 base_conv_targets(u64 from) { return (kBaseConvWords - 4 * from) / (5 + from); }
 cudaError_t launch_base_conv(u64* result, u64 res_limb, u64 res_poly, const u64* operand, u64 op_limb, u64 op_poly,
                              u64 n, u64 polys, u64 from, u64 to, const BaseConvTable& tab, cudaStream_t stream);
+// The t-corrected conversion (BGV's mod-down by P_T = Q, tau the plain modulus), same strides and result layout:
+//   y_i = [x_i (P_T/q_i)^-1]_{q_i},  X~_m = [sum_i y_i [P_T/q_i]_m]_m,  k = [-X~_tau P_T^-1]_tau,
+//   result_e = [X~_e + [P_T]_{t_e} k]_{t_e},  canonical,
+// the residues of delta = X~ + P_T k: delta = x mod P_T, delta = 0 mod tau, 0 <= delta < P_T (from + tau - 1).  Table:
+//   per source i (3 words):  q_i, (P_T/q_i)^-1 mod q_i, its Shoup factor
+//   tau (6 + from words):    tau, floor(2^64 / tau), 2^64 mod tau, its Shoup factor, [-P_T^-1]_tau, its Shoup factor,
+//                            then [P_T/q_i]_tau for every source i
+//   per target e (6 words):  t_e, floor(2^64 / t_e), 2^64 mod t_e, its Shoup factor, [P_T]_{t_e}, its Shoup factor
+//   per target e (from words): [P_T/q_i]_{t_e} for every source i
+// so one launch takes at most base_conv_t_targets(from) targets: 67 for one source, 27 for 10, 3 for 64.
+inline u64 base_conv_t_targets(u64 from) { return (kBaseConvWords - 4 * from - 6) / (6 + from); }
+cudaError_t launch_base_conv_t(u64* result, u64 res_limb, u64 res_poly, const u64* operand, u64 op_limb, u64 op_poly,
+                               u64 n, u64 polys, u64 from, u64 to, const BaseConvTable& tab, cudaStream_t stream);
 
 // BFV multiplication by BEHZ (bfv.cu), coefficient form, every modulus below 2^61, l = |Q| and k = |B| in [1, 64].
 // The constants are too many for the kernel parameters (l = k = 64 takes ~9000 words), so they live in a device table

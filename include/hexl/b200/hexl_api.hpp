@@ -877,6 +877,53 @@ inline void BfvMultiplyRelinearizeHybrid(uint64_t* result, const uint64_t* ct1, 
                                                                digit_size, moduli, base_b, base_b_size, m_sk,
                                                                plain_modulus, relin_keys.Handle(), batch, stream));
 }
+
+// extension: BGV modulus switch by the last modulus, SEAL's RNSTool::mod_t_and_divide_q_last(_ntt)_inplace batched over
+// `count` polynomials of rns_modulus_size limbs each: DivideAndRoundQLast's layout and rules with the rounding replaced
+// by the correction delta = 0 mod plain_modulus (hexl_b200_bgv_mod_switch).  The message picks up [q_L^-1]_t.
+inline void BgvModSwitch(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                         uint64_t rns_modulus_size, uint64_t plain_modulus, uint64_t count, bool ntt_form,
+                         void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bgv_mod_switch(result, operand, n, moduli, rns_modulus_size, plain_modulus, count,
+                                              ntt_form ? 1 : 0, stream));
+}
+
+// extension: KeySwitchHybrid for BGV -- the mod-down by P subtracts a correction that is 0 mod plain_modulus
+// (hexl_b200_bgv_key_switch_hybrid).  result is accumulated into.
+inline void BgvKeySwitchHybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
+                               uint64_t q_size, uint64_t p_size, uint64_t digit_size, uint64_t key_component_count,
+                               const uint64_t* moduli, uint64_t plain_modulus, const KeySwitchKeys& keys,
+                               uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bgv_key_switch_hybrid(result, target, n, level_size, q_size, p_size, digit_size,
+                                                     key_component_count, moduli, plain_modulus, keys.Handle(), batch,
+                                                     stream));
+}
+
+// extension: ApplyGaloisKeySwitchHybridHoisted for BGV (hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted)
+inline void BgvApplyGaloisKeySwitchHybridHoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                                 uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                                 uint64_t digit_size, const uint64_t* moduli, uint64_t plain_modulus,
+                                                 const KeySwitchKeys* const* galois_keys, const uint64_t* galois_elts,
+                                                 uint64_t num_elts, uint64_t batch = 1, void* stream = nullptr) {
+  std::vector<const hexl_b200_keys*> handles(num_elts);
+  for (uint64_t r = 0; r < num_elts; ++r) handles[r] = galois_keys[r] ? galois_keys[r]->Handle() : nullptr;
+  b200_detail::Throw(hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted(
+      results, ciphertexts, n, level_size, q_size, p_size, digit_size, moduli, plain_modulus, handles.data(),
+      galois_elts, num_elts, batch, stream));
+}
+
+// extension: MultiplyRelinearizeHybrid for BGV, mod_switch = 1 dropping q_{level_size-1} in the same t-corrected
+// mod-down as P (hexl_b200_bgv_multiply_relinearize_hybrid).  mod_switch = 0 equals DyadicMultiply followed by
+// BgvKeySwitchHybrid bit for bit.  ct1 == ct2 squares.
+inline void BgvMultiplyRelinearizeHybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                         uint64_t level_size, uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                         const uint64_t* moduli, uint64_t plain_modulus,
+                                         const KeySwitchKeys& relin_keys, bool mod_switch, uint64_t batch = 1,
+                                         void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bgv_multiply_relinearize_hybrid(result, ct1, ct2, n, level_size, q_size, p_size,
+                                                               digit_size, moduli, plain_modulus, relin_keys.Handle(),
+                                                               mod_switch ? 1 : 0, batch, stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

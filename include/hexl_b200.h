@@ -744,6 +744,87 @@ int hexl_b200_bfv_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* 
                                               uint64_t base_b_size, uint64_t m_sk, uint64_t plain_modulus,
                                               const hexl_b200_keys* relin_keys, uint64_t batch, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------- BGV
+ * BGV keeps the message mod the plain modulus tau = plain_modulus (SEAL's t) in the low part of the phase, so every
+ * division by a modulus product P_T must subtract a correction delta with delta = 0 (mod tau); the rounded correction of
+ * the CKKS calls is not, and its error, not a multiple of tau, destroys the message.  The calls below replace it by the
+ * t-corrected mod-down.  T is the set of moduli dropped, P_T = prod T, and x_t (t in T) the T-limbs in coefficient form,
+ * canonical (an inverse transform of them in NTT form):
+ *   y_t   = [x_t (P_T/t)^-1]_t                                                   (no rounding offset)
+ *   X~_m  = [ sum_t y_t [P_T/t]_m ]_m   for m in {q_i : i < l'} and m = tau       (one integer X~ = X + u P_T, 0 <= u < |T|)
+ *   k     = [ -X~_tau P_T^-1 ]_tau
+ *   delta_i = [ X~_i + [P_T]_{q_i} k ]_{q_i}
+ *   out_i = (ext_i - NTT_{q_i}(delta_i)) P_T^-1 mod q_i  (NTT form)   or   (ext_i - delta_i) P_T^-1 mod q_i  (coefficients)
+ * The integer delta = X~ + P_T k satisfies delta = X (mod P_T), delta = 0 (mod tau) and 0 <= delta < P_T (|T| + tau - 1),
+ * so out is exactly (X_ext - delta) / P_T, and the message mod tau is multiplied by [P_T^-1]_tau.  With T one prime p the
+ * conversion returns x itself (u = 0): k = [-x p^-1]_tau and delta = x + p k, SEAL's formula
+ * (RNSTool::mod_t_and_divide_q_last_ntt_inplace and the BGV branch of Evaluator::switch_key_inplace), so digit_size = 1
+ * with one special prime is SEAL's BGV relinearization and rotation bit for bit.  OpenFHE's BGV takes
+ * delta = tau FBC([x tau^-1]_P) instead: its results differ from these bit for bit, with the same noise bound.
+ * Exactness, for every modulus below 2^61, every tau in [2, 2^61) and |T| <= 64: each sum of |T| products
+ * y_t [P_T/t]_m < (2^61 - 1)^2 is below 64 (2^61 - 1)^2 < 2^128 and is reduced once; k [P_T]_{q_i} is added after that
+ * reduction (a Shoup product, exact for any 64-bit k, and one conditional subtraction), never as a 65th term of the
+ * 128-bit sum, which could then exceed 2^128.  The constants travel in the kernel parameters: one conversion launch
+ * takes at most floor((474 - 4 |T|) / (6 + |T|)) targets (67 for |T| = 1, 27 for 10, 3 for 64), where the rounded
+ * conversion of the CKKS calls takes floor((480 - 4 |T|) / (5 + |T|)); device calls capture into CUDA graphs.
+ * Every BGV call refuses (HEXL_B200_ERR_INVALID_ARG) plain_modulus outside [2, 2^61) and plain_modulus sharing a factor
+ * with any modulus it is given, on top of the refusals of its CKKS counterpart.  The caller tracks the correction
+ * factor [P_T^-1]_tau, as SEAL does.  Not covered: BGV forms of the linear transforms, the inner sum and the lazy
+ * relinearization, the SEAL-shaped KeySwitch, sharded key handles (refused), key generation, encoding, encryption and
+ * decryption. */
+
+/* BGV modulus switch by the last modulus (extension; SEAL's RNSTool::mod_t_and_divide_q_last_inplace and
+ * mod_t_and_divide_q_last_ntt_inplace, OpenFHE's BGV ModReduce): the layout, forms, in-place rule and refusals of
+ * hexl_b200_divide_and_round_q_last, with the rounding replaced by the t-correction of T = {q_L}: limbs 0..L-1 of every
+ * polynomial get (X - delta) / q_L mod q_i, canonical, delta = x_L + q_L [-x_L q_L^-1]_tau with x_L the last limb in
+ * coefficient form; limb L is not written.  The message mod tau is multiplied by [q_L^-1]_tau.  In NTT form this is bit
+ * for bit the inverse transform, the coefficient-form call and the forward transform.  On the device, per chunk of
+ * polynomials (~256 MiB of scratch): in NTT form one gathering copy and one inverse transform of the last limbs; then per
+ * block of 64 moduli one conversion launch, in NTT form one forward transform of delta, and one finish launch. */
+int hexl_b200_bgv_mod_switch(uint64_t* result, const uint64_t* operand, uint64_t n, const uint64_t* moduli,
+                             uint64_t rns_modulus_size, uint64_t plain_modulus, uint64_t count, int ntt_form,
+                             void* stream);
+
+/* BGV hybrid key switch (extension; SEAL's Evaluator::switch_key_inplace for BGV with OpenFHE's hybrid digits): the
+ * arguments, layouts, definitions and launches of hexl_b200_key_switch_hybrid, with ModDown_P the t-corrected mod-down
+ * (T = {p_0..p_{K-1}}) in place of the rounded one; its conversion launches are per block of base_conv_t targets.  It
+ * is BGV's relinearization of a three-component ciphertext (d2 into (d0, d1), key_component_count = 2) and, after
+ * hexl_b200_apply_galois, the non-hoisted rotation.  Refusals: those of hexl_b200_key_switch_hybrid and the BGV ones. */
+int hexl_b200_bgv_key_switch_hybrid(uint64_t* result, const uint64_t* target, uint64_t n, uint64_t level_size,
+                                    uint64_t q_size, uint64_t p_size, uint64_t digit_size,
+                                    uint64_t key_component_count, const uint64_t* moduli, uint64_t plain_modulus,
+                                    const hexl_b200_keys* keys, uint64_t batch, void* stream);
+
+/* BGV hoisted rotations with hybrid keys (extension; SEAL's rotate_rows / rotate_columns for several elements with one
+ * mod-up): hexl_b200_apply_galois_key_switch_hybrid_hoisted with the t-corrected ModDown_P:
+ *   out_r = [sigma_g(c0), 0] + ModDown^tau_P(prod^r).
+ * For g = 1 it is hexl_b200_bgv_key_switch_hybrid of c1 into (c0, 0) bit for bit.  Arguments, layouts, launches,
+ * scratch, host staging and refusals as for the CKKS call, plus the BGV refusals. */
+int hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted(uint64_t* results, const uint64_t* ciphertexts, uint64_t n,
+                                                         uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                                         uint64_t digit_size, const uint64_t* moduli,
+                                                         uint64_t plain_modulus,
+                                                         const hexl_b200_keys* const* galois_keys,
+                                                         const uint64_t* galois_elts, uint64_t num_elts,
+                                                         uint64_t batch, void* stream);
+
+/* BGV ciphertext multiplication with relinearization by hybrid keys (extension; SEAL's multiply + relinearize
+ * [+ mod_switch_to_next] for BGV), optionally modulus-switched in the same mod-down: hexl_b200_multiply_relinearize_hybrid
+ * with the t-corrected mod-down, mod_switch in the place of rescale.  With the tensor d, prod and ext of that call:
+ *   T = {p_0..p_{K-1}} (mod_switch = 0) or {q_{l-1}, p_0..p_{K-1}} (mod_switch = 1),  result = ModDown^tau_T(ext), stored,
+ * l' = l - mod_switch limbs.  mod_switch = 0 is bit for bit hexl_b200_dyadic_multiply followed by
+ * hexl_b200_bgv_key_switch_hybrid of d2 into (d0, d1) (delta depends only on the limbs of T, where ext = prod, and
+ * (prod + P d - delta) P^-1 = (prod - delta) P^-1 + d).  mod_switch = 1 drops q_{l-1} in the same mod-down as P, with one
+ * t-correction instead of the two of that chain followed by hexl_b200_bgv_mod_switch, so it is NOT the chain bit for bit;
+ * the message picks up [(q_{l-1})^-1]_tau and the key switch's error is divided by q_{l-1}.  Launches, scratch, host
+ * staging and squaring as for the CKKS call; refusals as for it (mod_switch other than 0 or 1, mod_switch = 1 with
+ * level_size < 2 or p_size > 63) plus the BGV ones. */
+int hexl_b200_bgv_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* ct1, const uint64_t* ct2, uint64_t n,
+                                              uint64_t level_size, uint64_t q_size, uint64_t p_size,
+                                              uint64_t digit_size, const uint64_t* moduli, uint64_t plain_modulus,
+                                              const hexl_b200_keys* relin_keys, int mod_switch, uint64_t batch,
+                                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif
