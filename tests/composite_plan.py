@@ -1,6 +1,6 @@
-"""The scratch rounds of the RNS composites (hexl_b200/csrc/capi_keyswitch.cu, capi_galois.cu, capi_hybrid.cu) restated
-in Python, and the shapes of tests/test_gpu_composite_rounds.py, tests/test_gpu_hybrid_rounds.py and
-tests/test_gpu_bsgs_rounds.py.
+"""The scratch rounds of the RNS composites (hexl_b200/csrc/capi_keyswitch.cu, capi_galois.cu, capi_hybrid.cu,
+capi_bfv.cu) restated in Python, and the shapes of tests/test_gpu_composite_rounds.py, tests/test_gpu_hybrid_rounds.py,
+tests/test_gpu_bsgs_rounds.py and tests/test_gpu_evaluator_rounds.py.
 
 Each composite splits one device call into rounds that fit about 256 MiB of pool scratch:
 
@@ -22,6 +22,16 @@ MultiplyRelinearizeHybrid) around one mod-up and one mod-down:
     bsgs_launches           the same for LinearTransformHybridBSGS: a baby mod-up, per row the sums, per keyed giant
                             a one-component mod-down and a mod-up, and the final mod-down (bsgs_rows: what it runs)
 
+and the evaluator calls built on them (tests/test_gpu_evaluator_rounds.py):
+
+    base_conv_t_blocks      BGV's t-corrected conversion: base_conv_t_targets of the source count per launch; the tau
+                            option of hybrid_mod_down_blocks / _launches and hybrid_launches uses it
+    bgv_mod_switch_rounds   BgvModSwitch: polynomials per chunk, in both forms (bgv_mod_switch_launches)
+    relin_sum_launches      MultiplyRelinearizeSumHybrid's tensor sums (hybrid_launches "mul_relin_sum")
+    bfv_launches            the BEHZ product of BfvMultiply; hybrid_launches "bfv_relin" adds the switch of d2 in
+                            coefficient form (the coef option of hybrid_mod_up_launches / hybrid_mod_down_launches)
+    inner_sum_exact.inner_sum_launches restates InnerSumHybrid from these primitives; its host lines are pinned here.
+
 Every function returns the list of round (or launch) sizes.  SOURCE holds the source file under hexl_b200/csrc and the
 lines of it each formula restates;
 tests/test_composite_plan.py asserts they are still there, so a change of the budget or of a formula fails on the CPU
@@ -31,6 +41,8 @@ from __future__ import annotations
 
 PARAM_BLOCK = 64          # internal.h: kParamBlock, moduli per kernel parameter block
 SCRATCH_BYTES = 256 << 20
+RELIN_SUM_PAIRS = 32      # hybrid_rotation.h: kRelinSumPairs, pairs per tensor-sum launch
+STAGING_SLOTS = 3         # capi.h: kSlots, the rotating staging slots of a device
 
 SOURCE = {
     "rescale": ("capi_keyswitch.cu",
@@ -77,6 +89,94 @@ SOURCE = {
                       "const uint64_t per = std::max<uint64_t>(1, kParamBlock / jc);",
                       "for (uint64_t j0 = 0; j0 < D; j0 += jc) {",
                       "for (uint64_t k0 = 0; k0 < keyed.size(); k0 += per) {"]),
+    # BGV: the t-corrected conversion's table holds 4 words per source, 6 for tau and 6 + F per target
+    "base_conv_t_targets": ("internal.h",
+                            ["inline u64 base_conv_t_targets(u64 from) "
+                             "{ return (kBaseConvWords - 4 * from - 6) / (6 + from); }"]),
+    "base_conv_t_blocks": ("capi_hybrid.cu",
+                           ["const uint64_t tau = plain_modulus, tblock = base_conv_t_targets(F);",
+                            "for (uint64_t e0 = 0; e0 < to_count; e0 += tblock) {\n"
+                            "      const uint64_t cnt = std::min(tblock, to_count - e0);"]),
+    "bgv_mod_down": ("capi_hybrid.cu",
+                     ["hybrid_mod_down(dev, results[r], prod + r * nb * kcc * n, tmp, n, level, p_size, kcc, h, bmods, "
+                      "true, s,\n                            false, plain_modulus))",
+                      "if (plain_modulus)  // BGV: the t-corrected mod-down by P, or by q_{level-1} P (the merged "
+                      "modulus switch)\n    return hybrid_mod_down(dev, result, prod, tmp, n, level - rescale, "
+                      "p_size + rescale, 2, h, bmods, false, s, false,\n                           plain_modulus);"]),
+    # BgvModSwitch: one multi-line pin per step, each unique in the file (DivideAndRoundQLast shares single lines)
+    "bgv_mod_switch": ("capi_keyswitch.cu",
+                       ["const uint64_t L = rns - 1, q_last = moduli[L];\n"
+                        "  const uint64_t block = std::min<uint64_t>(L, kParamBlock);\n"
+                        "  uint64_t chunk = std::max<uint64_t>(1, (256ull << 20) / ((block + 1) * n * 8));\n"
+                        "  chunk = std::min(chunk, count);",
+                        "if (ntt_form) {\n"
+                        "      CU(cudaMemcpy2DAsync(t_last, n * 8, last, rns * n * 8, n * 8, cnt, cudaMemcpyDeviceToDevice,"
+                        " s));\n"
+                        "      if (int rc = ntt_multi_on_device(false, dev, h + L, 1, t_last, t_last, 1, cnt, s)) return rc;",
+                        "for (uint64_t i0 = 0; i0 < L; i0 += kParamBlock) {\n"
+                        "      const uint64_t cm = std::min<uint64_t>(kParamBlock, L - i0);\n"
+                        "      if (int rc = base_convert_on_device(tmp, cnt * n, n, last, n, last_poly, n, cnt, &q_last, 1,"
+                        " moduli + i0, cm,\n"
+                        "                                          false, s, plain_modulus))\n"
+                        "        return rc;\n"
+                        "      if (ntt_form)\n"
+                        "        if (int rc = ntt_multi_on_device(true, dev, h + i0, cm, tmp, tmp, 4, cnt, s)) return rc;",
+                        "launch_ks_finish(result + p0 * rns * n, op, tmp, n, cnt, rns, i0, cm, fin, true, false, s);"]),
+    "mul_relin_sum": ("capi_hybrid.cu",
+                      ["if (pairs == 1)\n    return multiply_relinearize_hybrid_on_device(",
+                       "for (uint64_t i0 = 0; i0 < level; i0 += kParamBlock) {\n"
+                       "    const uint64_t cnt = std::min<uint64_t>(kParamBlock, level - i0);\n"
+                       "    const KsModuli mods = ks_mac_moduli(bmods + i0, nullptr, cnt);\n"
+                       "    for (uint64_t r0 = 0; r0 < pairs; r0 += kRelinSumPairs) {\n"
+                       "      const uint64_t rcnt = std::min<uint64_t>(kRelinSumPairs, pairs - r0);"]),
+    "relin_sum_pairs": ("hybrid_rotation.h", [f"constexpr int kRelinSumPairs = {RELIN_SUM_PAIRS};"]),
+    # the host-buffer switches stage one ciphertext per slot, the slots rotating
+    "staging_slots": ("capi.h", [f"constexpr int kSlots = {STAGING_SLOTS};",
+                                 "for (u64 first = lo; first < hi; first += per_chunk, slot = (slot + 1) % kSlots)"]),
+    "host_switch_chunk": ("capi_keyswitch.cu", ["return stage_items(use, batch, 1, [&](int dev, u64, u64, auto&& stage) {"]),
+    "bfv": ("capi_bfv.cu",
+            ["const uint64_t inputs = square ? 2 : 4;",
+             "cudaError_t e = launch_bfv_extend(ext, poly, ct1, comp, n, 2, l, k, ext_tab, s);\n"
+             "  if (e == cudaSuccess && !square) e = launch_bfv_extend(",
+             "for (uint64_t p = 0; p < inputs; ++p) hs.insert(hs.end(), pl.h.data(), pl.h.data() + M);\n"
+             "  if (int rc = ntt_multi_on_device(true, dev, hs.data(), inputs * M, ext, ext, 1, 1, s)) return rc;\n"
+             "  for (uint64_t first = 0; first < M; first += kParamBlock) {",
+             "for (uint64_t p = 0; p < 3; ++p) hs.insert(hs.end(), pl.h.data(), pl.h.data() + M);\n"
+             "  if (int rc = ntt_multi_on_device(false, dev, hs.data(), 3 * M, tensor, tensor, 1, 1, s)) return rc;\n"
+             "  e = launch_bfv_scale(out, tensor, poly, n, 3, l, k, scale_tab, s);"]),
+    # one launch_ntt_multi per block of 64 handles: the BFV transforms' handles run one polynomial each
+    "ntt_multi_blocks": ("capi_ntt.cu",
+                         ["for (uint64_t first = 0; first < count; first += kParamBlock) {\n"
+                          "    const uint64_t cnt = std::min<uint64_t>(kParamBlock, count - first);\n"
+                          "    NttMulti multi{};"]),
+    "bfv_relin": ("capi_hybrid.cu",
+                  ["if (!coef)\n    if (int rc = ws.get(&t_coef, level * n)) return rc;",
+                   "if (!coef)\n    if (int rc = ntt_multi_on_device(false, dev, h.data(), level, t_coef, target, 1, 1, s, "
+                   "nullptr, false, mul))",
+                   "if (coef) {\n      uint64_t* data = prod + i0 * kcc * n;\n"
+                   "      if (int rc = ntt_multi_on_device(false, dev, h.data() + i0, cnt, data, data, 1, kcc, s)) "
+                   "return rc;\n"
+                   "    } else if (int rc = ntt_multi_on_device(true, dev, h.data() + i0, cnt, tmp, tmp, 4, kcc, s)) {",
+                   "if (int rc = bfv_product_on_device(dev, plan, BfvOutputs{{result, result + comp, d2}}, ct1, ct2, s)) "
+                   "return rc;\n  if (int rc = hybrid_mod_up(dev, d2, n, level, q_size, p_size, alpha, h, bmods, ws,",
+                   "prod + b0 * 2 * n, nb * 2 * n, &keys, nullptr, 1, s);\n"
+                   "                             },\n"
+                   "                             s, nullptr, true))\n"
+                   "    return rc;\n"
+                   "  return hybrid_mod_down(dev, result, prod, tmp, n, level, p_size, 2, h, bmods, true, s, true);"]),
+    # restated by inner_sum_exact.inner_sum_launches
+    "inner_sum": ("capi_hybrid.cu",
+                  ["const uint64_t span = (mode & (kSumNextY | kSumRYWrite | kSumCopy1)) ? nb : level;\n"
+                   "    for (uint64_t b0 = 0; b0 < span; b0 += kParamBlock) {",
+                   "if (d_keyed || s_keyed) {\n      const uint64_t* c1 = xa + comp;\n      if (y_a) {\n"
+                   "        if (int rc = hybrid_mod_down(dev, xa_own + comp, y1, tmp, n, level, p_size, 1, h, bmods, "
+                   "true, s)) return rc;",
+                   "uint64_t* prod = d_keyed ? yn : yr;",
+                   "const uint64_t pstride = (uint64_t)(yr - yn);",
+                   "prod + b0 * 2 * n, pstride, keys, elts, count, s, true);",
+                   "if (rescale) return hybrid_mod_down(dev, result, yr, tmp, n, level - 1, p_size + 1, 2, h, bmods, "
+                   "false, s);\n  if (!y_r) return 0;\n"
+                   "  return hybrid_mod_down(dev, result, yr, tmp, n, level, p_size, 2, h, bmods, true, s);"]),
     "bsgs": ("capi_hybrid.cu",
              ["if (!baby_keys[i]) continue;",                                         # stored: a keyed baby ...
               "if (diag[j * n1 + i]) {\n        stored[i] = used_keys.size();",       # ... with a diagonal
@@ -141,6 +241,17 @@ def base_conv_blocks(from_count, to_count):
     return _split(to_count, base_conv_targets(from_count))
 
 
+def base_conv_t_targets(from_count):
+    """targets one t-corrected conversion launch takes (BGV): 4 words per source, 6 for tau, 6 + from_count per
+    target"""
+    return (BASE_CONV_WORDS - 4 * from_count - 6) // (6 + from_count)
+
+
+def base_conv_t_blocks(from_count, to_count):
+    """the targets of each t-corrected launch of base_convert_on_device"""
+    return _split(to_count, base_conv_t_targets(from_count))
+
+
 def hybrid_digit_widths(level, alpha):
     """the moduli of each digit at `level`: alpha each, the last one partial"""
     return [min(alpha, level - lo) for lo in range(0, level, alpha)]
@@ -160,11 +271,12 @@ def hybrid_round_slots(level, q_size, b0, cnt):
     return [b if b < level else q_size + (b - level) for b in range(b0, b0 + cnt)]
 
 
-def hybrid_mod_down_blocks(level, K, rescale=False):
+def hybrid_mod_down_blocks(level, K, rescale=False, tau=False):
     """hybrid_mod_down: per block of 64 data moduli, the targets of each base-conversion launch, from K special limbs,
-    or K + 1 with the merged rescale (q_{level-1} joins P and leaves the targets)"""
+    or K + 1 with the merged rescale (q_{level-1} joins P and leaves the targets); tau: BGV's t-corrected conversion"""
     targets, sources = level - int(rescale), K + int(rescale)
-    return [base_conv_blocks(sources, cnt) for cnt in _split(targets, PARAM_BLOCK)]
+    blocks = base_conv_t_blocks if tau else base_conv_blocks
+    return [blocks(sources, cnt) for cnt in _split(targets, PARAM_BLOCK)]
 
 
 def relin_tensor_data(level, b0, cnt):
@@ -185,12 +297,12 @@ def weighted_mac_launches(D, keyed, largest_q):
     return [(j, e) for j in _split(D, jc) for e in _split(keyed, per)]
 
 
-def hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs):
-    """hybrid_mod_up: the target's inverse transform, then per round one base conversion per digit and block of
-    targets, the forward transform of the round's digits and macs(D, largest) multiply-accumulate launches, largest the
-    round's largest modulus"""
+def hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs, coef=False):
+    """hybrid_mod_up: the target's inverse transform (none with coef: the target is already in coefficient form), then
+    per round one base conversion per digit and block of targets, the forward transform of the round's digits and
+    macs(D, largest) multiply-accumulate launches, largest the round's largest modulus"""
     D = -(-level // alpha)
-    total = sum(ntt(False, cnt) for cnt in _split(level, PARAM_BLOCK))    # the target back to coefficients
+    total = 0 if coef else sum(ntt(False, cnt) for cnt in _split(level, PARAM_BLOCK))  # the target to coefficients
     b0 = 0
     for cnt in hybrid_mod_up_rounds(n, level, K, alpha):
         total += sum(len(base_conv_blocks(w, cnt)) for w in hybrid_digit_widths(level, alpha))
@@ -199,21 +311,51 @@ def hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs):
     return total
 
 
-def hybrid_mod_down_launches(level, K, kcc, ntt, rescale=False):
+def hybrid_mod_down_launches(level, K, kcc, ntt, rescale=False, tau=False, coef=False):
     """hybrid_mod_down of kcc components: the special limbs' inverse transform, then per block of 64 data moduli the
-    rounding base conversions, a forward transform and the finish; with the merged rescale q_{level-1} joins P"""
+    rounding (tau: t-corrected) base conversions, a forward transform of the correction (coef: an inverse transform of
+    the products' data limbs instead) and the finish; with the merged rescale q_{level-1} joins P"""
     total = ntt(False, (K + int(rescale)) * kcc)
-    for cnt, blocks in zip(_split(level - int(rescale), PARAM_BLOCK), hybrid_mod_down_blocks(level, K, rescale)):
-        total += len(blocks) + ntt(True, cnt * kcc) + 1
+    for cnt, blocks in zip(_split(level - int(rescale), PARAM_BLOCK), hybrid_mod_down_blocks(level, K, rescale, tau)):
+        total += len(blocks) + ntt(not coef, cnt * kcc) + 1
     return total
 
 
-def hybrid_launches(call, n, level, K, alpha, basis, ntt, elts=1, keyed=None, rescale=False, kcc=2):
-    """kernel launches of one ciphertext of `call` ("switch", "hoisted", "linear", "mul_relin"): basis holds the moduli
-    of B (level data, then K special); ntt(forward, units) is the launch count of one multi-modulus transform of
-    `units` polynomials.  "switch" and "hoisted" run `elts` switches over one mod-up; "linear" takes `elts` elements,
-    `keyed` of them with keys."""
+def relin_sum_launches(level, pairs):
+    """MultiplyRelinearizeSumHybrid's tensor sums: none for one pair (it is MultiplyRelinearizeHybrid), else one launch
+    per block of 64 data limbs and chunk of RELIN_SUM_PAIRS pairs"""
+    return 0 if pairs == 1 else -(-level // PARAM_BLOCK) * -(-pairs // RELIN_SUM_PAIRS)
+
+
+def ntt_handles(ntt, forward, handles):
+    """one transform of `handles` polynomials under a handle each (group 1): one multi-modulus launch set per block of
+    64 handles, each block its own unit count"""
+    return sum(ntt(forward, cnt) for cnt in _split(handles, PARAM_BLOCK))
+
+
+def bfv_launches(M, square, ntt):
+    """bfv_product_on_device of one pair over M = l + k + 1 moduli (Q, B and m_sk): one extension launch per distinct
+    input ciphertext, the forward transforms of the lifted polynomials (2M, or 4M, one handle each), one tensor launch
+    per block of 64 moduli, the inverse transforms of the tensor's 3M polynomials and one scaling launch"""
+    inputs = 2 if square else 4
+    return ((1 if square else 2) + ntt_handles(ntt, True, inputs * M) + -(-M // PARAM_BLOCK)
+            + ntt_handles(ntt, False, 3 * M) + 1)
+
+
+def hybrid_launches(call, n, level, K, alpha, basis, ntt, elts=1, keyed=None, rescale=False, kcc=2, tau=False,
+                    pairs=1, M=None, square=False):
+    """kernel launches of one ciphertext of `call` ("switch", "hoisted", "linear", "mul_relin", "mul_relin_sum",
+    "bfv_relin"): basis holds the moduli of B (level data, then K special); ntt(forward, units) is the launch count of
+    one multi-modulus transform of `units` polynomials.  "switch" and "hoisted" run `elts` switches over one mod-up;
+    "linear" takes `elts` elements, `keyed` of them with keys; "mul_relin_sum" sums `pairs` products; "bfv_relin" is
+    the BEHZ product over M moduli (square: ct1 = ct2), then the switch of d2 in coefficient form.  tau: BGV's
+    t-corrected mod-downs (rescale is then the merged modulus switch)."""
     total = 0
+    if call == "mul_relin_sum":
+        total += relin_sum_launches(level, pairs)
+        call = "mul_relin"
+    if call == "bfv_relin":
+        total += bfv_launches(M, square, ntt)
     if call == "hoisted":
         total += elts                                                      # one automorphism launch per element
     if call == "linear":
@@ -228,9 +370,30 @@ def hybrid_launches(call, n, level, K, alpha, basis, ntt, elts=1, keyed=None, re
             return len(weighted_mac_launches(D, keyed, largest))
         return elts * len(ks_mac_launches(D, largest))
 
-    total += hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs)
-    downs = 1 if call in ("linear", "mul_relin") else elts
-    return total + downs * hybrid_mod_down_launches(level, K, kcc if call == "switch" else 2, ntt, rescale)
+    coef = call == "bfv_relin"
+    total += hybrid_mod_up_launches(n, level, K, alpha, basis, ntt, macs, coef)
+    downs = 1 if call in ("linear", "mul_relin", "bfv_relin") else elts
+    return total + downs * hybrid_mod_down_launches(level, K, kcc if call == "switch" else 2, ntt, rescale, tau, coef)
+
+
+def bgv_mod_switch_rounds(n, rns, count):
+    """BgvModSwitch: polynomials per chunk, in both forms: the gathered last limbs plus one block of deltas of `chunk`
+    polynomials fit the budget"""
+    block = min(rns - 1, PARAM_BLOCK)
+    chunk = min(max(1, SCRATCH_BYTES // ((block + 1) * n * 8)), count)
+    return _split(count, chunk)
+
+
+def bgv_mod_switch_launches(n, rns, count, ntt_form, ntt):
+    """BgvModSwitch: per chunk, in NTT form the last limbs' inverse transform (cnt units); per block of 64 moduli the
+    t-corrected conversion from the one last limb, in NTT form the forward transform of delta (cm x cnt units), and the
+    finish"""
+    total = 0
+    for cnt in bgv_mod_switch_rounds(n, rns, count):
+        total += ntt(False, cnt) if ntt_form else 0
+        for cm in _split(rns - 1, PARAM_BLOCK):
+            total += len(base_conv_t_blocks(1, cm)) + (ntt(True, cm * cnt) if ntt_form else 0) + 1
+    return total
 
 
 def bsgs_rows(babies, giants, present):
@@ -304,3 +467,8 @@ BSGS_SPARSE = ((False, True, True, True, True, True), (False, True, True, True),
 BSGS_SWEEP = ((False, True, True), (False, True, True), {(0, 0), (0, 1), (1, 0), (1, 2), (2, 1)})
 BSGS_BENCH = ((False,) + (True,) * 7, (False,) + (True,) * 7, None)
 BSGS_BENCH_SHAPE = (16, 30, 10, 10, 50, 50, 30)   # (log2 n, L, K, alpha, data bits, special bits, level)
+# tests/test_gpu_evaluator_rounds.py: BEHZ with full tiles, (log2 n, l, k): M = l + k + 1 = 129 moduli, tensor blocks
+# 64 + 64 + 1; and one host-buffer batch at production size, (HYBRID_SHAPES name, level, batch): one ciphertext per
+# staging slot, so the slots wrap (3 + 1)
+BEHZ_TILES = (12, 64, 64)
+EVALUATOR_HOST_BATCH = ("budget_a2", 30, 4)

@@ -175,6 +175,180 @@ def test_every_level_sweep_crosses_each_block_boundary():
     assert len(plan.hybrid_mod_down_blocks(29, 10, True)[0]) == 2
 
 
+# ------------------------------------------------------------------------------ the evaluator calls
+def _recorder():
+    calls = []
+
+    def ntt(forward, units):
+        calls.append((forward, units))
+        return 1
+    return calls, ntt
+
+
+def test_evaluator_spot_values():
+    assert [plan.base_conv_t_targets(f) for f in (1, 2, 3, 4, 10, 11, 64)] == [67, 58, 51, 45, 27, 25, 3]
+    assert plan.base_conv_t_blocks(10, 30) == [27, 3] and plan.base_conv_t_blocks(11, 29) == [25, 4]
+    assert plan.hybrid_mod_down_blocks(30, 10, tau=True) == [[27, 3]]
+    assert plan.hybrid_mod_down_blocks(30, 10, True, tau=True) == [[25, 4]]
+    assert plan.bgv_mod_switch_rounds(1 << 16, 31, 35) == [16, 16, 3]
+    assert plan.bgv_mod_switch_rounds(1 << 14, 70, 33) == [31, 2]
+    assert plan.bgv_mod_switch_rounds(1 << 12, 6, 8) == [8]            # test_gpu_bgv.py's in-place counts: one chunk
+    # per chunk: the last limbs' inverse transform, then per block of moduli one conversion, a forward transform of
+    # delta and the finish; coefficient form: the conversion and the finish
+    calls, ntt = _recorder()
+    assert plan.bgv_mod_switch_launches(1 << 16, 31, 35, True, ntt) == 3 * (1 + 3)
+    assert calls == [(False, 16), (True, 30 * 16), (False, 16), (True, 30 * 16), (False, 3), (True, 30 * 3)]
+    assert plan.bgv_mod_switch_launches(1 << 16, 31, 35, False, _one) == 3 * 2
+    calls, ntt = _recorder()
+    assert plan.bgv_mod_switch_launches(1 << 14, 70, 33, True, ntt) == 2 * (1 + 2 * 3)
+    assert calls == [(False, 31), (True, 64 * 31), (True, 5 * 31), (False, 2), (True, 64 * 2), (True, 5 * 2)]
+    assert plan.bgv_mod_switch_launches(1 << 14, 70, 33, False, _one) == 2 * 2 * 2
+    assert [plan.relin_sum_launches(30, k) for k in (1, 2, 32, 33)] == [0, 1, 1, 2]
+    assert plan.relin_sum_launches(70, 65) == 2 * 3
+    # BEHZ: the transforms run one handle per polynomial, 64 handles a launch set
+    calls, ntt = _recorder()
+    assert plan.bfv_launches(62, False, ntt) == 2 + 4 + 1 + 3 + 1
+    assert calls == [(True, 64)] * 3 + [(True, 56)] + [(False, 64)] * 2 + [(False, 58)]
+    assert plan.bfv_launches(62, True, _one) == 1 + 2 + 1 + 3 + 1
+    assert plan.bfv_launches(129, False, _one) == 2 + 9 + 3 + 7 + 1
+    # the relinearized BFV call: no inverse transform of the target, the mod-down's per-block transform inverse
+    basis = [(1 << 45) + 1] * 8
+    calls, ntt = _recorder()
+    plan.hybrid_launches("bfv_relin", 1 << 12, 6, 2, 2, basis, ntt, M=13, square=True)
+    assert calls == [(True, 26), (False, 39),                  # BfvMultiply: 2M forward, 3M inverse
+                     (True, 24),                               # the mod-up's one round: 8 moduli x 3 digits
+                     (False, 4), (False, 12)]                  # the mod-down: K x 2, then 6 x 2 data limbs back
+    calls, ntt = _recorder()
+    plan.hybrid_launches("mul_relin_sum", 1 << 12, 6, 2, 2, basis, ntt, pairs=3)
+    assert calls == [(False, 6), (True, 24), (False, 4), (True, 12)]
+
+
+def test_t_blocks_of_every_hybrid_shape():
+    """the t-corrected mod-down's blocks at each HYBRID_SHAPES level, without and with the merged modulus switch: one
+    more source (6 + F words per target instead of 5 + F, 6 more for tau) than CKKS's rounded conversion"""
+    want = {("bench_rescale", 30): ([[27, 3]], [[25, 4]]),
+            ("budget_a2", 30): ([[27, 3]], [[25, 4]]), ("budget_a2", 29): ([[27, 2]], [[25, 3]]),
+            ("budget_a3", 30): ([[30]], [[29]]), ("budget_a3", 28): ([[28]], [[27]]),
+            ("mixed_chunks", 24): ([[24]], [[23]])}
+    got = {(name, level): (plan.hybrid_mod_down_blocks(level, K, tau=True),
+                           plan.hybrid_mod_down_blocks(level, K, True, tau=True))
+           for name, (_, _, K, _, _, _, levels) in plan.HYBRID_SHAPES.items() for level in levels}
+    assert got == want
+    # at K = 10 both differ from CKKS's 29 + 1 and 27 + 2
+    assert plan.hybrid_mod_down_blocks(30, 10) == [[29, 1]] and plan.hybrid_mod_down_blocks(30, 10, True) == [[27, 2]]
+
+
+def _earlier_relin(n, level, K, alpha, rescale, fwd, inv, t_sources=False):
+    """tests/test_gpu_mul_relin.py's relin_launches (and with t_sources tests/test_gpu_bgv.py's multiply count) below
+    2^60: the mod-up with one multiply-accumulate per round, and the mod-down from K + rescale special limbs"""
+    import hybrid_exact as hx
+
+    def targets(s):
+        return (474 - 4 * s) // (6 + s) if t_sources else (480 - 4 * s) // (5 + s)
+
+    groups, nb = hx.digits(level, alpha), level + K
+    ichunk = min(max(1, (256 << 20) // (len(groups) * n * 8)), nb, 64)
+    up = inv * -(-level // 64) + sum(sum(-(-min(ichunk, nb - b0) // ((480 - 4 * len(S)) // (5 + len(S))))
+                                         for S in groups) + fwd + 1 for b0 in range(0, nb, ichunk))
+    lv, k = level - int(rescale), K + int(rescale)
+    return up, inv + sum(-(-min(64, lv - i0) // targets(k)) + fwd + 1 for i0 in range(0, lv, 64))
+
+
+def test_evaluator_launches_agree_with_the_earlier_counts():
+    """below 2^60 the plan gives the counts the per-call GPU files derived on their own: test_gpu_mul_relin_sum.py's
+    sum_launches, test_gpu_bfv.py's bfv_launches and relinearized count, and test_gpu_bgv.py's switch, rotation,
+    multiply and modulus-switch counts, with transforms of different launch counts in each direction"""
+    fwd, inv = 2, 3
+
+    def ntt(forward, units):
+        return fwd if forward else inv
+
+    n = 1 << 12
+    for L, K, alpha, level in [(6, 2, 2, 6), (6, 2, 2, 5), (30, 10, 10, 30), (70, 2, 64, 70), (70, 2, 64, 65),
+                               (12, 1, 1, 12), (20, 2, 5, 12), (30, 1, 1, 30)]:
+        basis = [(1 << 45) + 1] * (level + K)
+        for rescale in (False, True):
+            up, down = _earlier_relin(n, level, K, alpha, rescale, fwd, inv)
+            for pairs in (1, 2, 33, 65):
+                extra = 0 if pairs == 1 else -(-level // 64) * -(-pairs // 32)
+                got = plan.hybrid_launches("mul_relin_sum", n, level, K, alpha, basis, ntt, rescale=rescale,
+                                           pairs=pairs)
+                assert got == up + down + extra, (L, K, alpha, level, rescale, pairs)
+            up, down = _earlier_relin(n, level, K, alpha, rescale, fwd, inv, t_sources=True)
+            assert plan.hybrid_launches("mul_relin", n, level, K, alpha, basis, ntt, rescale=rescale, tau=True) == \
+                up + down
+        up, down = _earlier_relin(n, level, K, alpha, False, fwd, inv, t_sources=True)
+        assert plan.hybrid_launches("switch", n, level, K, alpha, basis, ntt, tau=True) == up + down
+        up2 = up + sum(1 for _ in range(0, level + K, min(max(1, (256 << 20) // (-(-level // alpha) * n * 8)),
+                                                          level + K, 64)))   # a second multiply-accumulate per round
+        assert plan.hybrid_launches("hoisted", n, level, K, alpha, basis, ntt, elts=2, tau=True) == 2 + up2 + 2 * down
+        blocks = -(-(level - 1) // 64)
+        assert plan.bgv_mod_switch_launches(n, level, 2, True, ntt) == inv + blocks * (2 + fwd)
+        assert plan.bgv_mod_switch_launches(n, level, 2, False, ntt) == 2 * blocks
+        for k in (level, level + 1):
+            M = level + k + 1
+            for square in (False, True):
+                inputs = 2 if square else 4
+                bfv = (1 if square else 2) + fwd * -(-inputs * M // 64) + -(-M // 64) + inv * -(-3 * M // 64) + 1
+                assert plan.bfv_launches(M, square, ntt) == bfv
+                up, down = _earlier_relin(n, level, K, alpha, False, fwd, inv)
+                lb = -(-level // 64)
+                assert plan.hybrid_launches("bfv_relin", n, level, K, alpha, basis, ntt, M=M, square=square) == \
+                    bfv + up + down - inv * lb - fwd * lb + inv * lb
+
+
+def _divisible(units):
+    """the GPU tests measure a transform of `units` polynomials as c copies, c a divisor in [2, 64]"""
+    return any(max(units, 2) % d == 0 for d in range(2, 65))
+
+
+def test_evaluator_shapes_have_the_plan_their_names_claim(port):
+    import bfv_exact as bfx
+    import inner_sum_exact as ix
+    # BgvModSwitch: several chunks at both RESCALE_SHAPES, blocks_n14's each in two parameter blocks
+    for shape, (n, _, limbs, count) in plan.RESCALE_SHAPES.items():
+        assert _several_uneven(plan.bgv_mod_switch_rounds(n, limbs, count)), shape
+    assert plan.RESCALE_SHAPES["blocks_n14"][2] - 1 > plan.PARAM_BLOCK
+    # the sums: 33 pairs take two tensor-sum chunks, the second shorter; at g = 5 and k = 7, bit 1 has a keyed
+    # doubling and a keyed shift (one mod-up for both), and k = 16 doubles four times
+    assert _several_uneven(plan._split(33, plan.RELIN_SUM_PAIRS))
+    for logn in {v[0] for v in plan.HYBRID_SHAPES.values()}:
+        bits = ix.inner_sum_bits(5, 7, 1 << logn)
+        assert all(e not in (None, 1) for e in bits[1]), bits
+        assert [d is not None for d, _ in ix.inner_sum_bits(5, 16, 1 << logn)] == [True] * 4 + [False]
+    # BEHZ_TILES: 129 moduli, tensor blocks 64 + 64 + 1
+    logn, l, k = plan.BEHZ_TILES
+    assert l == k == plan.PARAM_BLOCK and _several_uneven(plan._split(l + k + 1, plan.PARAM_BLOCK))
+    # the host batch: one ciphertext per slot, the last slot of the wrap shorter
+    name, level, batch = plan.EVALUATOR_HOST_BATCH
+    assert level in plan.HYBRID_SHAPES[name][-1]
+    assert _several_uneven(plan._split(batch, plan.STAGING_SLOTS))
+    # every transform the plan asks of the new file has a unit count the GPU test can measure
+    units = []
+
+    def ntt(forward, u):
+        units.append(u)
+        return 1
+    for name in plan.HYBRID_SHAPES:
+        n, L, K, alpha, mods, levels = _hybrid_mods(port, name)
+        for level in levels:
+            basis = mods[:level] + mods[L:]
+            M = level + bfx.seal_base_b_size(mods[:level], 65537) + 1
+            for rs in (False, True):
+                plan.hybrid_launches("mul_relin_sum", n, level, K, alpha, basis, ntt, rescale=rs, pairs=33)
+                plan.hybrid_launches("mul_relin", n, level, K, alpha, basis, ntt, rescale=rs, tau=True)
+                for k in (7, 16):
+                    ix.inner_sum_launches(n, level, K, alpha, basis, ntt, 5, k, rs)
+            plan.hybrid_launches("hoisted", n, level, K, alpha, basis, ntt, elts=2, tau=True)
+            for square in (False, True):
+                plan.hybrid_launches("bfv_relin", n, level, K, alpha, basis, ntt, M=M, square=square)
+    for n, _, limbs, count in plan.RESCALE_SHAPES.values():
+        for form in (True, False):
+            plan.bgv_mod_switch_launches(n, limbs, count, form, ntt)
+    plan.hybrid_launches("bfv_relin", 1 << logn, l, 2, 32, [(1 << 57) + 1] * (l + 2), ntt, M=l + k + 1)
+    assert units and all(_divisible(u) for u in units), sorted(u for u in set(units) if not _divisible(u))
+
+
 # ------------------------------------------------------------------------------ LinearTransformHybridBSGS
 def _one(forward, units):
     return 1

@@ -17,6 +17,7 @@ import numpy as np
 import pytest
 
 import bgv_exact as bx
+import composite_plan as plan
 import hybrid_exact as hx
 from test_gpu_hybrid_key_switch import SENTINEL, _check, _levels, _ntt_launches, _primes, dev, host
 from test_gpu_hybrid_rotation import _mod_up_launches
@@ -375,15 +376,10 @@ def test_held_stream(hb, buffers_case, which):
 
 
 # ------------------------------------------------------------------------------------------------ launch counts
-def t_targets(sources):
-    """targets per t-corrected conversion launch (include/hexl_b200.h)"""
-    return (474 - 4 * sources) // (6 + sources)
-
-
 def bgv_mod_down_launches(level, K, fwd, inv):
     """the special limbs' inverse transform; per block of 64 data moduli the t-corrected conversions, a forward
-    transform and the finish"""
-    return inv + sum(-(-min(64, level - i0) // t_targets(K)) + fwd + 1 for i0 in range(0, level, 64))
+    transform and the finish (composite_plan's t-corrected mod-down, fwd and inv launches per transform)"""
+    return plan.hybrid_mod_down_launches(level, K, 2, lambda forward, units: fwd if forward else inv, tau=True)
 
 
 @pytest.mark.parametrize("L, K, alpha, level", [(6, 2, 2, 6), (30, 10, 10, 30), (70, 2, 64, 70), (70, 2, 64, 65),

@@ -125,7 +125,8 @@ def _ntt(hb, n):
         key = (n, forward, units)
         if key not in _NTT_LAUNCHES:
             u = max(units, 2)
-            c = next(d for d in range(2, 65) if u % d == 0)
+            c = next((d for d in range(2, 65) if u % d == 0), None)
+            assert c is not None, f"{units} units have no divisor in [2, 64] to measure them as c copies by"
             h = hb.GetNTT(n, hb.GeneratePrimes(1, 50, True, n)[0])
             x = torch.zeros(u * n, dtype=torch.int64, device="cuda")
             fn = hb.ComputeForwardMulti if forward else hb.ComputeInverseMulti
