@@ -151,6 +151,9 @@ _sig("hexl_b200_bgv_apply_galois_key_switch_hybrid_hoisted", _int,
      [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _vp, _vp, _u64, _u64, _vp])
 _sig("hexl_b200_bgv_multiply_relinearize_hybrid", _int,
      [_vp, _vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64, _vp, _int, _u64, _vp])
+_sig("hexl_b200_plain_lift", _int, [_vp, _vp, _u64, _u64, _vp, _u64, _u64, _u64, _int, _u64, _vp])
+_sig("hexl_b200_bfv_add_plain", _int, [_vp, _vp, _vp, _u64, _u64, _u64, _vp, _u64, _u64, _int, _u64, _vp])
+_sig("hexl_b200_bfv_multiply_plain", _int, [_vp, _vp, _vp, _u64, _u64, _int, _u64, _vp, _u64, _u64, _u64, _vp])
 
 #: every symbol include/hexl_b200.h declares (checked against the header by the tests)
 EXPORTED = sorted(n for n in dir(_lib) if n.startswith("hexl_b200_"))
@@ -850,6 +853,54 @@ def BfvMultiplyRelinearizeHybrid(result, ct1, ct2, n, level_size, q_size, p_size
                                                           plain_modulus,
                                                           relin_keys._h if relin_keys is not None else None, batch,
                                                           _stream(stream, rc or ac or bc)))
+    return result
+
+
+# ------------------------------------------------------------------ plaintexts of BFV and BGV
+def PlainLift(result, plain, plain_coeff_count, n, moduli, level_size, plain_modulus, correction_factor=1,
+              ntt_form=False, count=1, stream=None):
+    """Lift `count` plaintexts (plain_coeff_count words each, mod plain_modulus) into level_size limbs of n words each
+    (hexl_b200_plain_lift): m' = [m correction_factor]_t, limb i = [m' - t]_{q_i} if m' >= floor((t + 1) / 2) else
+    [m']_{q_i}; ntt_form=True then applies the forward transform.  Plaintext p is stored at result[p * level_size*n:]."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); pp, pn, pc = _buf(plain)
+    _need("moduli", mods.size, level_size)
+    _need("result", rn, count * level_size * n); _need("plain", pn, count * plain_coeff_count)
+    _check(_lib.hexl_b200_plain_lift(rp, pp, plain_coeff_count, n, mods.ctypes.data, level_size, plain_modulus,
+                                     correction_factor, int(bool(ntt_form)), count, _stream(stream, rc or pc)))
+    return result
+
+
+def BfvAddPlain(result, ct, plain, plain_coeff_count, n, moduli, level_size, plain_modulus, subtract=False,
+                plain_count=1, batch=1, stream=None):
+    """BFV add_plain / sub_plain (hexl_b200_bfv_add_plain): c0 of ciphertext c (ct[c * 2*level_size*n:], coefficient
+    form) +- round(Q m / t) over the first plain_coeff_count coefficients, stored at result[c * 2*level_size*n:].  One
+    plaintext for all ciphertexts (plain_count=1) or one each (plain_count=batch, at plain[c * plain_coeff_count:]).
+    result may be ct."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); cp, cn, cc = _buf(ct); pp, pn, pc = _buf(plain)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, level_size)
+    _need("result", rn, batch * per); _need("ct", cn, batch * per); _need("plain", pn, plain_count * plain_coeff_count)
+    _check(_lib.hexl_b200_bfv_add_plain(rp, cp, pp, plain_coeff_count, plain_count, n, mods.ctypes.data, level_size,
+                                        plain_modulus, int(bool(subtract)), batch, _stream(stream, rc or cc or pc)))
+    return result
+
+
+def BfvMultiplyPlain(result, ct, plain, plain_coeff_count, n, moduli, level_size, plain_modulus, plain_ntt_form=False,
+                     plain_count=1, batch=1, stream=None):
+    """BFV multiply_plain (hexl_b200_bfv_multiply_plain): ciphertext c (coefficient form) times the lifted plaintext,
+    negacyclic per limb, stored at result[c * 2*level_size*n:] in coefficient form.  plain_ntt_form=True takes
+    PlainLift(ntt_form=True) outputs (level_size*n words each) and ignores plain_coeff_count.  result may be ct."""
+    mods = np.ascontiguousarray(moduli, dtype=np.uint64)
+    rp, rn, rc = _buf(result); cp, cn, cc = _buf(ct); pp, pn, pc = _buf(plain)
+    per = 2 * level_size * n
+    _need("moduli", mods.size, level_size)
+    _need("result", rn, batch * per); _need("ct", cn, batch * per)
+    _need("plain", pn, plain_count * (level_size * n if plain_ntt_form else plain_coeff_count))
+    _check(_lib.hexl_b200_bfv_multiply_plain(rp, cp, pp, plain_coeff_count, plain_count, int(bool(plain_ntt_form)), n,
+                                             mods.ctypes.data, level_size, plain_modulus, batch,
+                                             _stream(stream, rc or cc or pc)))
     return result
 
 

@@ -24,7 +24,7 @@ LIB = os.path.join(LIB_DIR, "libhexl_b200.so")
 
 SOURCES = ["capi.cu", "capi_ntt.cu", "capi_eltwise.cu", "capi_keyswitch.cu", "capi_galois.cu", "capi_hybrid.cu",
            "ntt.cu", "ntt_multi.cu", "eltwise.cu", "seal.cu", "galois.cu", "rns.cu", "bfv.cu", "capi_bfv.cu",
-           "numtheory.cpp"]
+           "plain.cu", "capi_plain.cu", "numtheory.cpp"]
 HEADERS = ["capi.h", "internal.h", "modarith.cuh", "ntt_kernels.cuh", "galois.cuh", "hybrid_rotation.h", "numtheory.h",
            os.path.join(ROOT, "include", "hexl_b200.h")]
 

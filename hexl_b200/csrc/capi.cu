@@ -165,6 +165,83 @@ int debug_bounds(const u64* p, u64 n, u64 bound, const char* what, std::initiali
   return check_bounds(p, n, bound, pi, what, stream);
 }
 
+// ---------------------------------------------------------------- constant tables
+static std::mutex g_table_mu;
+static std::map<std::vector<uint64_t>, std::map<int, uint64_t*>> g_tables;
+
+int device_table(const std::vector<uint64_t>& tab, int dev, cudaStream_t user_stream, const uint64_t** out,
+                 const char* what) {
+  std::lock_guard<std::mutex> lk(g_table_mu);
+  auto& per_dev = g_tables[tab];
+  auto it = per_dev.find(dev);
+  if (it != per_dev.end()) {
+    *out = it->second;
+    return 0;
+  }
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (user_stream && cudaStreamIsCapturing(user_stream, &cap) != cudaSuccess) cudaGetLastError();
+  if (cap != cudaStreamCaptureStatusNone)
+    return fail(HEXL_B200_ERR_INVALID_ARG,
+                "%s for these moduli are not uploaded to this device yet and the stream is being captured: "
+                "run the call once before capturing",
+                what);
+  uint64_t* p = nullptr;
+  cudaStream_t s = nullptr;
+  CU(cudaMalloc(&p, tab.size() * sizeof(uint64_t)));
+  cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(p, tab.data(), tab.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);  // the copy has landed before any kernel can read the table
+  if (s) cudaStreamDestroy(s);
+  if (e != cudaSuccess) {
+    cudaFree(p);
+    return cuda_fail(e, what);
+  }
+  per_dev[dev] = p;
+  *out = p;
+  return 0;
+}
+
+// ---------------------------------------------------------------- multi-word integers
+void big_mul(Big& a, uint64_t x) {
+  unsigned __int128 carry = 0;
+  for (auto& w : a) {
+    carry += (unsigned __int128)w * x;
+    w = (uint64_t)carry;
+    carry >>= 64;
+  }
+  if (carry) a.push_back((uint64_t)carry);
+}
+void big_add_at(Big& a, size_t word, uint64_t x) {
+  if (a.size() <= word) a.resize(word + 1, 0);
+  for (size_t i = word; x; ++i) {
+    if (i == a.size()) a.push_back(0);
+    a[i] += x;
+    x = a[i] < x ? 1 : 0;
+  }
+}
+bool big_le(Big a, Big b) {
+  while (!a.empty() && a.back() == 0) a.pop_back();
+  while (!b.empty() && b.back() == 0) b.pop_back();
+  if (a.size() != b.size()) return a.size() < b.size();
+  for (size_t i = a.size(); i-- > 0;)
+    if (a[i] != b[i]) return a[i] < b[i];
+  return true;
+}
+uint64_t big_divmod(Big& a, uint64_t d) {
+  unsigned __int128 rem = 0;
+  for (size_t i = a.size(); i-- > 0;) {
+    const unsigned __int128 cur = (rem << 64) | a[i];
+    a[i] = (uint64_t)(cur / d);
+    rem = cur % d;
+  }
+  return (uint64_t)rem;
+}
+uint64_t big_mod(const Big& a, uint64_t m) {
+  unsigned __int128 rem = 0;
+  for (size_t i = a.size(); i-- > 0;) rem = ((rem << 64) | a[i]) % m;
+  return (uint64_t)rem;
+}
+
 // ---------------------------------------------------------------- scratch pool
 // Stream-ordered scratch memory for the composites, from a pool of our own per device
 // (release threshold = keep everything: a KeySwitch re-uses the same few buffers call

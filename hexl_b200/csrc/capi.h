@@ -1,6 +1,7 @@
 // What the host sources of the C ABI (include/hexl_b200.h) share: capi.cu (library state, staging, scratch pool),
 // capi_ntt.cu, capi_eltwise.cu, capi_keyswitch.cu (key switch, key handles, rescale), capi_galois.cu and
-// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations and multiplication with hybrid keys, CKKS and BGV).
+// capi_hybrid.cu (hybrid key switch, fast base conversion, rotations and multiplication with hybrid keys, CKKS and BGV),
+// capi_bfv.cu (BFV multiplication) and capi_plain.cu (the plaintext operands of BFV and BGV).
 // Host-side responsibilities, all one-off or O(1) per call:
 //   * argument validation mirroring the reference's HEXL_CHECKs,
 //   * NTT handle = (N, q, root) -> twiddle tables, built on the host exactly as
@@ -313,6 +314,20 @@ int check_limb_bounds(const u64* p, u64 polys, u64 limbs, u64 words, Bound&& bou
       if (int rc = check_bounds(p + (c * limbs + i) * words, words, bound(i), pi, what, stream)) return rc;
   return 0;
 }
+
+// A device copy of a constant table, one per table content and device, kept for the life of the process like the NTT
+// tables (capi.cu).  The cold path uploads synchronously on a private stream, so it is refused inside a capture of
+// user_stream; `what` names the table in that refusal.
+int device_table(const std::vector<uint64_t>& tab, int dev, cudaStream_t user_stream, const uint64_t** out,
+                 const char* what);
+
+// Little-endian multi-word integers (capi.cu), for the host-side constants of the BFV calls
+using Big = std::vector<uint64_t>;
+void big_mul(Big& a, uint64_t x);                    // a *= x
+void big_add_at(Big& a, size_t word, uint64_t x);    // a += x 2^(64 word)
+bool big_le(Big a, Big b);                           // a <= b
+uint64_t big_divmod(Big& a, uint64_t d);             // a = floor(a / d); returns the remainder (d >= 1)
+uint64_t big_mod(const Big& a, uint64_t m);          // a mod m (m >= 1)
 
 int scratch_pool(cudaMemPool_t* out);  // the library's pool on the current device
 

@@ -46,39 +46,6 @@ void push_twiddle(std::vector<uint64_t>& tab, uint64_t w, uint64_t m) {
   tab.insert(tab.end(), {t.w, t.wp});
 }
 
-// Little-endian multi-word integers, just enough for the bound
-using Big = std::vector<uint64_t>;
-void big_mul(Big& a, uint64_t x) {
-  unsigned __int128 carry = 0;
-  for (auto& w : a) {
-    carry += (unsigned __int128)w * x;
-    w = (uint64_t)carry;
-    carry >>= 64;
-  }
-  if (carry) a.push_back((uint64_t)carry);
-}
-void big_add_at(Big& a, size_t word, uint64_t x) {
-  if (a.size() <= word) a.resize(word + 1, 0);
-  for (size_t i = word; x; ++i) {
-    if (i == a.size()) a.push_back(0);
-    a[i] += x;
-    x = a[i] < x ? 1 : 0;
-  }
-}
-bool big_le(Big a, Big b) {
-  while (!a.empty() && a.back() == 0) a.pop_back();
-  while (!b.empty() && b.back() == 0) b.pop_back();
-  if (a.size() != b.size()) return a.size() < b.size();
-  for (size_t i = a.size(); i-- > 0;)
-    if (a[i] != b[i]) return a[i] < b[i];
-  return true;
-}
-
-// Device copies of the BEHZ tables, one per table content and device, kept for the life of the process like the NTT
-// tables.  The cold path uploads synchronously on a private stream, so it is refused inside a capture.
-std::mutex g_behz_mu;
-std::map<std::vector<uint64_t>, std::map<int, uint64_t*>> g_behz;
-
 }  // namespace
 
 bool behz_bound_holds(uint64_t n, uint64_t t, const uint64_t* q, uint64_t l, const uint64_t* b, uint64_t k,
@@ -187,42 +154,12 @@ int bfv_plan(BfvPlan* pl, uint64_t n, const uint64_t* moduli, uint64_t l, const 
   return 0;
 }
 
-static int behz_table(const std::vector<uint64_t>& tab, int dev, cudaStream_t user_stream, const uint64_t** out) {
-  std::lock_guard<std::mutex> lk(g_behz_mu);
-  auto& per_dev = g_behz[tab];
-  auto it = per_dev.find(dev);
-  if (it != per_dev.end()) {
-    *out = it->second;
-    return 0;
-  }
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (user_stream && cudaStreamIsCapturing(user_stream, &cap) != cudaSuccess) cudaGetLastError();
-  if (cap != cudaStreamCaptureStatusNone)
-    return fail(HEXL_B200_ERR_INVALID_ARG,
-                "BEHZ tables for these moduli are not uploaded to this device yet and the stream is being captured: "
-                "run the call once before capturing");
-  uint64_t* p = nullptr;
-  cudaStream_t s = nullptr;
-  CU(cudaMalloc(&p, tab.size() * sizeof(uint64_t)));
-  cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(p, tab.data(), tab.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);  // the copy has landed before any kernel can read the table
-  if (s) cudaStreamDestroy(s);
-  if (e != cudaSuccess) {
-    cudaFree(p);
-    return cuda_fail(e, "BEHZ table upload");
-  }
-  per_dev[dev] = p;
-  *out = p;
-  return 0;
-}
-
 int bfv_product_on_device(int dev, const BfvPlan& pl, const BfvOutputs& out, const uint64_t* ct1, const uint64_t* ct2,
                           cudaStream_t s) {
   const uint64_t n = pl.n, l = pl.l, k = pl.k, M = l + k + 1, comp = l * n, poly = M * n;
   const uint64_t *ext_tab = nullptr, *scale_tab = nullptr;
-  if (int rc = behz_table(pl.ext_tab, dev, s, &ext_tab)) return rc;
-  if (int rc = behz_table(pl.scale_tab, dev, s, &scale_tab)) return rc;
+  if (int rc = device_table(pl.ext_tab, dev, s, &ext_tab, "BEHZ tables")) return rc;
+  if (int rc = device_table(pl.scale_tab, dev, s, &scale_tab, "BEHZ tables")) return rc;
   const bool square = ct1 == ct2;
   const uint64_t inputs = square ? 2 : 4;
   Scratch ws(s);

@@ -230,6 +230,21 @@ struct BfvOutputs {
 cudaError_t launch_bfv_scale(const BfvOutputs& out, const u64* tensor, u64 d_poly, u64 n, u64 polys, u64 l, u64 k,
                              const u64* tab, cudaStream_t stream);
 
+// Plaintexts of BFV and BGV (plain.cu), coefficient form, every modulus below 2^61, t in [2, 2^61), l <= 64.
+// The lift of `count` plaintexts of pcc <= n words each (back to back) into l limbs of n words each:
+//   m' = [m cf]_t (cf_shoup = floor(cf 2^64 / t)),  limb i = m' >= ceil(t/2) ? [m' - t]_{q_i} : [m']_{q_i}
+struct PlainModuli {
+  u64 q[kParamBlock];
+  u64 mu[kParamBlock];  // floor(2^64 / q)
+};
+cudaError_t launch_plain_lift(u64* result, const u64* plain, u64 pcc, u64 n, u64 count, u64 l, u64 t, u64 cf,
+                              u64 cf_shoup, const PlainModuli& mods, cudaStream_t stream);
+// BFV add_plain / sub_plain on c0 of `batch` ciphertexts (2 l limbs of n words each): slots [0, cover) of c0 get
+// +- round(Q m / t) mod q_i; ciphertext c reads its plaintext at plain + c plain_stride.  result may be ct.  tab: the
+// device table capi_plain.cu builds (plain.cu states its layout).
+cudaError_t launch_bfv_add_plain(u64* result, const u64* ct, const u64* plain, u64 pcc, u64 plain_stride, u64 n,
+                                 u64 cover, u64 batch, u64 l, bool subtract, const u64* tab, cudaStream_t stream);
+
 // Galois automorphism sigma_g (galois.cu).  NTT form: `polys` polynomials of 2^log_n words, one launch, words move
 // unchanged (result[j] = operand[pi_g(j)]).  Coefficient form: limbs [i0, i0 + cnt) of `polys` polynomials of rns
 // limbs each, limb i0 + e under mods.q[e]; galois_inv = g^-1 mod 2n.  result and operand must not overlap.

@@ -924,6 +924,36 @@ inline void BgvMultiplyRelinearizeHybrid(uint64_t* result, const uint64_t* ct1, 
                                                                digit_size, moduli, plain_modulus, relin_keys.Handle(),
                                                                mod_switch ? 1 : 0, batch, stream));
 }
+
+// extension: the lift of `count` BFV / BGV plaintexts (plain_coeff_count words each, mod plain_modulus) into
+// level_size limbs of n words each, m' = [m correction_factor]_t centred into every q_i, then the forward transform
+// when ntt_form (hexl_b200_plain_lift; SEAL's transform_to_ntt_inplace(Plaintext&, parms_id) with ntt_form).
+inline void PlainLift(uint64_t* result, const uint64_t* plain, uint64_t plain_coeff_count, uint64_t n,
+                      const uint64_t* moduli, uint64_t level_size, uint64_t plain_modulus,
+                      uint64_t correction_factor = 1, bool ntt_form = false, uint64_t count = 1,
+                      void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_plain_lift(result, plain, plain_coeff_count, n, moduli, level_size, plain_modulus,
+                                          correction_factor, ntt_form ? 1 : 0, count, stream));
+}
+
+// extension: BFV add_plain (subtract: sub_plain) on `batch` coefficient-form ciphertexts, c0 +- round(Q m / t)
+// (hexl_b200_bfv_add_plain).  plain_count is 1 (one plaintext for every ciphertext) or batch.  result may be ct.
+inline void BfvAddPlain(uint64_t* result, const uint64_t* ct, const uint64_t* plain, uint64_t plain_coeff_count,
+                        uint64_t plain_count, uint64_t n, const uint64_t* moduli, uint64_t level_size,
+                        uint64_t plain_modulus, bool subtract = false, uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bfv_add_plain(result, ct, plain, plain_coeff_count, plain_count, n, moduli, level_size,
+                                             plain_modulus, subtract ? 1 : 0, batch, stream));
+}
+
+// extension: BFV multiply_plain on `batch` coefficient-form ciphertexts, INTT(NTT(ct_k) . NTT(lift(m))) per component
+// (hexl_b200_bfv_multiply_plain).  plain_ntt_form takes PlainLift(ntt_form = true) outputs.  result may be ct.
+inline void BfvMultiplyPlain(uint64_t* result, const uint64_t* ct, const uint64_t* plain, uint64_t plain_coeff_count,
+                             uint64_t plain_count, bool plain_ntt_form, uint64_t n, const uint64_t* moduli,
+                             uint64_t level_size, uint64_t plain_modulus, uint64_t batch = 1, void* stream = nullptr) {
+  b200_detail::Throw(hexl_b200_bfv_multiply_plain(result, ct, plain, plain_coeff_count, plain_count,
+                                                  plain_ntt_form ? 1 : 0, n, moduli, level_size, plain_modulus, batch,
+                                                  stream));
+}
 }  // namespace b200
 
 }  // namespace hexl

@@ -825,6 +825,83 @@ int hexl_b200_bgv_multiply_relinearize_hybrid(uint64_t* result, const uint64_t* 
                                               const hexl_b200_keys* relin_keys, int mod_switch, uint64_t batch,
                                               void* stream);
 
+/* The lift of BFV / BGV plaintexts into the RNS basis of a ciphertext (extension; SEAL's transform_to_ntt_inplace
+ * (Plaintext&, parms_id) and the lift inside BFV and BGV multiply_plain and BGV add_plain).  Plaintext p is
+ * plain_coeff_count = pcc words at plain + p*pcc, coefficients mod t = plain_modulus (SEAL's Plaintext buffer, its
+ * coeff_count(); the coefficients from pcc to n are zero), and its lift is STORED at result + p*l*n, l = level_size
+ * limbs of n words.  With c = correction_factor, per coefficient m and limb i:
+ *   m' = [m c]_t,   out_i = [m' - t]_{q_i} if m' >= floor((t + 1) / 2), else [m']_{q_i}
+ * (the centred lift of m'; c = 1 is no correction, BGV's add_plain passes its correction factor).  Exact for every order
+ * of t and the q_i (t may exceed some q_i).  ntt_form = 1 then applies the forward transform (hexl_b200_ntt_forward_multi,
+ * canonical output) to every limb: the plaintext operand of BGV's add_plain / multiply_plain and of
+ * hexl_b200_bfv_multiply_plain(plain_ntt_form = 1).  Moduli below 2^61 (NTT-friendly for n when ntt_form = 1), t in
+ * [2, 2^61), l in [1, 64].  count = 0 does nothing.  HEXL_B200_ERR_INVALID_ARG for a null pointer, n not a power of two
+ * in [2, 2^20], l outside [1, 64], t outside [2, 2^61), correction_factor outside [1, t), pcc outside [1, n], ntt_form
+ * other than 0 or 1, a modulus outside [2, 2^61) (or not NTT-friendly with ntt_form = 1), and result overlapping plain;
+ * plaintext words >= t under hexl_b200_set_debug(1).  On the device: one launch for all count plaintexts (a thread per
+ * coefficient slot looping over the limbs), then with ntt_form = 1 the forward transform of the count x l limbs
+ * (ceil(count l / 64) transform launches); no library scratch.  Device calls capture into a CUDA graph once the
+ * transforms are warm.  Host buffers: one plaintext per staging step, split by plaintext over the devices of
+ * hexl_b200_set_host_devices.  Not covered: in place (the lift grows each plaintext from pcc to l x n words), encoding
+ * (the caller's BatchEncoder produced the plaintext), CKKS plaintexts (already in RNS form). */
+int hexl_b200_plain_lift(uint64_t* result, const uint64_t* plain, uint64_t plain_coeff_count, uint64_t n,
+                         const uint64_t* moduli, uint64_t level_size, uint64_t plain_modulus,
+                         uint64_t correction_factor, int ntt_form, uint64_t count, void* stream);
+
+/* BFV add_plain / sub_plain (extension; SEAL's Evaluator::add_plain / sub_plain for BFV,
+ * multiply_add_plain_with_scaling_variant / multiply_sub_plain_with_scaling_variant): c0 +- round(Q m / t) for each of
+ * `batch` ciphertexts.  Q = q_0..q_{l-1} (moduli, l = level_size: the ciphertext's level), t = plain_modulus.
+ * Ciphertext c is two components of l limbs of n words at ct + c*2*l*n, COEFFICIENT form, canonical; its plaintext is
+ * plain_coeff_count = pcc words at plain (plain_count = 1: one plaintext for every ciphertext) or at plain + c*pcc
+ * (plain_count = batch), coefficients below t, the coefficients from pcc to n zero.  Per coefficient j < pcc and limb i,
+ * with r = Q mod t and h = floor((t + 1) / 2):
+ *   fix = floor((m_j r + h) / t),   s = [m_j [floor(Q/t)]_{q_i} + fix]_{q_i},   c0_i[j] = [c0_i[j] +- s]_{q_i}
+ * (- with subtract = 1); m floor(Q/t) + fix = floor((Q m + h) / t), so this is SEAL's formula bit for bit.  The result
+ * is STORED at result + c*2*l*n: result == ct (SEAL's in-place operation) changes only those pcc slots of c0; any other
+ * result gets c0 in full and a copy of c1.  A result overlapping ct without being equal to it is refused.  fix is
+ * computed without a 128-bit division: a Shoup quotient of m r by t, corrected by at most one, plus [rem + h >= t]
+ * (plain.cu states the proof).  Moduli below 2^61 (any, not only NTT-friendly), t in [2, 2^61), l in [1, 64].
+ * batch = 0 does nothing.  HEXL_B200_ERR_INVALID_ARG for a null pointer, n not a power of two in [2, 2^20], l outside
+ * [1, 64], t outside [2, 2^61), pcc outside [1, n], plain_count other than 1 or batch, subtract other than 0 or 1, a
+ * modulus outside [2, 2^61), result partly overlapping ct, and result overlapping plain; ciphertext words >= their
+ * modulus and plaintext words >= t under hexl_b200_set_debug(1).  On the device: one launch for the whole batch (a
+ * thread per coefficient slot, fix computed once and applied to the l limbs), plus one device-to-device copy of the c1
+ * components when result != ct.  The constants (per limb q_i, floor(2^64 / q_i), [floor(Q/t)]_{q_i} and its Shoup
+ * factor; r, floor(r 2^64 / t), h) live in a device table built and uploaded on first use per (Q, t) and device, so a
+ * device call captures into a CUDA graph once it has run once on that device.  No library scratch.  Host buffers: one
+ * ciphertext per staging step (in and out on the same stream), a broadcast plaintext uploaded once per device, split by
+ * ciphertext over the devices of hexl_b200_set_host_devices.  Not covered: NTT-form BFV ciphertexts (SEAL refuses them
+ * too), BGV and CKKS add_plain (hexl_b200_plain_lift with the correction factor, then hexl_b200_eltwise_add_mod_multi
+ * on c0; CKKS plaintexts are already RNS), and sums of several plaintexts in one pass. */
+int hexl_b200_bfv_add_plain(uint64_t* result, const uint64_t* ct, const uint64_t* plain, uint64_t plain_coeff_count,
+                            uint64_t plain_count, uint64_t n, const uint64_t* moduli, uint64_t level_size,
+                            uint64_t plain_modulus, int subtract, uint64_t batch, void* stream);
+
+/* BFV multiply_plain (extension; SEAL's Evaluator::multiply_plain for BFV, multiply_plain_normal): each of `batch`
+ * coefficient-form ciphertexts times a plaintext, the product in coefficient form.  Layouts, Q, t, pcc and plain_count
+ * as for hexl_b200_bfv_add_plain.  Per component k and limb i, negacyclic products mod q_i:
+ *   result_k,i = INTT(NTT(ct_k,i) . NTT(lift(m)_i)),   lift that of hexl_b200_plain_lift with correction factor 1,
+ * canonical.  plain_ntt_form = 1 takes plaintexts that hexl_b200_plain_lift(ntt_form = 1) produced instead: l x n words
+ * each at plain (+ c*l*n), canonical; pcc is then not read (a PIR server transforms its database once).  result may
+ * equal ct; partial overlap is refused.  Bit for bit the chain hexl_b200_plain_lift(ntt_form = 1);
+ * hexl_b200_ntt_forward_multi of ct; hexl_b200_eltwise_mult_mod_multi of each component by the lifted plaintext;
+ * hexl_b200_ntt_inverse_multi.  Moduli below 2^61 and NTT-friendly for n; otherwise the refusals of
+ * hexl_b200_bfv_add_plain (subtract aside) and plain_ntt_form other than 0 or 1; plaintext words (NTT form: >= q_i)
+ * refused under hexl_b200_set_debug(1) like the ciphertext's.  On the device: each coefficient-form plaintext is lifted
+ * and transformed once (one lift launch and ceil(l / 64) forward transform launches; once per call when broadcast);
+ * per ciphertext, one forward transform of its two components into result (ceil(2l / 64) launches) and one inverse
+ * transform per component that multiplies by the transformed plaintext on load (2 ceil(l / 64) launches): there is no
+ * separate product pass, and the product never makes a round trip through HBM.  Library scratch: l x n words (none with
+ * plain_ntt_form = 1).  Device calls capture into a CUDA graph once the transforms are warm.  Host buffers: one
+ * ciphertext per staging step; a broadcast plaintext is uploaded, lifted and transformed once per device.  Not covered:
+ * NTT-form BFV ciphertexts, plaintext-weighted sums sum_i pt_i . ct_i in one pass, SEAL's fast path for monomial
+ * plaintexts (the same result), and BGV (hexl_b200_plain_lift(ntt_form = 1), then hexl_b200_eltwise_mult_mod_multi on
+ * both components). */
+int hexl_b200_bfv_multiply_plain(uint64_t* result, const uint64_t* ct, const uint64_t* plain,
+                                 uint64_t plain_coeff_count, uint64_t plain_count, int plain_ntt_form, uint64_t n,
+                                 const uint64_t* moduli, uint64_t level_size, uint64_t plain_modulus, uint64_t batch,
+                                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif
